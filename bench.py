@@ -5,7 +5,7 @@ One "step" = one complete pass of the hot path over one batch: the infer branch 
 conditioner (start state, all sampler steps through DiffNet, denorm epilogue) for B utterances of T frames.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--config 1|2|3|4|sweep] [--precision fp16s|fp16x2|fp16x3|fp16|fp32]
-                  [--impl reference]
+                  [--impl reference] [--dump-outputs DIR]
 
 --config (BASELINE.json `configs`, default 2 = the configuration the metric is quoted on):
    1  DiffSpeech LJ   B=1  T=512   K=100  DDPM              (the reference's own CPU-runnable case)
@@ -13,13 +13,17 @@ conditioner (start state, all sampler steps through DiffNet, denorm epilogue) fo
    3  DiffSinger PopCS B=8 T=2048  K=1000 DDPM, beta <= 0.02, dilation cycle 4
    4  DiffSinger OpenCpop B=32 T=1024 PNDM (PLMS) interval 40 of K=1000 (25 steps, 26 evaluations), dilation cycle 4
    sweep  B in {1,4,16,64} x T in {256,1024,4096}, K in {25,100,1000} (K: 3 points at B=16,T=1024); one JSON line, points in "sweep"
-Every line carries `roofline` (the residual-stack kernel against the measured sustained tensor peak), `cpu_baseline` (the
+Every line carries `roofline` (the step kernel against the H100 SXM data-sheet dense FP16 peak), `cpu_baseline` (the
 reference's PyTorch-CPU algorithm = oracle port on this box's host cores; plus `eager_cuda`: the same port on the GPU through
 cuDNN / cuBLAS eager kernels, TF32 off and on) and `e2e` (through dsx_infer_host with pinned HOST buffers).
 
 N > 1 (torchrun, one rank per GPU): utterance-sharded, B per GPU fixed (weak scaling), ONE all-gather of the finished mels
 per step inside the timed region.  The strong-scaled BASELINE configs[3] (B=32 total, PLMS) is measured in the same run and
 reported under extra.strong_config4.  Prints ONE JSON line on rank 0.
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step returned -- the mel spectrograms
+[B * N, T, 80] of dsx_infer -- as DIR/mel.npy (float32).  Inputs, weights and noise seeds depend only on the arguments, so
+two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -36,10 +40,12 @@ import torch
 import torch.distributed as dist
 
 _JSON_OUT = sys.stdout
-# algorithmic FLOPs per mel frame (SURVEY.md 8d): whole DiffNet evaluation, conditioner projection hoisted
+# algorithmic FLOPs per mel frame: whole DiffNet evaluation, conditioner projection hoisted
 FLOP_PER_FRAME_EVAL = 21184512
 # the residual stack, per frame and layer: 2*(3*256*512 + 256*512)  (dilated conv + output projection, both halves)
 FLOP_PER_FRAME_LAYER = 2 * (3 * 256 * 512 + 256 * 512)
+# NVIDIA H100 SXM data sheet, dense FP16 tensor throughput (700 W board); a power-limited card runs below it
+H100_FP16_DENSE_TFLOPS = 989.0
 
 CONFIGS = {
     "1": dict(B=1, T=512, K=100, sampler="ddpm", T_sched=100, max_beta=0.06, cycle=1,
@@ -385,6 +391,7 @@ def timed_steps(arm, steps, warmup, world, dev, flush, gather_total=None, clocks
         cs.start()
     l0 = arm.s.info(arm.capi.INFO_KERNEL_LAUNCHES)
     times = []
+    mel = None
     for i in range(steps):
         flush.zero_()                                          # L2 flush between timed iterations
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -404,7 +411,7 @@ def timed_steps(arm, steps, warmup, world, dev, flush, gather_total=None, clocks
     if world > 1:
         dist.all_reduce(total_ms, op=dist.ReduceOp.MAX)
     assert torch.isfinite(mel).all()
-    return float(total_ms.item()), (l1 - l0), clk
+    return float(total_ms.item()), (l1 - l0), clk, mel
 
 
 def roofline_of(arm, prec, ms_per_step):
@@ -415,12 +422,7 @@ def roofline_of(arm, prec, ms_per_step):
     reported."""
     capi = arm.capi
     cfg, B, T = arm.cfg, arm.B, arm.T
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = peaks.get("bf16_tflops_sustained", 1400.0)
+    peak = H100_FP16_DENSE_TFLOPS
 
     def profile(fused):
         arm.s.set_option(capi.OPT_FUSED_HEAD, 1 if fused else 0)
@@ -434,25 +436,15 @@ def roofline_of(arm, prec, ms_per_step):
     ns_s, n_s, t_stack = profile(False)
     ns, n, t_eval = profile(True)
     stack_launches = arm.s.info(capi.INFO_STACK_KERNEL_LAUNCHES)
-    traffic, traffic_note = None, "not captured for this configuration"
-    try:     # dram__bytes_read.sum + dram__bytes_write.sum of one `ncu --set full` capture of this kernel, per launch
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r02_stack_traffic.json")))
-        if cfg is CONFIGS["2"] and prec in tj:
-            traffic = tj[prec]["dram_bytes_read"] + tj[prec]["dram_bytes_write"]
-            traffic_note = tj.get("note", "static: from the committed ncu capture of this command (profiles/), not re-measured by this run")
-    except Exception:
-        pass
     flops_stack = FLOP_PER_FRAME_LAYER * B * T * 20
     flops_eval = FLOP_PER_FRAME_EVAL * B * T
-    fused = bool(stack_launches) and arm.s.info(capi.INFO_KERNEL_LAUNCHES) > 0
-    kernel = ("k_tc_stack (dsx_stack.cu, tcgen05): the whole diffusion step in one launch -- residual stack with x in registers / y in shared "
-              "memory, deferred skip GEMM, head projections, sampler update, next input projection") if stack_launches else \
-        "k_tc_layer (dsx_tc.cu: round-1 residual-stack kernel)"
+    kernel = ("k_hp_step (dsx_hopper.cu, wgmma): the whole diffusion step in one cooperative launch -- residual stack, head "
+              "projections, sampler update, next input projection") if stack_launches else \
+        "k_hp_step (dsx_hopper.cu, wgmma): residual layers of one evaluation in one cooperative launch"
     ach = flops_eval / t_eval / 1e12
     whole = FLOP_PER_FRAME_EVAL * B * T * n_evals(cfg) / (ms_per_step * 1e-3) / 1e12
     return {"bound": "tensor", "kernel": kernel, "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
-            "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1.4 PFLOP/s sustained",
-            "traffic": traffic, "traffic_note": traffic_note,
+            "peak_source": "NVIDIA H100 SXM data sheet, dense FP16 (not a measured peak)",
             "flops_per_launch": flops_eval, "avg_launch_us": t_eval * 1e6, "evaluations_profiled": n,
             "kernel_share_of_step": ns * 1e-6 / ms_per_step, "mma_passes": PASSES.get(prec),
             "stack_only": {"note": "head as a separate kernel (DSX_OPT_FUSED_HEAD = 0): the 20 residual layers + skip GEMM alone",
@@ -492,8 +484,11 @@ def e2e_of(dsx, cfg, prec, dev, rank, world, steps):
 def bench_config(dsx, cfg, prec, args, dev, rank, world, local_rank, flush, full=True):
     arm = Arm(dsx, cfg, prec, dev, rank)
     B, T = arm.B, arm.T
-    total_ms, launches, clk = timed_steps(arm, args.steps, args.warmup, world, dev, flush, gather_total=B * world,
-                                          clocks_index=local_rank)
+    total_ms, launches, clk, mel = timed_steps(arm, args.steps, args.warmup, world, dev, flush, gather_total=B * world,
+                                               clocks_index=local_rank)
+    if full and args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "mel.npy"), mel.float().cpu().numpy())
     ms = total_ms / args.steps
     out = {"value": world * B * T / (ms * 1e-3), "ms_per_step": ms, "launches": int(launches), "clocks": clk,
            "roofline": roofline_of(arm, prec, ms) if prec != "fp32" else None,
@@ -516,6 +511,8 @@ def main():
     ap.add_argument("--cpu-evals", type=int, default=3)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's output (mel.npy, float32) to DIR")
     args = ap.parse_args()
 
     # stdout carries exactly ONE JSON line: everything libraries print there (NCCL's version banner, ...) goes to stderr
@@ -542,7 +539,7 @@ def main():
     import diffsinger_b200 as dsx
 
     prec = args.precision
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)       # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)       # several times the 50 MB L2
     main_res = bench_config(dsx, cfg, prec, args, dev, rank, world, local_rank, flush)
     B, T, K = cfg["B"], cfg["T"], cfg["K"]
 
@@ -552,14 +549,14 @@ def main():
             if other == prec:
                 continue
             arm = Arm(dsx, cfg, other, dev, rank)
-            tms, _, _ = timed_steps(arm, 2, 2, world, dev, flush)
+            tms, _, _, _ = timed_steps(arm, 2, 2, world, dev, flush)
             arm.close()
             extra[other] = {"value": B * T / (tms / 2 * 1e-3), "unit": "frames/s", "ms_per_step": tms / 2, "note": NOTES[other]}
     if not args.no_extra and world > 1 and 32 % world == 0:
         # BASELINE configs[3] strong-scaled: B = 32 utterances in total, 32 / N per GPU, one all-gather per step
         c4 = CONFIGS["4"]
         arm = Arm(dsx, c4, prec, dev, rank, B=32 // world)
-        tms, _, _ = timed_steps(arm, 2, 2, world, dev, flush, gather_total=32)
+        tms, _, _, _ = timed_steps(arm, 2, 2, world, dev, flush, gather_total=32)
         arm.close()
         extra["strong_config4"] = {"value": 32 * c4["T"] / (tms / 2 * 1e-3), "unit": "frames/s", "ms_per_step": tms / 2, "scaling": "strong",
                                    "workload": c4["name"], "B_total": 32, "B_per_gpu": 32 // world,

@@ -1,4 +1,4 @@
-"""diffsinger_b200 -- B200-native (sm_100a) reverse-diffusion sampler for DiffSinger / DiffSpeech.
+"""diffsinger_b200 -- H100-native (sm_90a) reverse-diffusion sampler for DiffSinger / DiffSpeech.
 
 The compute lives in ``lib/libdsx.so`` (hand-written CUDA behind the C ABI of ``include/dsx.h``);
 this package is the thin host side that mirrors the reference's ``DiffNet`` / ``GaussianDiffusion``

@@ -48,7 +48,7 @@ class DiffNetParams(ctypes.Structure):
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"dsx CUDA library not found at {LIB_PATH}; build it with `python diffsinger_b200/build.py` "
-        "(nvcc, sm_100a).  There is no CPU fallback.")
+        "(nvcc, sm_90a).  There is no CPU fallback.")
 lib = ctypes.CDLL(LIB_PATH)
 
 _i, _i64, _u64, _vp = ctypes.c_int, ctypes.c_int64, ctypes.c_uint64, ctypes.c_void_p

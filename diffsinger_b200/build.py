@@ -1,4 +1,4 @@
-"""Builds the C-ABI CUDA library in-tree (diffsinger_b200/lib/libdsx.so) with nvcc for sm_100a.
+"""Builds the C-ABI CUDA library in-tree (diffsinger_b200/lib/libdsx.so) with nvcc for sm_90a (H100).
 
     python diffsinger_b200/build.py            # incremental (skips when sources are older than the .so)
     python diffsinger_b200/build.py --force
@@ -8,11 +8,11 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = [os.path.join(HERE, "csrc", f) for f in ("dsx_api.cu", "dsx_simt.cu", "dsx_tc.cu", "dsx_stack.cu", "dsx_selftest.cu")]
-HDR = [os.path.join(HERE, "csrc", f) for f in ("dsx_internal.h", "dsx_ptx.cuh", "dsx_rng.cuh", "dsx_tc_common.cuh")] + \
+SRC = [os.path.join(HERE, "csrc", f) for f in ("dsx_api.cu", "dsx_simt.cu", "dsx_hopper.cu")]
+HDR = [os.path.join(HERE, "csrc", f) for f in ("dsx_internal.h", "dsx_ptx.cuh", "dsx_rng.cuh")] + \
       [os.path.join(os.path.dirname(HERE), "include", "dsx.h")]
 LIB = os.path.join(HERE, "lib", "libdsx.so")
-NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_100a,code=sm_100a",
+NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

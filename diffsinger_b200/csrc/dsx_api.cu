@@ -35,14 +35,14 @@ int dev_alloc(dsx_handle* h, void** p, size_t bytes, bool model_owned) {
 }
 
 static void free_ws(Workspace& w) {
-  void* ptrs[] = {w.X, w.SKIP, w.CONDF, w.G1, w.Zf, w.Y, w.CONDH, w.CP, w.S16, w.Z, w.DTAB, w.EMB, w.TVALS, w.EPS, w.XTMP, w.XSTATE};
+  void* ptrs[] = {w.X, w.SKIP, w.CONDF, w.G1, w.Zf, w.Y, w.CONDH, w.CP, w.S16, w.DTAB, w.EMB, w.TVALS, w.EPS, w.XTMP, w.XSTATE};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   w = Workspace();
 }
 
 // Grow-only workspace: every buffer keeps its byte capacity; a call with a new (B, T) that fits re-uses the allocations
-// (only the tensor maps are re-encoded, see tc_prepare_maps), so utterance lengths that change from call to call cost no
+// (only the geometry changes), so utterance lengths that change from call to call cost no
 // cudaFree / cudaMalloc (cudaFree synchronises the device).  New allocations are zeroed on the caller's stream.
 int ensure_workspace(dsx_handle* h, const Geom& g, int rows, cudaStream_t s) {
   Workspace& w = h->ws;
@@ -72,8 +72,7 @@ int ensure_workspace(dsx_handle* h, const Geom& g, int rows, cudaStream_t s) {
     NEED(Y, nf * m.C * 2 * 4);
     NEED(CONDH, nf * m.H * 2 * 2);
     NEED(S16, nf * m.C * 2 * 2);
-    NEED(Z, static_cast<size_t>(m.L) * nf * m.C * 2);
-    NEED(CP, static_cast<size_t>(m.L) * g.tiles * 2 * 256 * kTile * 4);
+    NEED(CP, static_cast<size_t>(m.L) * nf * 2 * m.C * 4);
     if (cond_before[0] != w.CONDH || cond_before[1] != w.CP) h->cond_ready = false;
   } else {
     const void* cond_before = w.CONDF;
@@ -105,21 +104,10 @@ int check_status(dsx_handle* h, cudaStream_t s, const char* what) {
   if (*h->status_host != 0) {
     int code = *h->status_host;
     cudaMemsetAsync(h->status_dev, 0, sizeof(int), s);
-    // the tiles of the aborted launch stopped at different layers: their publish counters are no longer in lockstep.
-    // Zero them and forget the geometry so the next stack launch starts from a clean state (the handle stays usable).
-    reset_flags(h);
-    set_error("%s: in-kernel watchdog tripped (code %d: 1xx producer, 2xx MMA issuer, 3xx epilogue wait)", what, code);
+    set_error("%s: in-kernel self-check tripped (code %d)", what, code);
     return DSX_E_KERNEL;
   }
   return DSX_OK;
-}
-
-void reset_flags(dsx_handle* h) {
-  if (h->flags_dev) cudaMemset(h->flags_dev, 0, static_cast<size_t>(h->flags_cap) * sizeof(unsigned int));
-  h->flag_count = 0;
-  h->flags_geom_b = 0;
-  h->flags_geom_t = 0;
-  h->flags_kind = 0;
 }
 
 // Residual layers [0, nl) of one evaluation; `head` (may be null): what follows them in the step.  Returns through
@@ -192,7 +180,6 @@ static int prepare(dsx_handle* h, const float* cond, dsx_strides cs, int B, int 
   DSX_CUDA(cudaSetDevice(h->device));
   g.set(B, T);
   DSX_TRY(ensure_workspace(h, g, rows, s));
-  if (h->precision != DSX_PREC_FP32_SIMT) DSX_TRY(tc_prepare_maps(h, g));
   if (!cond) {
     DSX_CHECK(h->cond_ready && h->cond_geom.B == B && h->cond_geom.T == T, DSX_E_STATE,
               "cond == NULL needs a conditioner set for the same (B, T) by dsx_set_cond or an earlier call (have %s %dx%d, asked %dx%d)",
@@ -400,11 +387,8 @@ int dsx_create(int device, dsx_handle** out) {
   dsx_handle* h = new dsx_handle();
   h->device = device;
   h->sm_count = prop.multiProcessorCount;
-  h->tc_group = 2;
-  if (prop.major != 10) {
-    // the tcgen05 kernels are sm_100a-only; other devices can still run the fp32 path
-    h->tc_group = 0;
-  }
+  // the tensor-core kernels are built for sm_90a (wgmma) only; other devices can still run the fp32 path
+  h->tc_group = (prop.major == 9 && prop.minor == 0) ? 2 : 0;
   if (cudaMalloc(&h->status_dev, sizeof(int)) != cudaSuccess ||
       cudaMallocHost(&h->status_host, sizeof(int)) != cudaSuccess) {
     set_error("status word allocation failed");
@@ -432,9 +416,6 @@ void dsx_destroy(dsx_handle* h) {
   for (cudaEvent_t e : h->prof_events) cudaEventDestroy(e);
   for (void* p : h->stage)
     if (p) cudaFree(p);
-  if (h->trace_dev) cudaFree(h->trace_dev);
-  if (h->flags_dev) cudaFree(h->flags_dev);
-  if (h->ll_dev) cudaFree(h->ll_dev);
   if (h->status_dev) cudaFree(h->status_dev);
   if (h->status_host) cudaFreeHost(h->status_host);
   delete h;
@@ -454,15 +435,14 @@ int dsx_load_diffnet(dsx_handle* h, const dsx_diffnet_params* p, int M, int C, i
   free_ws(h->ws);
   h->ws_epoch++;
   h->cond_ready = false;
-  h->tm_geom = Geom();
   memset(&h->m, 0, sizeof(h->m));
   h->m.M = M; h->m.C = C; h->m.H = H; h->m.L = L; h->m.cycle = dilation_cycle;
   h->precision = precision;
   if (precision != DSX_PREC_FP32_SIMT) {
-    DSX_CHECK(h->tc_group != 0, DSX_E_INVALID, "tcgen05 precisions need an sm_100 device");
-    DSX_CHECK(tc_supported(h), DSX_E_INVALID, "tcgen05 path needs residual_channels == hidden_size == 256");
+    DSX_CHECK(h->tc_group != 0, DSX_E_INVALID, "tensor-core precisions need an sm_90 (H100) device");
+    DSX_CHECK(tc_supported(h), DSX_E_INVALID, "tensor-core path needs residual_channels == hidden_size == 256");
     DSX_CHECK(dilation_cycle <= 4, DSX_E_INVALID,
-              "tcgen05 path supports dilations up to 8 (dilation_cycle_length <= 4, got %d); use DSX_PREC_FP32_SIMT", dilation_cycle);
+              "tensor-core path supports dilations up to 8 (dilation_cycle_length <= 4, got %d); use DSX_PREC_FP32_SIMT", dilation_cycle);
   }
   DSX_TRY(simt_pack_model(h, p, s));
   if (precision != DSX_PREC_FP32_SIMT) DSX_TRY(tc_pack_model(h, s));
@@ -488,7 +468,6 @@ int dsx_diffnet_forward(dsx_handle* h, const float* x, dsx_strides xs, const int
   Geom g;
   DSX_TRY(prepare(h, cond, cs, B, T, B, g, s));
   DSX_TRY(launch_embed_table(h, t, B, s));
-  h->want_taps = 1;                      // dsx_debug_read may follow
   DSX_TRY(run_eval(h, x, xs, g, 0, 1, eps, s));
   return check_status(h, s, "dsx_diffnet_forward");
 }
@@ -535,7 +514,6 @@ int dsx_sample_ddpm(dsx_handle* h, float* x_inout, const float* cond, dsx_stride
             "steps t_start=%d n_steps=%d outside schedule of %d", t_start, n_steps, h->sched_T);
   Geom g;
   DSX_TRY(prepare(h, cond, cs, B, T, n_steps + 1, g, s));
-  h->want_taps = 0;
   DSX_TRY(sample_ddpm_impl(h, x_inout, g, t_start, n_steps, noise, seed, s));
   return check_status(h, s, "dsx_sample_ddpm");
 }
@@ -549,7 +527,6 @@ int dsx_sample_plms(dsx_handle* h, float* x_inout, const float* cond, dsx_stride
   Geom g;
   const int rows = (t_start + interval - 1) / interval + 2;
   DSX_TRY(prepare(h, cond, cs, B, T, rows, g, s));
-  h->want_taps = 0;
   DSX_TRY(sample_plms_impl(h, x_inout, g, t_start, interval, s));
   return check_status(h, s, "dsx_sample_plms");
 }
@@ -566,7 +543,6 @@ int dsx_infer(dsx_handle* h, const float* cond, dsx_strides cs, const float* fs2
   Geom g;
   const int rows = pndm_interval > 0 ? (K_step + pndm_interval - 1) / pndm_interval + 2 : K_step + 1;
   DSX_TRY(prepare(h, cond, cs, B, T, rows, g, s));
-  h->want_taps = 0;
   const int M = h->m.M;
   const size_t mel = static_cast<size_t>(B) * M * T;
   float* x = h->ws.XSTATE;   // x_t, [B,1,M,T]
@@ -651,7 +627,7 @@ int dsx_get_info(dsx_handle* h, int what, int64_t* out) {
     case DSX_INFO_TC_CTA_GROUP: *out = h->tc_group; break;
     case DSX_INFO_LAYER_KERNEL_LAUNCHES: *out = static_cast<int64_t>(h->prof_used / 2); break;
     case DSX_INFO_STACK_MODE: *out = h->stack_mode; break;
-    case DSX_INFO_CLUSTER_OCCUPANCY: *out = h->cluster_occ; break;
+    case DSX_INFO_CLUSTER_OCCUPANCY: *out = h->step_occ[1] > 0 ? h->step_occ[1] : 0; break;
     case DSX_INFO_STACK_KERNEL_LAUNCHES: *out = h->stack_launches; break;
     case DSX_INFO_STACK_ROWS: *out = h->stack_rows_used; break;
     case DSX_INFO_LAYER_KERNEL_NS: {
@@ -674,11 +650,10 @@ int dsx_set_option(dsx_handle* h, int what, int64_t value) {
   DSX_CHECK(h, DSX_E_INVALID, "null handle");
   switch (what) {
     case DSX_OPT_TC_CTA_GROUP:
-      DSX_CHECK(value == 2, DSX_E_INVALID, "the residual-layer kernel is cta_group::2 only (cta_group::1 is exercised by dsx_selftest)");
-      DSX_CHECK(h->tc_group != 0, DSX_E_INVALID, "no tcgen05 on this device");
-      h->tc_group = static_cast<int>(value);
+      DSX_CHECK(value == 2, DSX_E_INVALID, "DSX_OPT_TC_CTA_GROUP only accepts 2 (kept for ABI compatibility)");
+      DSX_CHECK(h->tc_group != 0, DSX_E_INVALID, "no tensor-core path on this device");
       break;
-    case DSX_OPT_CP_PREFETCH: h->cp_prefetch = static_cast<int>(value); break;
+    case DSX_OPT_CP_PREFETCH: break;   // no prefetch stage to tune in the sm_90 kernels; results never depended on it
     case DSX_OPT_STACK_MODE: h->stack_mode = static_cast<int>(value); break;
     case DSX_OPT_STACK_KERNEL: h->stack_kernel = static_cast<int>(value); break;
     case DSX_OPT_GATE_APPROX: h->gate_approx = static_cast<int>(value); break;
@@ -715,23 +690,10 @@ int dsx_debug_read(dsx_handle* h, int which, float* out, int B, int T, void* str
   return DSX_OK;
 }
 
-int dsx_debug_trace(dsx_handle* h, int enable, int64_t* out_host) {
+int dsx_debug_trace(dsx_handle* h, int, int64_t*) {
   DSX_CHECK(h, DSX_E_INVALID, "null handle");
-  DSX_CUDA(cudaSetDevice(h->device));
-  const size_t bytes = 10 * 256 * sizeof(long long);       // [2][3][256] role stamps, then [256][4] per-CTA entry / exit
-  if (out_host && h->trace_dev) {
-    DSX_CUDA(cudaDeviceSynchronize());
-    DSX_CUDA(cudaMemcpy(out_host, h->trace_dev, (enable == 2 ? 10 : 6) * 256 * sizeof(long long), cudaMemcpyDeviceToHost));
-  }
-  if (enable && !h->trace_dev) {
-    DSX_CUDA(cudaMalloc(&h->trace_dev, bytes));
-    DSX_CUDA(cudaMemset(h->trace_dev, 0, bytes));
-  } else if (!enable && h->trace_dev) {
-    DSX_CUDA(cudaDeviceSynchronize());
-    cudaFree(h->trace_dev);
-    h->trace_dev = nullptr;
-  }
-  return DSX_OK;
+  set_error("the sm_90 kernels record no clock64 timeline");
+  return DSX_E_INVALID;
 }
 
 int dsx_debug_set_layer_limit(dsx_handle* h, int n_layers) {

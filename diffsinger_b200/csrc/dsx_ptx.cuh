@@ -1,375 +1,65 @@
-// sm_100a PTX wrappers used by the dsx kernels: mbarrier, TMA (cp.async.bulk.tensor), tcgen05
-// (alloc / mma / commit / ld), cluster helpers, and the in-kernel watchdog.
-//
-// Everything here is written against the PTX ISA 8.7 forms that nvcc 12.9 accepts for
-// sm_100a; SASS evidence: tcgen05.mma -> UTCHMMA, tcgen05.ld -> LDTM, TMA -> UTMALDG.
+// sm_90a PTX wrappers used by the tensor-core kernels (dsx_hopper.cu): warpgroup MMA (wgmma) with shared-memory
+// descriptors, cp.async copies into the 128-byte-swizzled operand layout, and the gate math of the epilogues.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
 
 namespace dsx {
 
-// ------------------------------------------------------------------------------------------
-// watchdog: every spin-wait in the kernels is bounded.  On expiry the waiter records a code
-// in a global status word and the whole CTA drains (waits return false from then on), so a
-// protocol bug shows up as DSX_E_KERNEL on the host instead of a hung GPU.
-// ------------------------------------------------------------------------------------------
-struct Watchdog {
-  int* status;            // global int, 0 = ok
-  unsigned long long deadline_ns;
-};
-
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-__device__ __forceinline__ uint32_t lane_id() {
-  uint32_t l;
-  asm volatile("mov.u32 %0, %laneid;" : "=r"(l));
-  return l;
+// ---- operand layout --------------------------------------------------------------------------
+// K-major operand tile, 128-byte swizzle: rows of 64 fp16 (128 B), 8-row swizzle atoms 1024 B apart.  The 16-byte chunk c
+// of row r lives at r * 128 + ((c ^ (r & 7)) << 4); tiles start on 1024-byte boundaries.
+__device__ __forceinline__ uint32_t sw128(int r, int c) { return static_cast<uint32_t>(r * 128 + ((c ^ (r & 7)) << 4)); }
+
+// wgmma shared-memory matrix descriptor (sm_90): start >> 4 in bits [0,14), leading byte offset >> 4 in [16,30) (unused by
+// swizzled K-major layouts, 1 by convention), stride byte offset >> 4 in [32,46) = 1024 B between 8-row atoms, swizzle mode
+// in [62,64) with 1 = 128-byte swizzle.  Advancing K by 16 fp16 inside the 128-byte row is +32 bytes = +2 on the descriptor.
+__device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr) {
+  return static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4) | (static_cast<uint64_t>(1) << 16) |
+         (static_cast<uint64_t>(1024 >> 4) << 32) | (static_cast<uint64_t>(1) << 62);
 }
 
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// generic-proxy writes to shared memory (st.shared, cp.async) -> visible to the async proxy that wgmma reads through
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// D[64 x 128] (+)= A[64 x 16] . B[128 x 16]^T, fp16 operands from shared memory (both K-major), fp32 accumulators in
+// registers.  Thread t of the warpgroup holds d[4 i + j] = D[16 (t / 32) + (t % 32) / 4 + 8 (j / 2)][8 i + 2 (t % 4) + j % 2].
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db, int accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-
-// ---- cluster ---------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_arrive() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void cluster_wait() {
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cta address -> shared::cluster address of the same offset in CTA `rank`
-__device__ __forceinline__ uint32_t mapa(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-
-// ---- mbarrier --------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void fence_mbar_init() {
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-               : "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `rank` of the cluster (rank may be self)
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  uint32_t a = mapa(smem_u32(bar), rank);
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(a) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// default-semantics (release.cta) arrive on a barrier of another CTA of the cluster: enough for TMEM / shared
-// memory hand-offs inside a CTA pair (what CUTLASS's ClusterBarrier::arrive(cta_id) emits)
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-  uint32_t a = mapa(smem_u32(bar), rank);
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(a) : "memory");
-}
-// Bounded wait.  Returns false if the watchdog expired (caller should bail out).
-template <bool CLUSTER = false>
-__device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, const Watchdog& wd, int code) {
-  auto probe = [&]() { return CLUSTER ? mbar_try_wait_cluster(bar, parity) : mbar_try_wait(bar, parity); };
-  if (probe()) return true;
-  uint32_t spins = 0;
-  while (true) {
-    if (probe()) return true;
-    if (((++spins) & 0x3ff) == 0) {
-      if (*(volatile int*)wd.status != 0) return false;
-      if (globaltimer_ns() > wd.deadline_ns) {
-        atomicCAS(wd.status, 0, code);
-        return false;
-      }
-    }
-  }
-}
-
-// ---- proxy / tcgen05 fences -------------------------------------------------------------
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_all() {
-  asm volatile("fence.proxy.async;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// ---- TMA ------------------------------------------------------------------------------
-__device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
-}
-// G = cta_group.  For G == 2 the mbarrier is the one at the same offset in the pair's leader CTA
-// (cluster rank `lead`, the even rank of the pair).
-template <int G>
-__device__ __forceinline__ void tma_load_2d(const void* tmap, uint64_t* bar, void* dst, int c0, int c1,
-                                            uint32_t lead = 0) {
-  if constexpr (G == 1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-  } else {
-    uint32_t lead_bar = mapa(smem_u32(bar), lead);
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-        "%4}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(lead_bar), "r"(c0), "r"(c1)
-        : "memory");
-  }
-}
-template <int G>
-__device__ __forceinline__ void tma_load_3d(const void* tmap, uint64_t* bar, void* dst, int c0, int c1, int c2,
-                                            uint32_t lead = 0) {
-  if constexpr (G == 1) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], "
-        "[%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-  } else {
-    uint32_t lead_bar = mapa(smem_u32(bar), lead);
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-        "%4, %5}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(lead_bar), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-  }
-}
-
-// TMA store of one box shared::cta -> global (bulk async-group completion)
-__device__ __forceinline__ void tma_store_3d(const void* tmap, const void* src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_3d_hint(const void* tmap, const void* src, int c0, int c1, int c2, uint64_t policy) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4}], [%1], %5;"
-               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "l"(policy)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all committed bulk groups of this thread have finished READING their shared-memory source
-__device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-// ... have completed (their global writes are visible to this thread's later async-proxy operations)
-__device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-// ---- TMEM allocation (one full warp; same warp frees) ----------------------------------------
-template <int G>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  if constexpr (G == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int G>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (G == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  } else {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  }
-}
-
-// ---- UMMA descriptors ---------------------------------------------------------------------
-// K-major operand tile, 128-byte swizzle: rows of 64 fp16 (128 B), 8-row swizzle atoms 1024 B
-// apart (SBO), LBO unused for swizzled K-major layouts.  Bit layout: cute::UMMA::SmemDescriptor
-// (start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), base_offset [49,52),
-// layout_type [61,64) with SWIZZLE_128B = 2).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// Instruction descriptor, kind::f16: D fp32, A/B fp16, both K-major.  (cute::UMMA::InstrDescriptor:
-// c_format [4,6)=1, a_format [7,10)=0 (F16), b_format [10,13)=0, n>>3 [17,23), m>>4 [24,29).)
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int m, int n) {
-  return (1u << 4) | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; one thread issues for the CTA (pair).
-template <int G>
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  if constexpr (G == 1) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-
-// tcgen05.commit: the mbarrier gets one arrival when every MMA issued so far by this thread has
-// completed (implies tcgen05.fence::before_thread_sync).  G == 2: delivered to the barrier at the
-// same offset in both CTAs of the pair.
-template <int G>
-__device__ __forceinline__ void umma_commit(uint64_t* bar, uint16_t pair_mask = 3) {
-  if constexpr (G == 1) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-  } else {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-        ::"r"(smem_u32(bar)), "h"(pair_mask)
-        : "memory");
-  }
-}
-
-// ---- TMEM -> registers --------------------------------------------------------------------
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives lane (base_lane + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+      "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate)
       : "memory");
 }
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x4(uint32_t taddr, uint32_t (&r)[4]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
-// ---- misc math ----------------------------------------------------------------------------
-// ---- streaming global access (read-once data: keep it out of L1 and first in line for L2 eviction) ----
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-  uint64_t pol;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
+// ---- cp.async -----------------------------------------------------------------------------------
+// 16 bytes global -> shared; valid == false writes zeros (src is not read)
+__device__ __forceinline__ void cp16(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
 }
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t pol;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
-__device__ __forceinline__ float4 ld_stream_f4(const float* p, uint64_t pol) {
-  float4 v;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
-               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-               : "l"(p), "l"(pol));
-  return v;
-}
-// asynchronous prefetch of `bytes` (multiple of 16) of global memory into L2
-__device__ __forceinline__ void prefetch_l2_bulk(const void* p, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}
+__device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// Packed fp32 pairs (FADD2 / FMUL2 / FFMA2 on sm_100: one issue slot for two IEEE round-to-nearest operations, bit-identical
-// to the scalar forms): the epilogues are issue / latency bound with two warps per scheduler, and half the instructions is
-// also half the code to fetch.
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-  float2 r;
-  asm("{\n\t.reg .b64 ra, rb, rc;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tadd.rn.f32x2 rc, ra, rb;\n\tmov.b64 {%0, %1}, rc;\n\t}"
-      : "=f"(r.x), "=f"(r.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return r;
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-  float2 r;
-  asm("{\n\t.reg .b64 ra, rb, rc;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmul.rn.f32x2 rc, ra, rb;\n\tmov.b64 {%0, %1}, rc;\n\t}"
-      : "=f"(r.x), "=f"(r.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return r;
-}
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-  float2 r;
-  asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-      "fma.rn.f32x2 rd, ra, rb, rc;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-      : "=f"(r.x), "=f"(r.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-  return r;
-}
+// ---- math ---------------------------------------------------------------------------------------
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -385,14 +75,17 @@ __device__ __forceinline__ float rcp_approx(float x) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-
-// hi/lo fp16 split of an fp32 value: v ~= hi + lo with |v - hi - lo| <~ 2^-22 |v| (lo may be subnormal)
-__device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
-  hi = __float2half_rn(v);
-  lo = __float2half_rn(v - __half2float(hi));
+// sigmoid(g) * tanh(f) with tanh.approx (relative error ~2^-11, below the fp16 rounding of the gate output that follows)
+__device__ __forceinline__ float gate_fast(float g, float f) {
+  return fmaf(0.5f, tanh_approx(0.5f * g), 0.5f) * tanh_approx(f);
 }
-__device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
-  return static_cast<uint32_t>(__half_as_ushort(a)) | (static_cast<uint32_t>(__half_as_ushort(b)) << 16);
+// sigmoid(g) * tanh(f) = (1 - E2) / ((1 + E1)(1 + E2)), E1 = e^-g, E2 = e^-2f: absolute error ~2e-7.  f is clamped at -15
+// (tanh = -1 to 2e-13) so E2 stays finite.
+__device__ __forceinline__ float gate_acc(float g, float f) {
+  const float e1 = ex2_approx(-1.4426950408889634f * g);
+  const float e2 = ex2_approx(-2.8853900817779268f * fmaxf(f, -15.f));
+  return (1.f - e2) * rcp_approx((1.f + e1) * (1.f + e2));
 }
+__device__ __forceinline__ uint32_t h2_bits(__half2 v) { return *reinterpret_cast<uint32_t*>(&v); }
 
 }  // namespace dsx

@@ -1,4 +1,4 @@
-"""Drop-in installation inside the reference tree (SURVEY.md section 8b).
+"""Drop-in installation inside the reference tree.
 
     import diffsinger_b200.dropin as dropin; dropin.install()      # after utils.hparams.set_hparams(...)
 
@@ -7,7 +7,7 @@ replaces, without editing any reference file,
   * ``usr.diff.shallow_diffusion_tts.OfflineGaussianDiffusion`` (usr/diffsinger_task.py:128) and
   * ``usr.diff.diffusion.GaussianDiffusion`` (the older full-T sampler, usr/task.py:18)
 -- and the names bound from them in ``usr.*`` / ``tasks.*`` / ``inference.*`` modules already imported -- by subclasses
-whose ``forward(infer=True)`` runs the sm_100a sampler, and the ``'wavenet'`` entry of every ``DIFF_DECODERS`` registry by
+whose ``forward(infer=True)`` runs the sm_90a sampler, and the ``'wavenet'`` entry of every ``DIFF_DECODERS`` registry by
 ``diffsinger_b200.DiffNet``.  Construction arguments, parameter / buffer names, ``p_losses`` and the returned ``ret`` dict
 are the reference's own, so the task files run unchanged.
 """

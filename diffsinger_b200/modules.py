@@ -1,11 +1,11 @@
-"""Host-side mirror of the reference's class surface for the hot path (SURVEY.md section 8b):
+"""Host-side mirror of the reference's class surface for the hot path:
 
   * ``DiffNet``            usr/diff/net.py:81-130        (same ctor, parameter names, forward contract)
   * ``GaussianDiffusion``  usr/diff/shallow_diffusion_tts.py:71-282 (same ctor, buffers, forward / ret dict)
 
 Same state-dict keys (``denoise_fn.residual_layers.{l}.dilated_conv.weight`` ...), so reference
 checkpoints load with ``strict=True``.  Under ``torch.no_grad`` / ``infer=True`` every evaluation goes
-to the sm_100a kernels through the C ABI and fails loudly on CPU tensors.  The training branch
+to the sm_90a kernels through the C ABI and fails loudly on CPU tensors.  The training branch
 (``p_losses`` under autograd) is outside this round's scope (section 8f rank 4): it keeps the module
 graph in plain PyTorch ops so existing training code still runs, and is never used for inference.
 """

@@ -1,4 +1,4 @@
-"""Utterance sharding across GPUs (SURVEY.md section 8e): batch rows are independent for the whole
+"""Utterance sharding across GPUs: batch rows are independent for the whole
 K-step loop, so each rank samples a contiguous slice of the batch with no per-step communication and
 ONE all-gather of the finished mel shards at the end (NCCL over NVLink / NVSwitch; gloo on CPU tests).
 """

@@ -164,7 +164,7 @@ class DsxSampler:
     def _cond_arg(self, cond, B, T):
         """Pointer to hand to the C ABI: NULL when the handle already holds the pack + projection of this very
         conditioner for (B, T) (same storage -- kept alive here so its address cannot be recycled -- same view, same
-        version counter), so per-step callers do not re-run them (SURVEY.md 8b, reference loop :261-270)."""
+        version counter), so per-step callers do not re-run them (reference loop usr/diff/shallow_diffusion_tts.py:261-270)."""
         st = cond.untyped_storage()
         key = (st.data_ptr(), cond.storage_offset(), tuple(cond.shape), tuple(cond.stride()), cond._version, B, T,
                self._wkey is not None)

@@ -1,8 +1,8 @@
 /*
- * dsx -- C ABI of the B200-native DiffSinger reverse-diffusion sampler.
+ * dsx -- C ABI of the H100-native (sm_90a) DiffSinger reverse-diffusion sampler.
  *
  * The reference (MoonInTheRiver/DiffSinger) has no native boundary: the hot path is a Python
- * class surface (SURVEY.md section 8b).  This header is the boundary a binding would target;
+ * class surface.  This header is the boundary a binding would target;
  * each entry point names the reference interface it replaces (paths relative to the
  * reference tree).  Conventions:
  *   - plain pointers and sizes only; device pointers unless a parameter says "host";
@@ -35,19 +35,18 @@ enum {
   DSX_E_NOMEM = -5
 };
 
-/* Arithmetic of the contractions of each residual layer (usr/diff/net.py:66-78).  In the tcgen05 modes the conditioner
+/* Arithmetic of the contractions of each residual layer (usr/diff/net.py:66-78).  In the tensor-core modes the conditioner
  * projection -- it does not depend on the diffusion step -- is computed once per call with hi+lo operands and kept in
  * fp32; the modes differ in the dilated conv and the output projection. */
 enum {
   DSX_PREC_FP32_SIMT = 0, /* fp32 CUDA-core path, any channel count                          */
-  DSX_PREC_FP16 = 1,      /* tcgen05 kind::f16, fp16 operands, fp32 accumulate (fast mode)   */
-  DSX_PREC_FP16X2 = 2,    /* tcgen05, weights as hi+lo fp16 pairs, running activations fp16: 2 MMA passes;
-                             max |d| ~2e-4 after 100 steps (default parity mode)                               */
-  DSX_PREC_FP16X3 = 3,    /* tcgen05, hi+lo fp16 split of both operands, 3 MMAs (fp32-equivalent)*/
-  DSX_PREC_FP16S = 4      /* tcgen05, ONE MMA pass; the weights are rounded to fp16 stochastically into R sets
+  DSX_PREC_FP16 = 1,      /* wgmma f16, fp16 operands, fp32 accumulate (fast mode)           */
+  DSX_PREC_FP16X2 = 2,    /* wgmma, weights as hi+lo fp16 pairs, running activations fp16: 2 MMA passes */
+  DSX_PREC_FP16X3 = 3,    /* wgmma, hi+lo fp16 split of both operands, 3 MMAs (fp32-equivalent)*/
+  DSX_PREC_FP16S = 4      /* wgmma, ONE MMA pass; the weights are rounded to fp16 stochastically into R sets
                              (DSX_OPT_SR_SETS, default 64) and evaluation j of a sampling loop uses set j % R, so the weight
-                             rounding error is unbiased and decorrelated across diffusion steps instead of accumulating:
-                             max |d| ~3e-4 after 100 steps at half the MMA work of FP16X2 */
+                             rounding error is unbiased and decorrelated across diffusion steps instead of accumulating,
+                             at half the MMA work of FP16X2 */
 };
 
 typedef struct dsx_handle dsx_handle;
@@ -182,35 +181,34 @@ enum {
   DSX_INFO_KERNEL_LAUNCHES = 1, /* kernels launched by this handle so far               */
   DSX_INFO_WORKSPACE_BYTES = 2,
   DSX_INFO_SM_COUNT = 3,
-  DSX_INFO_TC_CTA_GROUP = 4,    /* 1 or 2: cta_group of the tcgen05 path in use          */
+  DSX_INFO_TC_CTA_GROUP = 4,    /* 2 when the tensor-core (sm_90a) path is available on the device, else 0 */
   DSX_INFO_LAYER_KERNEL_NS = 5, /* DSX_OPT_PROFILE: summed device time of the residual-layer kernels since the
                                    option was set (CUDA events on the launching stream; synchronises)     */
   DSX_INFO_LAYER_KERNEL_LAUNCHES = 6, /* number of (start, stop) brackets = evaluations profiled */
   DSX_INFO_STACK_MODE = 7,
-  DSX_INFO_CLUSTER_OCCUPANCY = 8, /* co-resident CTA pairs of the layer kernel reported by the driver */
-  DSX_INFO_STACK_KERNEL_LAUNCHES = 9, /* launches of the register-resident stack kernel (dsx_stack.cu) so far */
-  DSX_INFO_STACK_ROWS = 10 /* frames per CTA of the last stack-kernel launch: 128, or 64 for small batches */
+  DSX_INFO_CLUSTER_OCCUPANCY = 8, /* co-resident 128-frame CTAs of the step kernel on the device (0 before the first launch) */
+  DSX_INFO_STACK_KERNEL_LAUNCHES = 9, /* one-launch-per-step launches (all layers + head, DSX_OPT_STACK_KERNEL) so far */
+  DSX_INFO_STACK_ROWS = 10 /* frames per CTA of the last such launch: 128, or 64 for small batches */
 };
 /* Tuning knobs (tests exercise every variant): */
 int dsx_set_option(dsx_handle* h, int what, int64_t value);
 enum {
-  DSX_OPT_TC_CTA_GROUP = 0, /* 2 (the layer kernel pairs CTAs; kept for forward compatibility) */
-  DSX_OPT_CP_PREFETCH = 1,  /* tuning knob, results do not depend on it: 1 = the layer kernel's activation producer streams the
-                               hoisted conditioner projection HBM -> L2 half a layer ahead of the gate epilogue */
+  DSX_OPT_TC_CTA_GROUP = 0, /* accepts 2 only; kept for ABI compatibility, no effect */
+  DSX_OPT_CP_PREFETCH = 1,  /* accepted and ignored (kept for ABI compatibility): the sm_90 kernels have no prefetch stage */
   DSX_OPT_PROFILE = 2,      /* 1: bracket the residual-layer kernel(s) of every evaluation with CUDA events; 2: bracket the
                                head / update kernel of every DDPM step instead; 0: off.  Setting it resets the sums */
-  DSX_OPT_STACK_MODE = 3,   /* 1 (default): all residual layers of an evaluation in ONE persistent launch whenever every
-                               128-frame tile can own an SM at once (tiles <= co-resident CTAs); 0: one launch per layer */
-  DSX_OPT_STACK_KERNEL = 4, /* 1 (default): the register-resident stack kernel (residual stream in registers, conv input in
-                               shared memory, skip sum in tensor memory) for FP16 / FP16X2 / FP16S; 0: the round-1 layer kernel */
+  DSX_OPT_STACK_MODE = 3,   /* 1 (default): all residual layers of an evaluation in ONE persistent cooperative launch (grid-wide
+                               barrier between layers); 0: one launch per layer */
+  DSX_OPT_STACK_KERNEL = 4, /* 1 (default): for FP16 / FP16X2 / FP16S the layers and the head of a step share ONE launch, with
+                               64-frame CTAs for small batches and FP16S's stochastically rounded weight sets; 0: the layers use
+                               the hi/lo weight planes at 128 frames per CTA (FP16S then runs the FP16X2 scheme) */
   DSX_OPT_SR_SETS = 5,      /* number of stochastically rounded weight sets of DSX_PREC_FP16S; set before dsx_load_diffnet */
-  DSX_OPT_GATE_APPROX = 7,  /* stack kernel: gate sigmoid(g) * tanh(f) with tanh.approx.f32 (1) or with ex2 / rcp to ~2e-7 (0);
-                               -1 (default) = 1: its 2^-11 relative error is below the fp16 rounding of the gate output that
-                               follows (K = 100 golden loop: 3.3e-4 either way in FP16S, 1.5e-4 / 1.6e-4 in FP16X2) */
+  DSX_OPT_GATE_APPROX = 7,  /* gate sigmoid(g) * tanh(f) with tanh.approx.f32 (1) or with ex2 / rcp to ~2e-7 (0); -1 (default) =
+                               1 except for FP16X3: its 2^-11 relative error is below the fp16 rounding of the gate output */
   DSX_OPT_FUSED_HEAD = 9,   /* 1 (default): the skip / output projections, the sampler update and the next input projection run
-                               inside the stack kernel's launch (one kernel per diffusion step); 0: separate head kernel */
-  DSX_OPT_STACK_ROWS = 8,   /* stack kernel: frames per CTA.  0 (default) = 64 whenever the whole batch then fits the machine at once
-                               (small batches: twice the CTAs, about half the time per layer), else 128; 64 / 128 force it */
+                               inside the layers' launch (one kernel per diffusion step); 0: a second launch */
+  DSX_OPT_STACK_ROWS = 8,   /* frames per CTA of the one-launch-per-step form.  0 (default) = 64 whenever the batch then has a
+                               resident CTA per 64-frame tile (small batches), else 128; 64 / 128 force it (results are bit-identical) */
   DSX_OPT_BATCH_OFFSET = 6  /* global index of this call's utterance 0: the in-kernel Philox noise of utterance b is drawn for
                                index (offset + b), so a batch sharded over ranks (one seed) reproduces the unsharded noise */
 };
@@ -219,19 +217,14 @@ enum {
  * buffers after a dsx_diffnet_forward.  which: 0 = residual stream after the last layer
  * executed, 1 = skip sum.  out: [B, T, C] contiguous. */
 int dsx_debug_read(dsx_handle* h, int which, float* out, int B, int T, void* stream);
-/* Debug timeline of the residual-layer kernel: enable != 0 makes CTAs 0 and 1 of every following layer
- * launch record clock64 stamps ([2][3 roles: producer, MMA issuer, epilogue][256] int64); out_host (may be
- * NULL) receives the current buffer contents (6*256 int64) after synchronising the device.  enable == 2: out_host
- * receives 10*256 int64, the extra [256][4] being per-CTA {globaltimer ns, clock64} at kernel entry and exit. */
+/* Kept for ABI compatibility: the sm_90 kernels record no clock64 timeline; always returns DSX_E_INVALID. */
 int dsx_debug_trace(dsx_handle* h, int enable, int64_t* out_host);
 /* Run only layers [0, n_layers) in the next dsx_diffnet_forward calls (<0: all). */
 int dsx_debug_set_layer_limit(dsx_handle* h, int n_layers);
 
-/* Hardware self-tests of the tcgen05 / TMA encodings this library relies on (one small
- * launch each, results checked on the host).  which = -1 runs all; returns 0 when every
- * selected test passes, otherwise DSX_E_KERNEL with the failing names in dsx_last_error().
- * which = 0 / 1: UMMA + TMA round trip with cta_group::1 / ::2; 2 = row-shifted SWIZZLE_128B operand descriptors (the
- * dilated taps rely on them); 3 = TMA ingest micro-benchmark (informational, only in -DDSX_EXPERIMENTS builds, not part of -1).
+/* Hardware self-test of the encodings the tensor-core kernels rely on: the swizzled cp.async operand loads (row shifts,
+ * zero fill outside [0, T)) and the wgmma shared-memory descriptors, on a small GEMM checked against a host product.
+ * which = -1 or 0 runs it; returns 0 when it passes, otherwise DSX_E_KERNEL with the report in dsx_last_error().
  * report (may be NULL): host buffer receiving a text report. */
 int dsx_selftest(int device, int which, char* report, int report_bytes);
 

@@ -6,7 +6,7 @@ samplers).  Nothing under ``oracle/`` is part of the shipped product: only ``tes
 ``bench.py`` may import it, and only as the checker / the timed CPU baseline.
 
 Parity pinning: the reference has no tests or golden vectors for this path
-(SURVEY.md §4), so the oracle is pinned against the live reference PyTorch modules
-imported from /root/reference in the build container (``oracle/ref_bridge.py`` +
+, so the oracle is pinned against the live reference PyTorch modules
+imported from a checkout of the reference (``oracle/ref_bridge.py`` +
 ``oracle/gen_golden.py``); the vectors it produced are committed in ``tests/golden``.
 """

@@ -17,7 +17,7 @@ entries can be fed in directly.  Arithmetic is torch CPU fp32 (the same ATen CPU
 the reference runs on), which is what "the reference's own CPU path" means for this repo.
 
 Pinning: ``oracle/gen_golden.py`` compares every function here against the live
-reference modules imported from /root/reference (bit-exact or <=1e-6) and writes the
+reference modules imported from a checkout of the reference (bit-exact or <=1e-6) and writes the
 vectors in ``tests/golden``; ``tests/test_oracle.py`` re-checks the oracle against those
 vectors wherever the tests run.
 """
@@ -42,7 +42,7 @@ def build_state_dict(seed=0, in_dims=80, residual_channels=256, encoder_hidden=2
 
     ``out_std``: the reference zero-initialises the last projection (net.py:105), which
     makes eps independent of x; fixtures re-draw it N(0, out_std) afterwards
-    (SURVEY.md section 8(d)).  Pass ``None`` to keep the zeros.
+    Pass ``None`` to keep the zeros.
     """
     import torch.nn as nn
 

@@ -1,8 +1,9 @@
 """TEST INFRASTRUCTURE ONLY -- pins the oracle against the LIVE reference and writes tests/golden.
 
-Run in the build container (needs /root/reference):
+Needs a checkout of the reference (DSX_REFERENCE_ROOT=<its directory>); run from the repository root:
 
-    cd /root/repo && python -m oracle.gen_golden
+    DSX_REFERENCE_ROOT=... python -m oracle.gen_golden                      # every fixture
+    DSX_REFERENCE_ROOT=... python -m oracle.gen_golden --reference-diffnet  # tests/golden/reference_diffnet.npz only
 
 Every vector written here is an output of the unmodified reference modules
 (usr/diff/net.py DiffNet, usr/diff/shallow_diffusion_tts.py GaussianDiffusion) on seeded
@@ -54,12 +55,44 @@ def make_ref_gd(ns, net, betas, K_step):
     return gd
 
 
+def write_reference_diffnet(ns):
+    """One evaluation of the reference's own DiffNet (seed 0, output_projection re-initialised with N(0, 0.02)) on seeded
+    inputs, its parameter names and shapes, and those of the whole GaussianDiffusion module built from the LJ config: lets
+    tests/test_reference_live.py check the package's DiffNet (same init stream, same state-dict surface), the installed
+    drop-in classes and the oracle against the reference without its source tree."""
+    net = make_ref_net(ns, 0, 1)
+    g = torch.Generator().manual_seed(2024)
+    x = torch.randn(2, 1, 80, 24, generator=g)
+    cond = torch.randn(2, 256, 24, generator=g)
+    t = torch.tensor([3, 50])
+    with torch.no_grad():
+        eps = net(x, t, cond)
+    sd = net.state_dict()
+    assert torch.equal(eps, O.diffnet_forward({k: v for k, v in sd.items()}, x, t, cond, 1))
+    # the state-dict surface of the whole sampler module as the task files build it (a checkpoint's `model.*` entries)
+    hp = ns.hparams
+    enc = ns.TokenTextEncoder(None, vocab_list=["a", "b", "c"], replace_oov=",")
+    gd = ns.GaussianDiffusion(enc, 80, ns.DiffNet(80), timesteps=hp["timesteps"], K_step=hp["K_step"], loss_type="l1",
+                              spec_min=hp["spec_min"], spec_max=hp["spec_max"])
+    gsd = gd.state_dict()
+    np.savez(os.path.join(OUT, "reference_diffnet.npz"), x=x.numpy(), cond=cond.numpy(), t=t.numpy(), eps=eps.numpy(),
+             keys=np.array(list(sd.keys())), shapes=np.array([",".join(map(str, v.shape)) for v in sd.values()]),
+             fingerprint=np.float64(fingerprint(sd)), gd_keys=np.array(list(gsd.keys())),
+             gd_shapes=np.array([",".join(map(str, v.shape)) for v in gsd.values()]),
+             gd_timesteps=np.int64(hp["timesteps"]), gd_K_step=np.int64(hp["K_step"]),
+             gd_spec_min=np.array(hp["spec_min"], dtype=np.float32), gd_spec_max=np.array(hp["spec_max"], dtype=np.float32),
+             gd_max_beta=np.float64(hp["max_beta"]), gd_schedule_type=np.array(hp["schedule_type"]))
+
+
 def main():
-    assert ref_bridge.available(), "needs /root/reference"
+    assert ref_bridge.available(), "set DSX_REFERENCE_ROOT to a checkout of the reference"
     torch.set_num_threads(8)
     ns = ref_bridge.load("usr/configs/lj_ds_beta6.yaml")
     sdt = ns.sdt
     os.makedirs(OUT, exist_ok=True)
+    write_reference_diffnet(ns)
+    if "--reference-diffnet" in sys.argv:
+        return
     report = {}
 
     # ---- 1. schedules --------------------------------------------------------------

@@ -1,5 +1,6 @@
-"""TEST INFRASTRUCTURE ONLY -- pins oracle/hifigan_oracle.py to the LIVE reference (container only: needs /root/reference)
-and writes tests/golden/hifigan_nsf.npz.  Run:  python oracle/gen_golden_hifigan.py
+"""TEST INFRASTRUCTURE ONLY -- pins oracle/hifigan_oracle.py to the LIVE reference (needs a checkout of the reference: DSX_REFERENCE_ROOT)
+and writes tests/golden/hifigan_nsf.npz and hifigan_nsf_b1t9.npz.
+Run:  DSX_REFERENCE_ROOT=<checkout> python oracle/gen_golden_hifigan.py [--single-utterance-case]
 
 The reference module is imported unmodified (stubs only for librosa / pycwt and scipy.signal.kaiser, which newer SciPy moved
 to scipy.signal.windows); weights are the constructor's random initialisation under a fixed seed, inputs are seeded; the NSF
@@ -15,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import hifigan_oracle as H  # noqa: E402
 
-REF_ROOT = os.environ.get("DSX_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("DSX_REFERENCE_ROOT", "")
 
 
 def load_reference():
@@ -45,7 +46,26 @@ def make_case(seed=0, B=2, T=16):
     return g, h, sd, mel, f0
 
 
+def write_single_utterance_case():
+    """A second case (other weights, one utterance of 9 frames, NSF source): tests/golden/hifigan_nsf_b1t9.npz."""
+    g, h, sd, mel, f0 = make_case(seed=3, B=1, T=9)
+    with torch.no_grad():
+        torch.manual_seed(11)
+        ref = g(mel, f0)
+        torch.manual_seed(11)
+        ora = H.generator(sd, h, mel, f0)
+    assert torch.equal(ref, ora), "the oracle must be bit-exact against the reference"
+    out = os.path.join(ROOT, "tests", "golden", "hifigan_nsf_b1t9.npz")
+    np.savez_compressed(out, mel=mel.numpy(), f0=f0.numpy(), wav_nsf=ref.numpy(), rng_seed=np.int64(11), weight_seed=np.int64(3),
+                        upsample_initial_channel=np.int64(h["upsample_initial_channel"]),
+                        **{"sd." + k: v.numpy() for k, v in sd.items()})
+    print("wrote", out, os.path.getsize(out) // 1024, "KB")
+
+
 def main():
+    write_single_utterance_case()
+    if "--single-utterance-case" in sys.argv:
+        return
     g, h, sd, mel, f0 = make_case()
     with torch.no_grad():
         torch.manual_seed(7)

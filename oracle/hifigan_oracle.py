@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE ONLY -- CPU restatement of the reference's HiFi-GAN (NSF) generator, the next row of the hot-path
-scope table (SURVEY.md section 8f rank 2: the vocoder that follows the sampler).  No kernel exists for it yet; this file and
+scope table (the vocoder that follows the sampler).  No kernel exists for it yet; this file and
 tests/golden/hifigan_*.npz pin the algorithm so that a kernel can be held to it.
 
 Functional torch-CPU fp32 (the ATen kernels the reference itself runs), every function citing the reference lines it

@@ -1,20 +1,17 @@
-"""TEST INFRASTRUCTURE ONLY -- imports the *live* reference from /root/reference.
+"""TEST INFRASTRUCTURE ONLY -- imports the *live* reference from the checkout named by DSX_REFERENCE_ROOT.
 
-Only usable in the build container (the GPU box has no /root/reference); used by
-``oracle/gen_golden.py`` to pin the oracle and by the container-only tests.
-Recipe: SURVEY.md appendix A (stub ``librosa`` / ``pycwt``, ``set_hparams`` before
-importing ``usr.diff.shallow_diffusion_tts`` because ``max_beta`` binds at import time,
-usr/diff/shallow_diffusion_tts.py:44).
+Used by ``oracle/gen_golden.py`` to pin the oracle and write the fixtures under ``tests/golden``.  Recipe: stub ``librosa`` / ``pycwt``, ``set_hparams`` before importing ``usr.diff.shallow_diffusion_tts``
+because ``max_beta`` binds at import time (usr/diff/shallow_diffusion_tts.py:44).
 """
 import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("DSX_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("DSX_REFERENCE_ROOT", "")
 
 
 def available():
-    return os.path.isdir(os.path.join(REF_ROOT, "usr", "diff"))
+    return bool(REF_ROOT) and os.path.isdir(os.path.join(REF_ROOT, "usr", "diff"))
 
 
 _loaded = {}

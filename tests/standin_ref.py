@@ -1,5 +1,5 @@
 """Writes a STAND-IN for the reference tree (the few modules `diffsinger_b200.dropin` touches) into a directory, so the
-installed subclasses can be driven end to end on a GPU box where /root/reference does not exist.
+installed subclasses can be driven end to end without a checkout of the reference.
 
 The stand-in keeps the reference's module paths, class names, constructor signatures and attributes
 (usr/diff/shallow_diffusion_tts.py:71-126,285-290; usr/diff/diffusion.py:178-232; usr/diff/net.py:81-105; usr/task.py:10-12)

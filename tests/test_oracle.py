@@ -16,7 +16,7 @@ def test_schedules_match_reference_buffers():
         S = O.make_schedule(betas)
         for b in O.SCHEDULE_BUFFERS:
             assert np.array_equal(S[b].numpy(), g[f"{name}.{b}"]), (name, b)
-    # appendix B anchors (SURVEY.md): coef1[0] = 1, coef2[0] = 0, clipped log-variance at 0 = ln(1e-20)
+    # schedule anchors: coef1[0] = 1, coef2[0] = 0, clipped log-variance at 0 = ln(1e-20)
     S = O.make_schedule(O.linear_beta_schedule(100, 0.06))
     assert S["posterior_mean_coef1"][0] == 1 and S["posterior_mean_coef2"][0] == 0
     assert abs(float(S["posterior_log_variance_clipped"][0]) - np.log(1e-20)) < 1e-4

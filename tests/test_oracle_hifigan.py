@@ -1,18 +1,15 @@
-"""CPU: the HiFi-GAN (NSF) oracle -- groundwork for the next scope row (SURVEY.md section 8f rank 2); no kernel yet -- against
-the fixture produced by the unmodified reference (oracle/gen_golden_hifigan.py), and against the live reference where the
-build container has it."""
-import os
-
+"""CPU: the HiFi-GAN (NSF) oracle -- groundwork for the next scope row; no kernel yet -- against two cases computed by the
+unmodified reference (oracle/gen_golden_hifigan.py, which asserts the oracle bit-exact against the reference when it writes
+them)."""
 import numpy as np
-import pytest
 import torch
 
 from conftest import golden
 from oracle import hifigan_oracle as H
 
 
-def _case():
-    g = golden("hifigan_nsf.npz")
+def _case(name="hifigan_nsf.npz"):
+    g = golden(name)
     sd = {k[3:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd.")}
     h = dict(H.HPARAMS_TTS, upsample_initial_channel=int(g["upsample_initial_channel"]))
     return g, sd, h, torch.from_numpy(g["mel"]), torch.from_numpy(g["f0"])
@@ -25,8 +22,9 @@ def test_generator_matches_reference_fixture():
         wav = H.generator(sd, h, mel, f0)
         plain = H.generator(sd, h, mel)
     assert wav.shape == (mel.shape[0], 1, mel.shape[2] * int(np.prod(h["upsample_rates"])))
-    assert np.array_equal(wav.numpy(), g["wav_nsf"])          # bit-exact: same ATen kernels, same RNG stream
-    assert np.array_equal(plain.numpy(), g["wav_plain"])
+    # same ATen kernels and RNG stream, but other host CPUs pick other conv kernels: a few ulps (3e-8 on a 0.1 signal)
+    for out, ref in ((wav, g["wav_nsf"]), (plain, g["wav_plain"])):
+        assert np.abs(out.numpy() - ref).max() <= 1e-6 * np.abs(ref).max()
     assert np.abs(g["wav_nsf"] - g["wav_plain"]).max() > 1e-4   # the harmonic source does reach the output
 
 
@@ -48,13 +46,12 @@ def test_flops_per_frame_of_the_shipped_config():
     assert H.flops_per_frame(H.HPARAMS_TTS) == 38510592.0
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/modules/hifigan"), reason="live reference only in the build container")
 def test_oracle_is_bit_exact_against_the_live_reference():
-    from oracle import gen_golden_hifigan as G
-    ref, h, sd, mel, f0 = G.make_case(seed=3, B=1, T=9)
+    """The reference's HifiGanGenerator on other weights (seed 3) and one utterance of 9 frames with the NSF source
+    (tests/golden/hifigan_nsf_b1t9.npz): bit-exact where the fixture was written, a few ulps on other host CPUs."""
+    g, sd, h, mel, f0 = _case("hifigan_nsf_b1t9.npz")
     with torch.no_grad():
-        torch.manual_seed(11)
-        a = ref(mel, f0)
-        torch.manual_seed(11)
+        torch.manual_seed(int(g["rng_seed"]))
         b = H.generator(sd, h, mel, f0)
-    assert torch.equal(a, b)
+    assert b.shape == g["wav_nsf"].shape
+    assert np.abs(b.numpy() - g["wav_nsf"]).max() <= 1e-6 * np.abs(g["wav_nsf"]).max()
