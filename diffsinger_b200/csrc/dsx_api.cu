@@ -418,6 +418,7 @@ void dsx_destroy(dsx_handle* h) {
     if (p) cudaFree(p);
   if (h->status_dev) cudaFree(h->status_dev);
   if (h->status_host) cudaFreeHost(h->status_host);
+  if (h->trace_dev) cudaFree(h->trace_dev);
   delete h;
 }
 
@@ -653,7 +654,7 @@ int dsx_set_option(dsx_handle* h, int what, int64_t value) {
       DSX_CHECK(value == 2, DSX_E_INVALID, "DSX_OPT_TC_CTA_GROUP only accepts 2 (kept for ABI compatibility)");
       DSX_CHECK(h->tc_group != 0, DSX_E_INVALID, "no tensor-core path on this device");
       break;
-    case DSX_OPT_CP_PREFETCH: break;   // no prefetch stage to tune in the sm_90 kernels; results never depended on it
+    case DSX_OPT_CP_PREFETCH: break;   // the step kernel's L2 prefetch is unconditional; results never depended on it
     case DSX_OPT_STACK_MODE: h->stack_mode = static_cast<int>(value); break;
     case DSX_OPT_STACK_KERNEL: h->stack_kernel = static_cast<int>(value); break;
     case DSX_OPT_GATE_APPROX: h->gate_approx = static_cast<int>(value); break;
@@ -690,10 +691,24 @@ int dsx_debug_read(dsx_handle* h, int which, float* out, int B, int T, void* str
   return DSX_OK;
 }
 
-int dsx_debug_trace(dsx_handle* h, int, int64_t*) {
+int dsx_debug_trace(dsx_handle* h, int enable, int64_t* out_host) {
   DSX_CHECK(h, DSX_E_INVALID, "null handle");
-  set_error("the sm_90 kernels record no clock64 timeline");
-  return DSX_E_INVALID;
+  DSX_CUDA(cudaSetDevice(h->device));
+  const size_t bytes = static_cast<size_t>(2) * h->sm_count * DSX_TRACE_SLOTS * sizeof(int64_t);
+  if (enable) {
+    if (!h->trace_dev) DSX_CUDA(cudaMalloc(&h->trace_dev, bytes));
+    DSX_CUDA(cudaMemset(h->trace_dev, 0, bytes));
+    DSX_CUDA(cudaDeviceSynchronize());
+    h->trace_on = true;
+    return DSX_OK;
+  }
+  h->trace_on = false;
+  if (out_host) {
+    DSX_CHECK(h->trace_dev, DSX_E_STATE, "no trace recorded (enable it first)");
+    DSX_CUDA(cudaDeviceSynchronize());
+    DSX_CUDA(cudaMemcpy(out_host, h->trace_dev, bytes, cudaMemcpyDeviceToHost));
+  }
+  return DSX_OK;
 }
 
 int dsx_debug_set_layer_limit(dsx_handle* h, int n_layers) {

@@ -19,7 +19,8 @@
 // Operands reach shared memory by cp.async in the 128-byte-swizzled K-major layout wgmma reads (dsx_ptx.cuh), double
 // buffered: one stage = a 256-row x 64-k weight tile (32 KB, shared by the warpgroups) + one 64 x 64 activation block per
 // warpgroup.  Each warpgroup's rows go through the same instruction sequence whatever NWG is, so 64- and 128-frame CTAs
-// give bit-identical results.
+// give bit-identical results.  While GEMM1 runs, the warpgroup prefetches the CP, x and skip rows its epilogues read
+// into L2, and the epilogues issue their global loads in batches ahead of their stores.
 //
 // Precision (MMA passes P per k-block): P = 1 fp16 operands; P = 2 adds a W_lo pass (weights as hi+lo fp16 pairs);
 // P = 3 accumulates A_hi*W_hi + A_hi*W_lo + A_lo*W_hi (~2^-22 relative).  The conditioner projection is always 3-pass.
@@ -46,6 +47,7 @@ constexpr int kSrRowsPerLayer = 32 * 256;  // rows per layer of one stochastical
 constexpr int kWBytes = 256 * 128;         // one weight tile: 256 rows x 64 fp16
 constexpr int kABytes = 64 * 128;          // one activation block: 64 rows x 64 fp16
 constexpr int kZBytes = 2 * 4 * kABytes;   // per warpgroup: z / h / x_in operand, [plane hi, lo][4 k-blocks]
+constexpr int kEpiBatch = 8;               // accumulator pairs whose global loads a layer epilogue issues at once
 
 template <int NWG>
 struct StepCfg {
@@ -94,7 +96,20 @@ struct HpParams {
   const float* d0;           // FiLM vector of layer 0 of the evaluation being prepared (TC_INPROJ)
   int d0_row_stride;
   int M;
+  long long* trace;          // dsx_debug_trace buffer [trace_ctas][DSX_TRACE_SLOTS], or nullptr
+  int trace_ctas;
 };
+
+// phase stamp of dsx_debug_trace (layout in dsx.h); one uniform branch when tracing is off
+__device__ __forceinline__ void stamp(const HpParams& p, int slot) {
+  if (p.trace != nullptr && threadIdx.x == 0 && slot < DSX_TRACE_SLOTS && static_cast<int>(blockIdx.x) < p.trace_ctas) {
+    long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
+    p.trace[static_cast<size_t>(blockIdx.x) * DSX_TRACE_SLOTS + slot] = t;
+  }
+}
+__device__ __forceinline__ int layer_slot(const HpParams& p, int l, int k) { return 1 + 9 * (l - p.l0) + k; }
+__device__ __forceinline__ int head_slot(const HpParams& p, int k) { return 1 + 9 * (p.l1 - p.l0) + k; }
 
 // ------------------------------------------------------------------------------------------
 // operand loads and the GEMM loop
@@ -128,13 +143,18 @@ __device__ __forceinline__ void fence_acc(float (&d)[N]) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+struct NoPrefetch {
+  __device__ __forceinline__ void operator()(int) const {}
+};
+
 // c0 (weight rows 0..127) [and c1 (rows 128..255) when NH == 2] = sum over nst stages of A_s . W_s^T.  load(s, buf) issues
-// the cp.async copies of stage s into buf; adesc(s, buf) is the descriptor of this warpgroup's A block of stage s.
-// Every thread of the CTA runs it (the weight tile is shared); it ends with the accumulators complete and the stage
-// buffers free.
-template <int NH, class Load, class ADesc>
+// the cp.async copies of stage s into buf; adesc(s, buf) is the descriptor of this warpgroup's A block of stage s;
+// pre(s) runs at stage s after the copies of stage s + 1 are issued (L2 prefetches of what the epilogues read, paced so
+// that they queue behind the operand copies).  Every thread of the CTA runs it (the weight tile is shared); it ends with
+// the accumulators complete and the stage buffers free.
+template <int NH, class Load, class ADesc, class Pre = NoPrefetch>
 __device__ __forceinline__ void gemm(float (&c0)[64], float (&c1)[64], int nst, Load load, ADesc adesc, uint8_t* buf0,
-                                     uint8_t* buf1) {
+                                     uint8_t* buf1, Pre pre = Pre()) {
   load(0, buf0);
   cp_commit();
   fence_acc(c0);
@@ -145,8 +165,10 @@ __device__ __forceinline__ void gemm(float (&c0)[64], float (&c1)[64], int nst, 
     if (s + 1 < nst) {
       load(s + 1, (s & 1) ? buf0 : buf1);
       cp_commit();
+      pre(s);
       cp_wait<1>();
     } else {
+      pre(s);
       cp_wait<0>();
     }
     fence_proxy_async_smem();
@@ -218,29 +240,48 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, uint
       load_a(bf + kWBytes + wg * kABytes, Yin + pass_aplane(ps) * p.plane, b, t0 + (tap - 1) * d, cb * 64, p.T, p.Tp, wtid);
     };
     auto adesc = [&](int, uint8_t* bf) { return wg_desc(smem_u32(bf + kWBytes + wg * kABytes)); };
-    gemm<2>(c0, c1, 12 * P, load, adesc, buf0, buf1);
+    // L2 prefetch of this warpgroup's epilogue operands, 16 KB per stage: its CP rows (64 x 2 KB, both chunks) during
+    // chunk 0, its X and SKIP rows (64 x 1 KB each) during chunk 1
+    auto pre = [&](int s) {
+      if (wtid != 0 || s >= 8) return;
+      if (h == 0) prefetch_l2(p.CP + (static_cast<size_t>(l) * NF + fbase) * 512 + s * 4096, 16384);
+      else if (s < 4) prefetch_l2(p.X + fbase * kC + s * 4096, 16384);
+      else if (l > 0) prefetch_l2(p.SKIP + fbase * kC + (s - 4) * 4096, 16384);
+    };
+    gemm<2>(c0, c1, 12 * P, load, adesc, buf0, buf1, pre);
+    stamp(p, layer_slot(p, l, 2 * h));
     const float* cp = p.CP + (static_cast<size_t>(l) * NF + fbase) * 512 + h * 256;
+    // the loads of kEpiBatch accumulator pairs are issued together, ahead of the stores that use them
 #pragma unroll
-    for (int e = 0; e < 64; e += 2) {
-      const int r = acc_row(wtid, e), n = acc_col(wtid, e);
-      const float2 cgv = *reinterpret_cast<const float2*>(cp + static_cast<size_t>(r) * 512 + n);
-      const float2 cfv = *reinterpret_cast<const float2*>(cp + static_cast<size_t>(r) * 512 + 128 + n);
-      float z0, z1;
-      if (p.fast_gate) {
-        z0 = gate_fast(c0[e] + cgv.x, c1[e] + cfv.x);
-        z1 = gate_fast(c0[e + 1] + cgv.y, c1[e + 1] + cfv.y);
-      } else {
-        z0 = gate_acc(c0[e] + cgv.x, c1[e] + cfv.x);
-        z1 = gate_acc(c0[e + 1] + cgv.y, c1[e + 1] + cfv.y);
+    for (int e0 = 0; e0 < 64; e0 += 2 * kEpiBatch) {
+      float2 cgv[kEpiBatch], cfv[kEpiBatch];
+#pragma unroll
+      for (int j = 0; j < kEpiBatch; ++j) {
+        const int e = e0 + 2 * j, r = acc_row(wtid, e), n = acc_col(wtid, e);
+        cgv[j] = ld_stream_f2(cp + static_cast<size_t>(r) * 512 + n);
+        cfv[j] = ld_stream_f2(cp + static_cast<size_t>(r) * 512 + 128 + n);
       }
-      const __half2 hh = __floats2half2_rn(z0, z1);
-      const uint32_t off = opnd_off(r, 128 * h + n);
-      *reinterpret_cast<__half2*>(zb + off) = hh;
-      if (P == 3) {
-        const float2 hf = __half22float2(hh);
-        *reinterpret_cast<__half2*>(zb + 4 * kABytes + off) = __floats2half2_rn(z0 - hf.x, z1 - hf.y);
+#pragma unroll
+      for (int j = 0; j < kEpiBatch; ++j) {
+        const int e = e0 + 2 * j, r = acc_row(wtid, e), n = acc_col(wtid, e);
+        float z0, z1;
+        if (p.fast_gate) {
+          z0 = gate_fast(c0[e] + cgv[j].x, c1[e] + cfv[j].x);
+          z1 = gate_fast(c0[e + 1] + cgv[j].y, c1[e + 1] + cfv[j].y);
+        } else {
+          z0 = gate_acc(c0[e] + cgv[j].x, c1[e] + cfv[j].x);
+          z1 = gate_acc(c0[e + 1] + cgv[j].y, c1[e + 1] + cfv[j].y);
+        }
+        const __half2 hh = __floats2half2_rn(z0, z1);
+        const uint32_t off = opnd_off(r, 128 * h + n);
+        *reinterpret_cast<__half2*>(zb + off) = hh;
+        if (P == 3) {
+          const float2 hf = __half22float2(hh);
+          *reinterpret_cast<__half2*>(zb + 4 * kABytes + off) = __floats2half2_rn(z0 - hf.x, z1 - hf.y);
+        }
       }
     }
+    stamp(p, layer_slot(p, l, 2 * h + 1));
   }
 
   // ---- GEMM2 + residual / skip epilogues ----
@@ -259,49 +300,71 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, uint
       return wg_desc(smem_u32(zb + (pass_aplane(ps) * 4 + kb) * kABytes));
     };
     gemm<2>(c0, c1, 4 * P, load, adesc, buf0, buf1);
-    const float* bias = p.b2 + static_cast<size_t>(l) * 512 + q * 256;
+    stamp(p, layer_slot(p, l, 4 + 2 * q));
+    // This thread's accumulators cover rows row0 and row0 + 8 and columns colb + 8 i + {0, 1} of each 128-column half
+    // (acc_row / acc_col), so every address below is a per-thread base plus a compile-time offset; with the offsets
+    // folded the unrolled loops hold no 64-bit address per element.
+    const int row0 = acc_row(wtid, 0), colb = acc_col(wtid, 0);
+    const bool ok0 = t0 + row0 < p.T, ok8 = t0 + row0 + 8 < p.T;
+    const size_t tb = (fbase + row0) * kC + colb;
+    const float* bias = p.b2 + static_cast<size_t>(l) * 512 + q * 256 + colb;
+    const float* dn = last ? nullptr : dnext + colb;
+    const float* src = (q == 0 ? p.X : p.SKIP) + tb;
+    float* dst = (q == 0 ? p.X : p.SKIP) + tb;
+    __half* yo = Yout + tb;
+    __half* so = p.S16 + tb;
+    const bool read_old = q == 0 || l > 0;
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
 #pragma unroll
-      for (int e = 0; e < 64; e += 2) {
-        const int r = acc_row(wtid, e), col = hh * 128 + acc_col(wtid, e);
-        if (t0 + r >= p.T) continue;
-        const float a0 = hh ? c1[e] : c0[e], a1 = hh ? c1[e + 1] : c0[e + 1];
-        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
-        const size_t off = (fbase + r) * kC + col;
-        if (q == 0) {
-          float2 xv = *reinterpret_cast<const float2*>(p.X + off);
-          xv.x = (xv.x + (a0 + bb.x)) * 0.70710678118654752440f;
-          xv.y = (xv.y + (a1 + bb.y)) * 0.70710678118654752440f;
-          *reinterpret_cast<float2*>(p.X + off) = xv;
-          if (!last) {
-            const float2 dv = __ldg(reinterpret_cast<const float2*>(dnext + col));
-            const float ya = xv.x + dv.x, yb = xv.y + dv.y;
-            const __half2 hy = __floats2half2_rn(ya, yb);
-            *reinterpret_cast<__half2*>(Yout + off) = hy;
-            if (p.ylo) {
-              const float2 hf = __half22float2(hy);
-              *reinterpret_cast<__half2*>(Yout + p.plane + off) = __floats2half2_rn(ya - hf.x, yb - hf.y);
+      for (int e0 = 0; e0 < 64; e0 += 2 * kEpiBatch) {
+        float2 old[kEpiBatch];
+#pragma unroll
+        for (int j = 0; j < kEpiBatch; ++j) {
+          const int e = e0 + 2 * j, o = ((e & 2) ? 8 * kC : 0) + hh * 128 + (e >> 2) * 8;
+          old[j] = make_float2(0.f, 0.f);
+          if (read_old && ((e & 2) ? ok8 : ok0)) old[j] = *reinterpret_cast<const float2*>(src + o);
+        }
+#pragma unroll
+        for (int j = 0; j < kEpiBatch; ++j) {
+          const int e = e0 + 2 * j, c = hh * 128 + (e >> 2) * 8, o = ((e & 2) ? 8 * kC : 0) + c;
+          if (!((e & 2) ? ok8 : ok0)) continue;
+          const float a0 = hh ? c1[e] : c0[e], a1 = hh ? c1[e + 1] : c0[e + 1];
+          const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + c));
+          if (q == 0) {
+            float2 xv = old[j];
+            xv.x = (xv.x + (a0 + bb.x)) * 0.70710678118654752440f;
+            xv.y = (xv.y + (a1 + bb.y)) * 0.70710678118654752440f;
+            *reinterpret_cast<float2*>(dst + o) = xv;
+            if (!last) {
+              const float2 dv = __ldg(reinterpret_cast<const float2*>(dn + c));
+              const float ya = xv.x + dv.x, yb = xv.y + dv.y;
+              const __half2 hy = __floats2half2_rn(ya, yb);
+              *reinterpret_cast<__half2*>(yo + o) = hy;
+              if (p.ylo) {
+                const float2 hf = __half22float2(hy);
+                *reinterpret_cast<__half2*>(yo + p.plane + o) = __floats2half2_rn(ya - hf.x, yb - hf.y);
+              }
             }
-          }
-        } else {
-          float2 sk = make_float2(a0 + bb.x, a1 + bb.y);
-          if (l > 0) {
-            const float2 old = *reinterpret_cast<const float2*>(p.SKIP + off);
-            sk.x = old.x + sk.x;
-            sk.y = old.y + sk.y;
-          }
-          *reinterpret_cast<float2*>(p.SKIP + off) = sk;
-          if (last) {
-            const float sa = sk.x * p.inv_sqrt_l, sb = sk.y * p.inv_sqrt_l;
-            const __half2 hs = __floats2half2_rn(sa, sb);
-            const float2 hf = __half22float2(hs);
-            *reinterpret_cast<__half2*>(p.S16 + off) = hs;
-            *reinterpret_cast<__half2*>(p.S16 + p.plane + off) = __floats2half2_rn(sa - hf.x, sb - hf.y);
+          } else {
+            float2 sk = make_float2(a0 + bb.x, a1 + bb.y);
+            if (l > 0) {
+              sk.x = old[j].x + sk.x;
+              sk.y = old[j].y + sk.y;
+            }
+            *reinterpret_cast<float2*>(dst + o) = sk;
+            if (last) {
+              const float sa = sk.x * p.inv_sqrt_l, sb = sk.y * p.inv_sqrt_l;
+              const __half2 hs = __floats2half2_rn(sa, sb);
+              const float2 hf = __half22float2(hs);
+              *reinterpret_cast<__half2*>(so + o) = hs;
+              *reinterpret_cast<__half2*>(so + p.plane + o) = __floats2half2_rn(sa - hf.x, sb - hf.y);
+            }
           }
         }
       }
     }
+    stamp(p, layer_slot(p, l, 5 + 2 * q));
   }
 }
 
@@ -330,6 +393,7 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, uint8_t* buf
     };
     auto adesc1 = [&](int, uint8_t* bf) { return wg_desc(smem_u32(bf + kWBytes + wg * kABytes)); };
     gemm<2>(c0, c1, 4 * HP, load1, adesc1, buf0, buf1);
+    stamp(p, head_slot(p, 0));
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
 #pragma unroll
@@ -344,6 +408,7 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, uint8_t* buf
         *reinterpret_cast<__half2*>(zb + 4 * kABytes + off) = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
       }
     }
+    stamp(p, head_slot(p, 1));
     // H2: eps (before bias) = h . W_out^T, N = 128 (rows >= M of the packed tile are zero)
     auto load2 = [&](int s, uint8_t* bf) {
       const int kb = s / HP, ps = s % HP;
@@ -355,6 +420,7 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, uint8_t* buf
       return wg_desc(smem_u32(zb + (pass_aplane(ps) * 4 + kb) * kABytes));
     };
     gemm<1>(c0, c1, 4 * HP, load2, adesc2, buf0, buf1);
+    stamp(p, head_slot(p, 2));
   }
 
   // ---- mel phase: eps, sampler update, x_in operand of the input projection ----
@@ -418,6 +484,7 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, uint8_t* buf
       *reinterpret_cast<__half2*>(zb + 4 * kABytes + off) = __floats2half2_rn(xv[0] - hf.x, xv[1] - hf.y);
     }
   }
+  stamp(p, head_slot(p, 3));
   if (!do_in) return;
 
   // ---- input projection: x0 = relu(x_in . W_in^T + b_in) -> X ; y0 = split(x0 + d_0) -> Y buffer 0 ----
@@ -430,6 +497,7 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, uint8_t* buf
     return wg_desc(smem_u32(zb + (pass_aplane(ps) * 4 + kb) * kABytes));
   };
   gemm<2>(c0, c1, 2 * HP, load3, adesc3, buf0, buf1);
+  stamp(p, head_slot(p, 4));
   const float* d0 = p.d0 + static_cast<size_t>(b) * p.d0_row_stride;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
@@ -451,6 +519,7 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, uint8_t* buf
       }
     }
   }
+  stamp(p, head_slot(p, 5));
 }
 
 template <int NWG>
@@ -460,9 +529,13 @@ __global__ void __launch_bounds__(NWG * 128, 1) k_hp_step(const __grid_constant_
   uint8_t* buf0 = base;
   uint8_t* buf1 = base + StepCfg<NWG>::STAGE;
   uint8_t* zb = base + 2 * StepCfg<NWG>::STAGE + (threadIdx.x >> 7) * kZBytes;
+  stamp(p, 0);
   for (int l = p.l0; l < p.l1; ++l) {
     for (int u = blockIdx.x; u < p.units; u += gridDim.x) layer_tile<NWG>(p, l, u, buf0, buf1, zb);
-    if (l + 1 < p.l1 || p.head_flags) cg::this_grid().sync();
+    if (l + 1 < p.l1 || p.head_flags) {
+      cg::this_grid().sync();
+      stamp(p, layer_slot(p, l, 8));
+    }
   }
   if (p.head_flags)
     for (int u = blockIdx.x; u < p.units; u += gridDim.x) head_tile<NWG>(p, u, buf0, buf1, zb);
@@ -699,6 +772,8 @@ static HpParams base_params(dsx_handle* h, const Geom& g, int rows) {
   prm.bs = m.skip_b;
   prm.bf = m.fin_b;
   prm.bin = m.in_b;
+  prm.trace = h->trace_on ? reinterpret_cast<long long*>(h->trace_dev) : nullptr;
+  prm.trace_ctas = 2 * h->sm_count;
   return prm;
 }
 

@@ -140,6 +140,8 @@ struct dsx_handle {
   int stack_mode = 1;               // 1: all residual layers of an evaluation in one launch
   std::vector<cudaEvent_t> prof_events;   // pairs (start, stop), prof_used of them recorded
   size_t prof_used = 0;
+  int64_t* trace_dev = nullptr;     // dsx_debug_trace: [2 * sm_count][DSX_TRACE_SLOTS] phase stamps of the step kernel
+  bool trace_on = false;
 };
 
 namespace dsx {

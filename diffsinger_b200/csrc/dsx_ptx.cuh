@@ -59,6 +59,22 @@ __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_grou
 template <int N>
 __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
+// ---- global memory hints ------------------------------------------------------------------------
+// bytes (a multiple of 16) at a 16-byte aligned global address -> L2, asynchronously; nothing waits for it
+__device__ __forceinline__ void prefetch_l2(const void* src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+}
+// load of data that is read once and never written by the kernel: no L1 allocation, first out of L2.  Not volatile, so
+// the compiler may move it across the stores around it.
+__device__ __forceinline__ float2 ld_stream_f2(const float* src) {
+  float2 v;
+  asm("{\n\t.reg .b64 pol;\n\tcreatepolicy.fractional.L2::evict_first.b64 pol, 1.0;\n\t"
+      "ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f32 {%0, %1}, [%2], pol;\n\t}"
+      : "=f"(v.x), "=f"(v.y)
+      : "l"(src));
+  return v;
+}
+
 // ---- math ---------------------------------------------------------------------------------------
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;

@@ -194,7 +194,8 @@ enum {
 int dsx_set_option(dsx_handle* h, int what, int64_t value);
 enum {
   DSX_OPT_TC_CTA_GROUP = 0, /* accepts 2 only; kept for ABI compatibility, no effect */
-  DSX_OPT_CP_PREFETCH = 1,  /* accepted and ignored (kept for ABI compatibility): the sm_90 kernels have no prefetch stage */
+  DSX_OPT_CP_PREFETCH = 1,  /* accepted and ignored (kept for ABI compatibility): the step kernel always prefetches the
+                               epilogue operands (conditioner projection, x, skip) into L2 */
   DSX_OPT_PROFILE = 2,      /* 1: bracket the residual-layer kernel(s) of every evaluation with CUDA events; 2: bracket the
                                head / update kernel of every DDPM step instead; 0: off.  Setting it resets the sums */
   DSX_OPT_STACK_MODE = 3,   /* 1 (default): all residual layers of an evaluation in ONE persistent cooperative launch (grid-wide
@@ -217,7 +218,21 @@ enum {
  * buffers after a dsx_diffnet_forward.  which: 0 = residual stream after the last layer
  * executed, 1 = skip sum.  out: [B, T, C] contiguous. */
 int dsx_debug_read(dsx_handle* h, int which, float* out, int B, int T, void* stream);
-/* Kept for ABI compatibility: the sm_90 kernels record no clock64 timeline; always returns DSX_E_INVALID. */
+/* Phase timeline of the step kernel (k_hp_step).  enable = 1 clears the handle's trace buffer and makes every later
+ * launch of the step kernel record into it; enable = 0 stops recording and, when out_host is not NULL, synchronises the
+ * device and copies the buffer out.  Each launch overwrites the slots it reaches, so the buffer holds the last launch.
+ * out_host: int64 [2 * DSX_INFO_SM_COUNT rows][DSX_TRACE_SLOTS], row = CTA (blockIdx.x), %globaltimer in ns, 0 = not
+ * reached.  Thread 0 of each CTA stamps when it finishes a phase; a CTA that walks over several tiles of a layer
+ * (more tiles than CTAs) overwrites the layer's slots, so they time its last tile only:
+ *   slot 0                                launch entry
+ *   slot 1 + 9 i + k, i = layer - l0      k = 0 / 2: GEMM1 chunk 0 / 1 end, 1 / 3: gate epilogue 0 / 1 end,
+ *                                         4 / 6: GEMM2 residual / skip half end, 5 / 7: residual / skip epilogue end,
+ *                                         8: exit of the grid barrier after the layer (0 when no barrier
+ *                                         follows: the last layer of a launch without a head)
+ *   slot 1 + 9 n + k, n = layers launched head: k = 0 H1 GEMM end, 1 H1 epilogue end, 2 H2 GEMM end, 3 mel update end,
+ *                                         4 input projection GEMM end, 5 input projection epilogue end
+ * Slots past DSX_TRACE_SLOTS are not recorded (at most 27 layers per launch). */
+enum { DSX_TRACE_SLOTS = 256 };
 int dsx_debug_trace(dsx_handle* h, int enable, int64_t* out_host);
 /* Run only layers [0, n_layers) in the next dsx_diffnet_forward calls (<0: all). */
 int dsx_debug_set_layer_limit(dsx_handle* h, int n_layers);
