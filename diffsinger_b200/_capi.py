@@ -23,6 +23,7 @@ SYMBOLS = (
     "dsx_version", "dsx_last_error", "dsx_create", "dsx_destroy", "dsx_load_diffnet", "dsx_set_schedule",
     "dsx_diffnet_forward", "dsx_sample_ddpm", "dsx_sample_plms", "dsx_infer", "dsx_infer_host", "dsx_get_info",
     "dsx_set_option", "dsx_set_cond", "dsx_plms_update", "dsx_debug_read", "dsx_debug_trace", "dsx_debug_set_layer_limit", "dsx_selftest",
+    "dsx_hifigan_create", "dsx_hifigan_destroy", "dsx_hifigan_load", "dsx_hifigan_forward",
 )
 
 
@@ -43,6 +44,20 @@ class DiffNetParams(ctypes.Structure):
                 ("dil_w", _fpp), ("dil_b", _fpp), ("dif_w", _fpp), ("dif_b", _fpp), ("cond_w", _fpp),
                 ("cond_b", _fpp), ("out_w", _fpp), ("out_b", _fpp), ("skip_w", _fp), ("skip_b", _fp),
                 ("fin_w", _fp), ("fin_b", _fp)]
+
+
+class HifiganConfig(ctypes.Structure):
+    _fields_ = [("num_upsamples", ctypes.c_int), ("upsample_rates", ctypes.c_int * 4),
+                ("upsample_kernel_sizes", ctypes.c_int * 4), ("upsample_initial_channel", ctypes.c_int),
+                ("resblock", ctypes.c_int), ("num_kernels", ctypes.c_int), ("resblock_kernel_sizes", ctypes.c_int * 3),
+                ("resblock_dilation_sizes", (ctypes.c_int * 3) * 3), ("audio_sample_rate", ctypes.c_int),
+                ("use_pitch_embed", ctypes.c_int)]
+
+
+class HifiganParams(ctypes.Structure):
+    _fields_ = [("conv_pre_w", _fp), ("conv_pre_g", _fp), ("conv_pre_b", _fp), ("ups_w", _fpp), ("ups_g", _fpp),
+                ("ups_b", _fpp), ("rb_w", _fpp), ("rb_g", _fpp), ("rb_b", _fpp), ("noise_w", _fpp), ("noise_b", _fpp),
+                ("source_w", _fp), ("source_b", _fp), ("conv_post_w", _fp), ("conv_post_g", _fp), ("conv_post_b", _fp)]
 
 
 if not os.path.exists(LIB_PATH):
@@ -72,9 +87,14 @@ lib.dsx_debug_read.argtypes = [_vp, _i, _vp, _i, _i, _vp]
 lib.dsx_debug_set_layer_limit.argtypes = [_vp, _i]
 lib.dsx_debug_trace.argtypes = [_vp, _i, _vp]
 lib.dsx_selftest.argtypes = [_i, _i, ctypes.c_char_p, _i]
+lib.dsx_hifigan_create.argtypes = [_i, ctypes.POINTER(HifiganConfig), ctypes.POINTER(_vp)]
+lib.dsx_hifigan_destroy.argtypes = [_vp]
+lib.dsx_hifigan_destroy.restype = None
+lib.dsx_hifigan_load.argtypes = [_vp, ctypes.POINTER(HifiganParams), _vp]
+lib.dsx_hifigan_forward.argtypes = [_vp, _vp, Strides, _vp, _vp, _vp, _vp, _u64, _i, _i, _vp, _vp]
 for _n in SYMBOLS:
-    if getattr(lib, _n).restype is ctypes.c_int or _n not in ("dsx_last_error", "dsx_destroy"):
-        if _n not in ("dsx_last_error", "dsx_destroy"):
+    if getattr(lib, _n).restype is ctypes.c_int or _n not in ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy"):
+        if _n not in ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy"):
             getattr(lib, _n).restype = _i
 
 

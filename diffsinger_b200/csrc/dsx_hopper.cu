@@ -190,9 +190,6 @@ __device__ __forceinline__ void gemm(float (&c0)[64], float (&c1)[64], int nst, 
   }
 }
 
-// accumulator element e of thread (warp w of the warpgroup, lane): row and column inside the 64 x 128 block
-__device__ __forceinline__ int acc_row(int wtid, int e) { return ((wtid >> 5) << 4) + ((wtid & 31) >> 2) + ((e & 2) ? 8 : 0); }
-__device__ __forceinline__ int acc_col(int wtid, int e) { return ((e >> 2) << 3) + ((wtid & 3) << 1) + (e & 1); }
 // byte offset of (row r, channel k) in a [4 k-blocks] K-major swizzled operand
 __device__ __forceinline__ uint32_t opnd_off(int r, int k) {
   return static_cast<uint32_t>((k >> 6) * kABytes) + sw128(r, (k & 63) >> 3) + (k & 7) * 2;

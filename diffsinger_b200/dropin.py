@@ -10,6 +10,12 @@ replaces, without editing any reference file,
 whose ``forward(infer=True)`` runs the sm_90a sampler, and the ``'wavenet'`` entry of every ``DIFF_DECODERS`` registry by
 ``diffsinger_b200.DiffNet``.  Construction arguments, parameter / buffer names, ``p_losses`` and the returned ``ret`` dict
 are the reference's own, so the task files run unchanged.
+
+    dropin.install_vocoder()
+
+replaces ``modules.hifigan.hifigan.HifiGanGenerator`` -- and the name bound from it in ``vocoders.*`` modules already
+imported -- by ``diffsinger_b200.HifiGanGenerator``, so ``vocoders/hifigan.py:load_model`` (strict ``load_state_dict``,
+``remove_weight_norm``, ``.to(device)``) and ``spec2wav`` run the vocoder on dsx unchanged.
 """
 import importlib
 import sys
@@ -137,3 +143,28 @@ def uninstall():
             cur = getattr(mod, attr, None)
             if cur is not None and id(cur) in back:
                 setattr(mod, attr, back[id(cur)])
+
+
+_vocoder = {}
+
+
+def install_vocoder():
+    from .vocoder import HifiGanGenerator
+    mod = importlib.import_module("modules.hifigan.hifigan")
+    _vocoder.setdefault("ref", mod.HifiGanGenerator)
+    _swap_vocoder(_vocoder["ref"], HifiGanGenerator)
+    return HifiGanGenerator
+
+
+def uninstall_vocoder():
+    if _vocoder:
+        from .vocoder import HifiGanGenerator
+        _swap_vocoder(HifiGanGenerator, _vocoder["ref"])
+
+
+def _swap_vocoder(old, new):
+    for name, mod in list(sys.modules.items()):
+        if mod is None or not (name == "modules.hifigan.hifigan" or name.startswith("vocoders.")):
+            continue
+        if getattr(mod, "HifiGanGenerator", None) is old:
+            mod.HifiGanGenerator = new

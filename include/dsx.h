@@ -243,6 +243,73 @@ int dsx_debug_set_layer_limit(dsx_handle* h, int n_layers);
  * report (may be NULL): host buffer receiving a text report. */
 int dsx_selftest(int device, int which, char* report, int report_bytes);
 
+/* ---- HiFi-GAN (NSF) vocoder: mel (+ f0) -> waveform --------------------------------------------------------------
+ * Replaces: modules/hifigan/hifigan.py:104-171 (HifiGanGenerator with ResBlock1 / ResBlock2) and the NSF harmonic source
+ * of modules/parallel_wavegan/models/source.py (SineGen, SourceModuleHnNSF), as vocoders/hifigan.py runs them.
+ * Convolutions run on tensor cores with fp16 operands and fp32 accumulation; the residual stream, the multi-receptive-field
+ * sum, the harmonic source and the output stay fp32.  A vocoder handle is independent of the sampler handles. */
+typedef struct dsx_hifigan dsx_hifigan;
+
+/* The generator's hyper-parameters (the `h` dict of HifiGanGenerator.__init__). */
+typedef struct {
+  int num_upsamples;                   /* len(upsample_rates): 1..4                                                     */
+  int upsample_rates[4];               /* u_i >= 1                                                                      */
+  int upsample_kernel_sizes[4];        /* k_i >= u_i, k_i % u_i == 0 and k_i - u_i even                                 */
+  int upsample_initial_channel;        /* C0, divisible by 2^num_upsamples                                              */
+  int resblock;                        /* 1 (ResBlock1: 3 dilated / plain conv pairs) or 2 (ResBlock2: 2 dilated convs) */
+  int num_kernels;                     /* len(resblock_kernel_sizes): 1..3                                              */
+  int resblock_kernel_sizes[3];        /* odd                                                                           */
+  int resblock_dilation_sizes[3][3];   /* ResBlock2 uses the first two of each row                                      */
+  int audio_sample_rate;               /* Hz, > 0                                                                       */
+  int use_pitch_embed;                 /* 1: the NSF source and noise_convs exist (f0 may be passed to the forward)      */
+} dsx_hifigan_config;
+
+/* Parameters, fp32 device pointers, each tensor contiguous in the reference's state-dict layout.  A weight-normalised
+ * conv passes weight_v as `*_w` and weight_g as `*_g`; a plain conv (after remove_weight_norm) passes `.weight` and
+ * `*_g` = NULL.  Per-module arrays are HOST arrays of device pointers:
+ *   ups_*:    num_upsamples entries (ups.i, ConvTranspose1d [C_in, C_out, k]);
+ *   rb_*:     num_upsamples * num_kernels blocks in resblocks.* order, each block's convs in state-dict order --
+ *             ResBlock1: convs1.0, convs1.1, convs1.2, convs2.0, convs2.1, convs2.2; ResBlock2: convs.0, convs.1;
+ *   noise_*:  num_upsamples entries (noise_convs.i, plain Conv1d [C, 1, k]); NULL without use_pitch_embed. */
+typedef struct {
+  const float* conv_pre_w;
+  const float* conv_pre_g;
+  const float* conv_pre_b;
+  const float* const* ups_w;
+  const float* const* ups_g;
+  const float* const* ups_b;
+  const float* const* rb_w;
+  const float* const* rb_g;
+  const float* const* rb_b;
+  const float* const* noise_w;
+  const float* const* noise_b;
+  const float* source_w;               /* m_source.l_linear.weight [1, 9] (use_pitch_embed) */
+  const float* source_b;               /* m_source.l_linear.bias   [1]                      */
+  const float* conv_post_w;
+  const float* conv_post_g;
+  const float* conv_post_b;
+} dsx_hifigan_params;
+
+/* Replaces: HifiGanGenerator(h).  Validates the configuration (DSX_E_INVALID). */
+int dsx_hifigan_create(int device, const dsx_hifigan_config* cfg, dsx_hifigan** out);
+void dsx_hifigan_destroy(dsx_hifigan* h);
+
+/* Replaces: load_state_dict (+ remove_weight_norm).  Applies the weight norm g * v / ||v|| (norm over every dim but 0;
+ * for ConvTranspose1d dim 0 is C_in) and packs fp16 tensor-core tiles.  Call again after every change of the weights. */
+int dsx_hifigan_load(dsx_hifigan* h, const dsx_hifigan_params* p, void* stream);
+
+/* Replaces: HifiGanGenerator.forward(mel, f0) as vocoders/hifigan.py:spec2wav calls it, one utterance at a time.
+ *   mel      logically [B, 80, T], any element strides ms (dsx_infer's [B, T, 80] output feeds it untransposed);
+ *   f0       [B, T] in Hz (0 = unvoiced), or NULL for the mel-only path (required NULL without use_pitch_embed);
+ *   lengths  int32 [B] frames, or NULL for all T: utterance b is computed exactly as if it were alone at lengths[b]
+ *            frames, and wav samples from lengths[b] * hop on are 0 (hop = product of the upsample rates);
+ *   phase0   [B, 9] initial phases of the harmonics (harmonic 0 is always 0), or NULL: Philox4x32-10 uniforms of `seed`;
+ *   src_noise [B, T * hop, 9] the source's additive gaussian noise, or NULL: Philox4x32-10 normals of `seed`;
+ *   wav      [B, 1, T * hop] contiguous. */
+int dsx_hifigan_forward(dsx_hifigan* h, const float* mel, dsx_strides ms, const float* f0, const int* lengths,
+                        const float* phase0, const float* src_noise, uint64_t seed, int B, int T, float* wav,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif
