@@ -24,7 +24,9 @@ SYMBOLS = (
     "dsx_diffnet_forward", "dsx_sample_ddpm", "dsx_sample_plms", "dsx_infer", "dsx_infer_host", "dsx_get_info",
     "dsx_set_option", "dsx_set_cond", "dsx_plms_update", "dsx_debug_read", "dsx_debug_trace", "dsx_debug_set_layer_limit", "dsx_selftest",
     "dsx_hifigan_create", "dsx_hifigan_destroy", "dsx_hifigan_load", "dsx_hifigan_forward",
+    "dsx_pe_create", "dsx_pe_destroy", "dsx_pe_load", "dsx_pe_forward",
 )
+_VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy")
 
 
 class DsxError(RuntimeError):
@@ -60,6 +62,21 @@ class HifiganParams(ctypes.Structure):
                 ("source_w", _fp), ("source_b", _fp), ("conv_post_w", _fp), ("conv_post_g", _fp), ("conv_post_b", _fp)]
 
 
+class PeConfig(ctypes.Structure):
+    _fields_ = [("n_mel_bins", ctypes.c_int), ("hidden", ctypes.c_int), ("predictor_hidden", ctypes.c_int),
+                ("predictor_kernel", ctypes.c_int), ("conv_layers", ctypes.c_int), ("causal", ctypes.c_int),
+                ("pitch_norm", ctypes.c_int), ("f0_mean", ctypes.c_float), ("f0_std", ctypes.c_float),
+                ("use_uv", ctypes.c_int)]
+
+
+class PeParams(ctypes.Structure):
+    _fields_ = [("prenet_w", _fpp), ("prenet_b", _fpp), ("bn_w", _fpp), ("bn_b", _fpp), ("bn_mean", _fpp),
+                ("bn_var", _fpp), ("prenet_out_w", _fp), ("prenet_out_b", _fp), ("enc_in_w", _fp), ("enc_in_b", _fp),
+                ("enc_w", _fpp), ("enc_b", _fpp), ("gn_w", _fpp), ("gn_b", _fpp), ("enc_out_w", _fp), ("enc_out_b", _fp),
+                ("pred_w", _fpp), ("pred_b", _fpp), ("ln_w", _fpp), ("ln_b", _fpp), ("linear_w", _fp), ("linear_b", _fp),
+                ("pos_embed_alpha", _fp)]
+
+
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"dsx CUDA library not found at {LIB_PATH}; build it with `python diffsinger_b200/build.py` "
@@ -92,10 +109,14 @@ lib.dsx_hifigan_destroy.argtypes = [_vp]
 lib.dsx_hifigan_destroy.restype = None
 lib.dsx_hifigan_load.argtypes = [_vp, ctypes.POINTER(HifiganParams), _vp]
 lib.dsx_hifigan_forward.argtypes = [_vp, _vp, Strides, _vp, _vp, _vp, _vp, _u64, _i, _i, _vp, _vp]
+lib.dsx_pe_create.argtypes = [_i, ctypes.POINTER(PeConfig), ctypes.POINTER(_vp)]
+lib.dsx_pe_destroy.argtypes = [_vp]
+lib.dsx_pe_destroy.restype = None
+lib.dsx_pe_load.argtypes = [_vp, ctypes.POINTER(PeParams), _vp]
+lib.dsx_pe_forward.argtypes = [_vp, _vp, Strides, _i, _i, _vp, _vp, _vp]
 for _n in SYMBOLS:
-    if getattr(lib, _n).restype is ctypes.c_int or _n not in ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy"):
-        if _n not in ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy"):
-            getattr(lib, _n).restype = _i
+    if _n not in _VOID:
+        getattr(lib, _n).restype = _i
 
 
 def check(rc, what=""):

@@ -1,0 +1,765 @@
+// Pitch extractor on sm_90a: mel [B, T, 80] -> pitch_pred [B, T, 2] and the denormalised f0 [B, T]
+// (modules/fastspeech/pe.py:119-149: Prenet, ConvStacks with GroupNorm, PitchPredictor, utils/pitch_utils.py:denorm_f0).
+//
+// Every conv and linear is one implicit GEMM on wgmma (k_pe_conv).  Activations are frames-major fp16 [B][T][C]; row m of
+// the GEMM is a frame, the K axis is (tap j, input channel c), and tap j reads frame m + tap0 + j, zero outside [0, T).
+// That one rule is the prenet's zero padding (tap0 = -2), the PitchPredictor's ConstantPad1d 'SAME' (tap0 = -(k-1)/2) and
+// 'LEFT' (tap0 = -(k-1)), and a linear (one tap).  A CTA covers 64 frames x ALL output channels (N <= 256), so a row's
+// normalisation and the head's P -> 2 linear run in the epilogue from registers: one warpgroup up to N = 128; at N = 256
+// two warpgroups share the A tile, each with its 128 columns (m64n128) and a row reduction through shared memory.  Operands reach shared memory by cp.async in the 128-byte-swizzled layout of dsx_ptx.cuh, double buffered per
+// 64-wide K chunk.  Epilogues by mode:
+//   PE_PRENET  bias, ReLU, BatchNorm (eval: per-channel scale and shift packed at load), padding mask -> fp16
+//   PE_LINEAR  bias, optional padding mask -> fp32 and / or fp16
+//   PE_GN      bias -> fp32 pre-norm values, plus per-tile, per-16-channel-group (count, mean, M2) partials
+//   PE_LN      bias, ReLU, LayerNorm over the row (two-pass, reduced over the accumulator quad) -> fp16
+//   PE_HEAD    PE_LN, then Linear(P, 2) from registers -> pitch_pred, and f0 with the uv and padding rules
+// GroupNorm statistics span a whole utterance, so k_pe_gn merges the tile partials in a fixed order (Chan's formula, no
+// atomics: deterministic) and applies x += relu(gn(y)).  The position embedding's positions are a scan per utterance
+// (k_pe_scan); k_pe_posadd adds alpha * table[pos] with the table evaluated in fp32 on the fly.
+#include <math.h>
+#include <stdio.h>
+
+#include <algorithm>
+
+#include "dsx_internal.h"
+#include "dsx_ptx.cuh"
+
+namespace dsx {
+namespace {
+
+constexpr int kPeMel = 80;
+constexpr int kPeRows = 64;           // frames per CTA
+constexpr int kPePrenetLayers = 3, kPePredLayers = 5, kPeEncKernel = 5, kPePrenetKernel = 5;
+constexpr int kPeMaxConvLayers = 16;
+constexpr float kBnEps = 1e-5f, kGnEps = 1e-5f, kLnEps = 1e-12f;
+
+enum { PE_PRENET = 0, PE_LINEAR = 1, PE_GN = 2, PE_LN = 3, PE_HEAD = 4 };
+enum { PE_MASK = 1, PE_OUT32 = 2, PE_OUT16 = 4 };
+
+struct PePacked {
+  int cin = 0, n = 0, taps = 0, tap0 = 0, nt = 0, kc = 0;
+  __half* w = nullptr;         // [kc][nt][64] fp16, K index = tap * cin + channel, zero padded
+  float* b = nullptr;          // [nt]
+  float* s = nullptr;          // per-channel scale (BatchNorm, GroupNorm / LayerNorm weight) [n], or null
+  float* t = nullptr;          // per-channel shift [n], or null
+};
+
+struct PeConvArgs {
+  const __half* x;             // [B][T][cin]
+  int cin, taps, tap0, kc;
+  const __half* w;
+  const float* bias;
+  int n, T, mode, flags;
+  const float* scale;          // PE_PRENET: BN scale; PE_LN / PE_HEAD: LayerNorm weight
+  const float* shift;          // PE_PRENET: BN shift; PE_LN / PE_HEAD: LayerNorm bias
+  const uint8_t* pad;          // [B][T] 1 = padding frame
+  float* o32;                  // [B][T][n]
+  __half* o16;                 // [B][T][n]
+  float* stats;                // PE_GN: [B][mtiles][n / 16][3]
+  int mtiles;
+  const float* hw;             // PE_HEAD: linear.weight [2][n] and bias [2]
+  const float* hb;
+  float* pitch;                // [B][T][2] or null
+  float* f0;                   // [B][T] or null
+  int pitch_norm, use_uv;
+  float f0_mean, f0_std;
+};
+
+template <int NT>
+struct PeShape {
+  static constexpr int WG = NT > 128 ? 2 : 1;      // warpgroups per CTA; each owns NH columns of the same 64 rows
+  static constexpr int NH = NT / WG;
+};
+
+template <int NT>
+constexpr int pe_smem() { return 2 * (kPeRows * 128 + NT * 128) + 1024; }
+
+// sum over the 4 threads of an accumulator quad (they hold the same two rows)
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
+}
+
+template <int NT>
+__global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvArgs p) {
+  constexpr int NH = PeShape<NT>::NH, WG = PeShape<NT>::WG, NTHR = 128 * WG;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  constexpr int kA = kPeRows * 128, kB = NT * 128, kStage = kA + kB;
+  __shared__ float red[4 * WG][16];
+  __shared__ float gmean[16];
+  __shared__ float xrow[WG][kPeRows];   // per-warpgroup row partials of the LayerNorm / head reductions
+  const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127, b = blockIdx.y, m0 = blockIdx.x * kPeRows;
+  const int T = p.T;
+
+  auto load = [&](int s, uint8_t* buf) {
+    const uint32_t da = smem_u32(buf), db = smem_u32(buf + kA);
+    for (int i = tid; i < kPeRows * 8; i += NTHR) {
+      const int r = i >> 3, c = i & 7;
+      const int kk = s * 64 + c * 8, j = kk / p.cin, ch = kk - j * p.cin;
+      const int src = m0 + r + p.tap0 + j;
+      const bool valid = j < p.taps && src >= 0 && src < T;
+      cp16(da + sw128(r, c), p.x + (static_cast<size_t>(b) * T + (valid ? src : 0)) * p.cin + (valid ? ch : 0), valid);
+    }
+    const __half* wsrc = p.w + static_cast<size_t>(s) * NT * 64;
+    for (int i = tid; i < NT * 8; i += NTHR) {
+      const int r = i >> 3, c = i & 7;
+      cp16(db + sw128(r, c), wsrc + r * 64 + c * 8, true);
+    }
+  };
+
+  float acc[NH / 2];
+#pragma unroll
+  for (int e = 0; e < NH / 2; ++e) acc[e] = 0.f;
+  load(0, smem);
+  cp_commit();
+#pragma unroll 1
+  for (int s = 0; s < p.kc; ++s) {
+    uint8_t* cur = smem + (s & 1) * kStage;
+    if (s + 1 < p.kc) {
+      load(s + 1, smem + ((s + 1) & 1) * kStage);
+      cp_commit();
+      cp_wait<1>();
+    } else {
+      cp_wait<0>();
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    const uint64_t da = wg_desc(smem_u32(cur)), db = wg_desc(smem_u32(cur + kA + wg * NH * 128));
+    wg_fence();
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4) wgmma_f16<NH>(acc, da + 2 * k4, db + 2 * k4, 1);
+    wg_commit();
+    wg_wait0();
+#pragma unroll
+    for (int e = 0; e < NH / 2; ++e) asm volatile("" : "+f"(acc[e])::"memory");
+    __syncthreads();
+  }
+
+  // ---- epilogue: thread wtid holds rows r0 = acc_row(wtid, 0) (e & 2 == 0) and r0 + 8 (e & 2 != 0) ----
+  const int n = p.n, c0 = wg * NH;
+  const int r0 = acc_row(wtid, 0);
+  const int mrow[2] = {m0 + r0, m0 + r0 + 8};
+  const size_t rbase = static_cast<size_t>(b) * T;
+  // sum of the two rows' values over all n columns: the quad, then (two warpgroups) both halves in a fixed order
+  auto row_sum = [&](float& s0, float& s1) {
+    s0 = quad_sum(s0);
+    s1 = quad_sum(s1);
+    if (WG > 1) {
+      if ((wtid & 3) == 0) {
+        xrow[wg][r0] = s0;
+        xrow[wg][r0 + 8] = s1;
+      }
+      __syncthreads();
+      s0 = xrow[0][r0] + xrow[1][r0];
+      s1 = xrow[0][r0 + 8] + xrow[1][r0 + 8];
+      __syncthreads();
+    }
+  };
+  // bias (+ ReLU) in place; columns >= n stay 0 (zero weights and bias)
+#pragma unroll
+  for (int e = 0; e < NH / 2; ++e) {
+    const int col = c0 + acc_col(wtid, e);
+    float v = col < n ? acc[e] + __ldg(p.bias + col) : 0.f;
+    if (p.mode == PE_PRENET || p.mode == PE_LN || p.mode == PE_HEAD) v = fmaxf(v, 0.f);
+    acc[e] = v;
+  }
+
+  if (p.mode == PE_GN) {
+    // per 16-channel group: count, mean and M2 over the tile's valid rows, two passes, fixed reduction order.  Local
+    // group gl of this warpgroup (global group c0 / 16 + gl) is elements e in [8 gl, 8 gl + 8).
+    const int rows = min(kPeRows, T - m0);
+    const bool ok0 = r0 < rows, ok1 = r0 + 8 < rows;
+    const int warp = tid >> 5, lane = tid & 31;
+    const int groups = n / 16;
+#pragma unroll
+    for (int pass = 0; pass < 2; ++pass) {
+#pragma unroll
+      for (int gl = 0; gl < NH / 16; ++gl) {
+        const int g = c0 / 16 + gl;
+        float sum = 0.f;
+        const float mu = pass ? gmean[g] : 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const bool ok = (i & 2) ? ok1 : ok0;
+          const float d = acc[8 * gl + i] - mu;
+          sum += ok ? (pass ? d * d : d) : 0.f;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        if (lane == 0) red[warp][g] = sum;
+      }
+      __syncthreads();
+      if (tid < groups) {
+        const int w0 = (tid / (NH / 16)) * 4;
+        const float tot = ((red[w0][tid] + red[w0 + 1][tid]) + red[w0 + 2][tid]) + red[w0 + 3][tid];
+        const float cnt = static_cast<float>(rows * 16);
+        if (pass == 0) {
+          gmean[tid] = tot / cnt;
+        } else {
+          float* st = p.stats + ((static_cast<size_t>(b) * p.mtiles + blockIdx.x) * groups + tid) * 3;
+          st[0] = cnt;
+          st[1] = gmean[tid];
+          st[2] = tot;
+        }
+      }
+      __syncthreads();
+    }
+  }
+
+  if (p.mode == PE_LN || p.mode == PE_HEAD) {
+    const float inv_n = 1.f / static_cast<float>(n);
+    float s[2] = {0.f, 0.f};
+#pragma unroll
+    for (int e = 0; e < NH / 2; ++e) s[(e >> 1) & 1] += acc[e];
+    row_sum(s[0], s[1]);
+    const float mean0 = s[0] * inv_n, mean1 = s[1] * inv_n;
+    float q[2] = {0.f, 0.f};
+#pragma unroll
+    for (int e = 0; e < NH / 2; ++e) {
+      const int col = c0 + acc_col(wtid, e);
+      const float d = acc[e] - ((e & 2) ? mean1 : mean0);
+      q[(e >> 1) & 1] += col < n ? d * d : 0.f;
+    }
+    row_sum(q[0], q[1]);
+    const float rstd0 = 1.f / sqrtf(q[0] * inv_n + kLnEps), rstd1 = 1.f / sqrtf(q[1] * inv_n + kLnEps);
+#pragma unroll
+    for (int e = 0; e < NH / 2; ++e) {
+      const int col = c0 + acc_col(wtid, e);
+      const bool hi = e & 2;
+      acc[e] = col < n ? (acc[e] - (hi ? mean1 : mean0)) * (hi ? rstd1 : rstd0) * __ldg(p.scale + col) + __ldg(p.shift + col)
+                       : 0.f;
+    }
+  }
+
+  if (p.mode == PE_HEAD) {
+    float o[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][output]
+#pragma unroll
+    for (int e = 0; e < NH / 2; ++e) {
+      const int col = c0 + acc_col(wtid, e);
+      if (col >= n) continue;
+      const int r = (e >> 1) & 1;
+      o[r][0] = fmaf(acc[e], __ldg(p.hw + col), o[r][0]);
+      o[r][1] = fmaf(acc[e], __ldg(p.hw + n + col), o[r][1]);
+    }
+    row_sum(o[0][0], o[1][0]);
+    row_sum(o[0][1], o[1][1]);
+    if (wg != 0 || (wtid & 3) != 0) return;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float p0 = o[r][0] + __ldg(p.hb), p1 = o[r][1] + __ldg(p.hb + 1);
+      const int m = mrow[r];
+      if (m >= T) continue;
+      const size_t idx = rbase + m;
+      if (p.pitch) *reinterpret_cast<float2*>(p.pitch + idx * 2) = make_float2(p0, p1);
+      if (p.f0) {   // denorm_f0 (utils/pitch_utils.py:63-76)
+        float f = p.pitch_norm == 1 ? p0 * p.f0_std + p.f0_mean : exp2f(p0);
+        if (p.use_uv && p1 > 0.f) f = 0.f;
+        if (p.pad[idx]) f = 0.f;
+        p.f0[idx] = f;
+      }
+    }
+    return;
+  }
+
+  // element-wise tail: PE_PRENET (BN affine + mask), PE_LINEAR, PE_GN (pre-norm values), PE_LN -> stores
+#pragma unroll
+  for (int e = 0; e < NH / 2; e += 2) {
+    const int col = c0 + acc_col(wtid, e), m = mrow[(e >> 1) & 1];
+    if (col >= n || m >= T) continue;
+    const size_t idx = (rbase + m) * n + col;
+    float v0 = acc[e], v1 = acc[e + 1];
+    if (p.mode == PE_PRENET) {
+      v0 = fmaf(v0, __ldg(p.scale + col), __ldg(p.shift + col));
+      v1 = fmaf(v1, __ldg(p.scale + col + 1), __ldg(p.shift + col + 1));
+    }
+    if ((p.flags & PE_MASK) && p.pad[rbase + m]) v0 = v1 = 0.f;
+    if (p.flags & PE_OUT32) *reinterpret_cast<float2*>(p.o32 + idx) = make_float2(v0, v1);
+    if (p.flags & PE_OUT16) *reinterpret_cast<__half2*>(p.o16 + idx) = __floats2half2_rn(v0, v1);
+  }
+}
+
+// ---- operand pack --------------------------------------------------------------------------------
+// mel logically [B, T, 80] (any strides: b, c = bin, t) -> fp16 [B][T][80] and pad[b][t] = all 80 bins exactly 0
+// (pe.py:29 mel.abs().sum(-1) == 0, decided on the fp32 values).  One warp per frame.
+__global__ void k_pe_pack_mel(const float* mel, dsx_strides ms, int B, int T, __half* out, uint8_t* pad) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= B * T) return;
+  const int b = warp / T, t = warp - b * T;
+  const float* src = mel + b * ms.b + t * ms.t;
+  bool nz = false;
+  for (int c = lane; c < kPeMel; c += 32) {
+    const float v = src[c * ms.c];
+    nz |= v != 0.f;
+    out[static_cast<size_t>(warp) * kPeMel + c] = __float2half_rn(v);
+  }
+  const unsigned any = __ballot_sync(0xffffffffu, nz);
+  if (lane == 0) pad[warp] = any ? 0 : 1;
+}
+
+// ---- GroupNorm ---------------------------------------------------------------------------------
+// Merge the per-tile (count, mean, M2) of utterance b in tile order (Chan et al.), then x += relu(gn(y)) over kGnRows
+// frames per block: writes the fp32 residual and the fp16 operand of the next conv (pe.py:107-109, ConvBlock.forward).
+constexpr int kGnRows = 32;
+__global__ void __launch_bounds__(256) k_pe_gn(const float* y, const float* stats, int mtiles, const float* gw,
+                                               const float* gb, int T, int n, float* x, __half* x16) {
+  __shared__ float mean_s[16], rstd_s[16];
+  const int b = blockIdx.y, groups = n / 16, tid = threadIdx.x;
+  if (tid < groups) {
+    const float* st = stats + static_cast<size_t>(b) * mtiles * groups * 3 + tid * 3;
+    float na = st[0], ma = st[1], m2 = st[2];
+    for (int i = 1; i < mtiles; ++i) {
+      const float* q = st + static_cast<size_t>(i) * groups * 3;
+      const float nb = q[0], nn = na + nb, d = q[1] - ma;
+      ma += d * (nb / nn);
+      m2 += q[2] + d * d * (na * nb / nn);
+      na = nn;
+    }
+    mean_s[tid] = ma;
+    rstd_s[tid] = 1.f / sqrtf(m2 / na + kGnEps);
+  }
+  __syncthreads();
+  const int t0 = blockIdx.x * kGnRows, t1 = min(T, t0 + kGnRows);
+  const size_t base = (static_cast<size_t>(b) * T + t0) * n, cnt = static_cast<size_t>(t1 - t0) * n;
+  for (size_t i = tid; i < cnt; i += blockDim.x) {
+    const int c = static_cast<int>(i % n), g = c >> 4;
+    const float v = (y[base + i] - mean_s[g]) * rstd_s[g] * gw[c] + gb[c];
+    const float r = x[base + i] + fmaxf(v, 0.f);
+    x[base + i] = r;
+    x16[base + i] = __float2half_rn(r);
+  }
+}
+
+// ---- position embedding ------------------------------------------------------------------------
+// pos[b][t] = cumsum(x[b, :, 0] != 0)[t] * (x[b, t, 0] != 0) (utils/__init__.py:145-157, padding_idx 0).  One block per
+// utterance, kScanChunk frames per thread per pass.
+constexpr int kScanThreads = 1024, kScanChunk = 8;
+__global__ void __launch_bounds__(kScanThreads) k_pe_scan(const float* x, int T, int n, int* pos) {
+  __shared__ int sh[kScanThreads];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const float* xb = x + static_cast<size_t>(b) * T * n;
+  int carry = 0;
+  for (int base = 0; base < T; base += kScanThreads * kScanChunk) {
+    const int t0 = base + tid * kScanChunk, t1 = min(T, t0 + kScanChunk);
+    int local = 0;
+    for (int t = t0; t < t1; ++t) local += xb[static_cast<size_t>(t) * n] != 0.f;
+    sh[tid] = local;
+    __syncthreads();
+    for (int off = 1; off < kScanThreads; off <<= 1) {
+      const int v = tid >= off ? sh[tid - off] : 0;
+      __syncthreads();
+      sh[tid] += v;
+      __syncthreads();
+    }
+    int s = carry + sh[tid] - local;
+    for (int t = t0; t < t1; ++t) {
+      const bool nz = xb[static_cast<size_t>(t) * n] != 0.f;
+      s += nz;
+      pos[static_cast<size_t>(b) * T + t] = nz ? s : 0;
+    }
+    carry += sh[kScanThreads - 1];
+    __syncthreads();
+  }
+}
+
+// out = fp16(x + alpha * table[pos]) (tts_modules.py:228-229).  table[p] = [sin(p f_i), cos(p f_i)], f_i = exp(-i ln(1e4) /
+// (n/2 - 1)), row 0 = 0 (common_layers.py:106-122), evaluated in fp32 with the full-range sinf / cosf.
+__global__ void k_pe_posadd(const float* x, const int* pos, const float* alpha, int total_rows, int n, float neg_emb,
+                            __half* out) {
+  const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
+  if (i >= static_cast<size_t>(total_rows) * n) return;
+  const int c = static_cast<int>(i % n), half = n / 2;
+  const int ps = pos[i / n];
+  float tab = 0.f;
+  if (ps != 0) {
+    const int fi = c < half ? c : c - half;
+    const float arg = static_cast<float>(ps) * expf(static_cast<float>(fi) * neg_emb);
+    tab = c < half ? sinf(arg) : cosf(arg);
+  }
+  out[i] = __float2half_rn(x[i] + alpha[0] * tab);
+}
+
+// ---- weight packing ------------------------------------------------------------------------------
+// Conv1d [n][cin][k] (Linear: k = 1) -> fp16 [kc][nt][64], K index kk = tap * cin + channel, zero padded; bias -> [nt]
+__global__ void k_pe_pack(const float* w, const float* bias, int cin, int n, int k, int nt, int kc, __half* wp,
+                          float* bp) {
+  const size_t total = static_cast<size_t>(kc) * nt * 64;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int q = static_cast<int>(i & 63);
+    const size_t t = i >> 6;
+    const int r = static_cast<int>(t % nt), s = static_cast<int>(t / nt);
+    const int kk = s * 64 + q, j = kk / cin, c = kk - j * cin;
+    float v = 0.f;
+    if (r < n && j < k) v = w[(static_cast<size_t>(r) * cin + c) * k + j];
+    wp[i] = __float2half_rn(v);
+    if (i < static_cast<size_t>(nt)) bp[i] = static_cast<int>(i) < n ? bias[i] : 0.f;
+  }
+}
+
+// BatchNorm1d in eval mode as y = x * scale + shift: scale = w / sqrt(var + eps), shift = b - mean * scale
+__global__ void k_pe_bn(const float* w, const float* b, const float* mean, const float* var, int n, float* scale,
+                        float* shift) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float s = w[i] / sqrtf(var[i] + kBnEps);
+  scale[i] = s;
+  shift[i] = b[i] - mean[i] * s;
+}
+
+int pe_ck(const char* what) {
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("%s: %s", what, cudaGetErrorString(e));
+    return DSX_E_CUDA;
+  }
+  return DSX_OK;
+}
+
+int pe_nt(int n) { return n <= 16 ? 16 : n <= 32 ? 32 : n <= 64 ? 64 : n <= 128 ? 128 : 256; }
+
+}  // namespace
+}  // namespace dsx
+
+using namespace dsx;
+
+struct dsx_pe {
+  int device = 0;
+  dsx_pe_config cfg{};
+  int P = 0;
+  bool loaded = false;
+  PePacked prenet[kPePrenetLayers], prenet_out, enc_in, enc_out, pred[kPePredLayers];
+  std::vector<PePacked> enc;
+  float* head = nullptr;       // linear.weight [2][P], bias [2]
+  float* alpha = nullptr;      // pos_embed_alpha [1]
+  std::vector<void*> owned;
+  void* ws = nullptr;
+  size_t ws_cap = 0;
+};
+
+namespace {
+
+int pe_alloc(dsx_pe* h, void** p, size_t bytes) {
+  cudaError_t e = cudaMalloc(p, bytes ? bytes : 1);
+  if (e != cudaSuccess) {
+    set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? DSX_E_NOMEM : DSX_E_CUDA;
+  }
+  h->owned.push_back(*p);
+  return DSX_OK;
+}
+
+void pe_free_model(dsx_pe* h) {
+  for (void* p : h->owned) cudaFree(p);
+  h->owned.clear();
+  h->enc.clear();
+  h->loaded = false;
+}
+
+int pe_copy(dsx_pe* h, float** dst, const float* src, int n, const char* what, cudaStream_t s) {
+  DSX_CHECK(src, DSX_E_INVALID, "missing %s", what);
+  DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(dst), static_cast<size_t>(n) * sizeof(float)));
+  DSX_CUDA(cudaMemcpyAsync(*dst, src, static_cast<size_t>(n) * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  return DSX_OK;
+}
+
+// pack one conv (k taps starting at tap0) or linear (k = 1, tap0 = 0) of cin -> n channels
+int pe_pack(dsx_pe* h, PePacked& pc, const float* w, const float* b, int cin, int n, int k, int tap0, const char* what,
+            cudaStream_t s) {
+  DSX_CHECK(w && b, DSX_E_INVALID, "missing %s weight or bias", what);
+  pc.cin = cin;
+  pc.n = n;
+  pc.taps = k;
+  pc.tap0 = tap0;
+  pc.nt = pe_nt(n);
+  pc.kc = (k * cin + 63) / 64;
+  const size_t nw = static_cast<size_t>(pc.kc) * pc.nt * 64;
+  DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(&pc.w), nw * sizeof(__half)));
+  DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(&pc.b), static_cast<size_t>(pc.nt) * sizeof(float)));
+  const int blocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 4096));
+  k_pe_pack<<<blocks, 256, 0, s>>>(w, b, cin, n, k, pc.nt, pc.kc, pc.w, pc.b);
+  return pe_ck("k_pe_pack");
+}
+
+template <int NT>
+int pe_launch(const PeConvArgs& a, int mtiles, int B, cudaStream_t s) {
+  k_pe_conv<NT><<<dim3(mtiles, B), 128 * PeShape<NT>::WG, pe_smem<NT>(), s>>>(a);
+  return pe_ck("k_pe_conv");
+}
+
+int pe_run(const PePacked& pc, PeConvArgs a, int B, cudaStream_t s) {
+  a.cin = pc.cin;
+  a.taps = pc.taps;
+  a.tap0 = pc.tap0;
+  a.kc = pc.kc;
+  a.w = pc.w;
+  a.bias = pc.b;
+  a.n = pc.n;
+  a.mtiles = (a.T + kPeRows - 1) / kPeRows;
+  switch (pc.nt) {
+    case 16: return pe_launch<16>(a, a.mtiles, B, s);
+    case 32: return pe_launch<32>(a, a.mtiles, B, s);
+    case 64: return pe_launch<64>(a, a.mtiles, B, s);
+    case 128: return pe_launch<128>(a, a.mtiles, B, s);
+    default: return pe_launch<256>(a, a.mtiles, B, s);
+  }
+}
+
+int pe_validate(const dsx_pe_config* c) {
+  DSX_CHECK(c, DSX_E_INVALID, "config is NULL");
+  DSX_CHECK(c->n_mel_bins == kPeMel, DSX_E_INVALID, "n_mel_bins must be 80 (got %d)", c->n_mel_bins);
+  DSX_CHECK(c->hidden >= 16 && c->hidden <= 256 && c->hidden % 16 == 0, DSX_E_INVALID,
+            "hidden must be a multiple of 16 in [16, 256] (got %d)", c->hidden);
+  DSX_CHECK(c->predictor_hidden >= 16 && c->predictor_hidden <= 256 && c->predictor_hidden % 16 == 0, DSX_E_INVALID,
+            "predictor_hidden must be a multiple of 16 in [16, 256] (got %d)", c->predictor_hidden);
+  DSX_CHECK(c->predictor_kernel >= 1 && c->predictor_kernel <= 31 && c->predictor_kernel % 2 == 1, DSX_E_INVALID,
+            "predictor_kernel must be odd and in [1, 31] (got %d)", c->predictor_kernel);
+  DSX_CHECK(c->conv_layers >= 0 && c->conv_layers <= kPeMaxConvLayers, DSX_E_INVALID,
+            "conv_layers must be in [0, %d] (got %d)", kPeMaxConvLayers, c->conv_layers);
+  DSX_CHECK(c->causal == 0 || c->causal == 1, DSX_E_INVALID, "causal must be 0 (SAME) or 1 (LEFT) (got %d)", c->causal);
+  DSX_CHECK(c->pitch_norm == 0 || c->pitch_norm == 1, DSX_E_INVALID, "pitch_norm must be 0 (log) or 1 (standard) (got %d)",
+            c->pitch_norm);
+  DSX_CHECK(c->use_uv == 0 || c->use_uv == 1, DSX_E_INVALID, "use_uv must be 0 or 1 (got %d)", c->use_uv);
+  DSX_CHECK(isfinite(c->f0_mean) && isfinite(c->f0_std), DSX_E_INVALID, "f0_mean and f0_std must be finite");
+  return DSX_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int dsx_pe_create(int device, const dsx_pe_config* cfg, dsx_pe** out) {
+  DSX_CHECK(out, DSX_E_INVALID, "out is NULL");
+  *out = nullptr;
+  DSX_TRY(pe_validate(cfg));
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0) {
+    set_error("no CUDA device available (%s); dsx has no CPU fallback", cudaGetErrorString(e));
+    return DSX_E_CUDA;
+  }
+  DSX_CHECK(device >= 0 && device < ndev, DSX_E_INVALID, "device %d out of range (%d devices)", device, ndev);
+  cudaDeviceProp prop;
+  DSX_CUDA(cudaGetDeviceProperties(&prop, device));
+  DSX_CHECK(prop.major == 9 && prop.minor == 0, DSX_E_CUDA,
+            "the pitch extractor's kernels are built for sm_90a; device %d is sm_%d%d", device, prop.major, prop.minor);
+  DSX_CUDA(cudaSetDevice(device));
+  DSX_CUDA(cudaFuncSetAttribute(k_pe_conv<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, pe_smem<16>()));
+  DSX_CUDA(cudaFuncSetAttribute(k_pe_conv<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, pe_smem<32>()));
+  DSX_CUDA(cudaFuncSetAttribute(k_pe_conv<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, pe_smem<64>()));
+  DSX_CUDA(cudaFuncSetAttribute(k_pe_conv<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, pe_smem<128>()));
+  DSX_CUDA(cudaFuncSetAttribute(k_pe_conv<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, pe_smem<256>()));
+  dsx_pe* h = new dsx_pe();
+  h->device = device;
+  h->cfg = *cfg;
+  h->P = cfg->predictor_hidden;
+  *out = h;
+  return DSX_OK;
+}
+
+void dsx_pe_destroy(dsx_pe* h) {
+  if (!h) return;
+  cudaSetDevice(h->device);
+  cudaDeviceSynchronize();
+  pe_free_model(h);
+  if (h->ws) cudaFree(h->ws);
+  delete h;
+}
+
+int dsx_pe_load(dsx_pe* h, const dsx_pe_params* p, void* stream) {
+  DSX_CHECK(h && p, DSX_E_INVALID, "null handle or params");
+  DSX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const dsx_pe_config& c = h->cfg;
+  const int H = c.hidden, P = h->P, L = c.conv_layers, k = c.predictor_kernel;
+  DSX_CHECK(p->prenet_w && p->prenet_b && p->bn_w && p->bn_b && p->bn_mean && p->bn_var, DSX_E_INVALID,
+            "missing per-layer prenet arrays");
+  DSX_CHECK(p->pred_w && p->pred_b && p->ln_w && p->ln_b, DSX_E_INVALID, "missing per-layer pitch_predictor arrays");
+  DSX_CHECK(L == 0 || (p->enc_w && p->enc_b && p->gn_w && p->gn_b), DSX_E_INVALID, "missing per-layer mel_encoder arrays");
+  DSX_CUDA(cudaStreamSynchronize(s));   // the old packs may still be read by queued work
+  pe_free_model(h);
+  char what[64];
+  for (int i = 0; i < kPePrenetLayers; ++i) {
+    snprintf(what, sizeof what, "mel_prenet.layers.%d.0", i);
+    PePacked& pc = h->prenet[i];
+    DSX_TRY(pe_pack(h, pc, p->prenet_w[i], p->prenet_b[i], i ? H : kPeMel, H, kPePrenetKernel, -kPePrenetKernel / 2,
+                    what, s));
+    DSX_CHECK(p->bn_w[i] && p->bn_b[i] && p->bn_mean[i] && p->bn_var[i], DSX_E_INVALID, "missing mel_prenet.layers.%d.2", i);
+    DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(&pc.s), H * sizeof(float)));
+    DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(&pc.t), H * sizeof(float)));
+    k_pe_bn<<<(H + 255) / 256, 256, 0, s>>>(p->bn_w[i], p->bn_b[i], p->bn_mean[i], p->bn_var[i], H, pc.s, pc.t);
+    DSX_TRY(pe_ck("k_pe_bn"));
+  }
+  DSX_TRY(pe_pack(h, h->prenet_out, p->prenet_out_w, p->prenet_out_b, H, H, 1, 0, "mel_prenet.out_proj", s));
+  if (L > 0) {
+    DSX_TRY(pe_pack(h, h->enc_in, p->enc_in_w, p->enc_in_b, H, H, 1, 0, "mel_encoder.in_proj", s));
+    h->enc.resize(L);
+    for (int i = 0; i < L; ++i) {
+      snprintf(what, sizeof what, "mel_encoder.conv.%d", i);
+      DSX_TRY(pe_pack(h, h->enc[i], p->enc_w[i], p->enc_b[i], H, H, kPeEncKernel, -kPeEncKernel / 2, what, s));
+      DSX_TRY(pe_copy(h, &h->enc[i].s, p->gn_w[i], H, "mel_encoder GroupNorm weight", s));
+      DSX_TRY(pe_copy(h, &h->enc[i].t, p->gn_b[i], H, "mel_encoder GroupNorm bias", s));
+    }
+    DSX_TRY(pe_pack(h, h->enc_out, p->enc_out_w, p->enc_out_b, H, H, 1, 0, "mel_encoder.out_proj", s));
+  }
+  const int tap0 = c.causal ? -(k - 1) : -(k - 1) / 2;   // ConstantPad1d LEFT (k - 1, 0) or SAME
+  for (int i = 0; i < kPePredLayers; ++i) {
+    snprintf(what, sizeof what, "pitch_predictor.conv.%d.1", i);
+    PePacked& pc = h->pred[i];
+    DSX_TRY(pe_pack(h, pc, p->pred_w[i], p->pred_b[i], i ? P : H, P, k, tap0, what, s));
+    DSX_TRY(pe_copy(h, &pc.s, p->ln_w[i], P, "pitch_predictor LayerNorm weight", s));
+    DSX_TRY(pe_copy(h, &pc.t, p->ln_b[i], P, "pitch_predictor LayerNorm bias", s));
+  }
+  DSX_CHECK(p->linear_w && p->linear_b && p->pos_embed_alpha, DSX_E_INVALID,
+            "missing pitch_predictor.linear or pos_embed_alpha");
+  DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(&h->head), (2 * P + 2) * sizeof(float)));
+  DSX_CUDA(cudaMemcpyAsync(h->head, p->linear_w, 2 * P * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  DSX_CUDA(cudaMemcpyAsync(h->head + 2 * P, p->linear_b, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  DSX_TRY(pe_copy(h, &h->alpha, p->pos_embed_alpha, 1, "pos_embed_alpha", s));
+  h->loaded = true;
+  return DSX_OK;
+}
+
+int dsx_pe_forward(dsx_pe* h, const float* mel, dsx_strides ms, int B, int T, float* pitch_pred, float* f0,
+                   void* stream) {
+  DSX_CHECK(h, DSX_E_INVALID, "null handle");
+  DSX_CHECK(h->loaded, DSX_E_STATE, "dsx_pe_load has not been called");
+  DSX_CHECK(mel, DSX_E_INVALID, "mel must not be NULL");
+  DSX_CHECK(B > 0 && T > 0, DSX_E_INVALID, "B and T must be positive (got %d, %d)", B, T);
+  DSX_CHECK(B <= 65535, DSX_E_INVALID, "B = %d utterances per call is above the 65535 the launch grid holds", B);
+  const dsx_pe_config& c = h->cfg;
+  const int H = c.hidden, P = h->P, L = c.conv_layers, C = std::max(H, P);
+  DSX_CHECK(static_cast<long long>(B) * T * C < (1ll << 31), DSX_E_INVALID, "B * T = %lld frames is too large",
+            static_cast<long long>(B) * T);
+  DSX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!pitch_pred && !f0) return DSX_OK;
+
+  // workspace: fp16 MEL / A0 / A1, fp32 X / Y, padding flags, positions, GroupNorm partials
+  const size_t frames = static_cast<size_t>(B) * T;
+  const int mtiles = (T + kPeRows - 1) / kPeRows;
+  auto al = [](size_t bytes) { return (bytes + 255) & ~size_t(255); };
+  const size_t need = al(frames * kPeMel * 2) + 2 * al(frames * C * 2) + 2 * al(frames * H * 4) + al(frames) +
+                      al(frames * 4) + al(static_cast<size_t>(B) * mtiles * (H / 16) * 3 * 4);
+  if (h->ws_cap < need) {
+    if (h->ws) {
+      DSX_CUDA(cudaStreamSynchronize(s));
+      cudaFree(h->ws);
+    }
+    h->ws = nullptr;
+    h->ws_cap = 0;
+    cudaError_t e = cudaMalloc(&h->ws, need + need / 8);
+    if (e != cudaSuccess) {
+      set_error("cudaMalloc(%zu) failed: %s", need + need / 8, cudaGetErrorString(e));
+      return e == cudaErrorMemoryAllocation ? DSX_E_NOMEM : DSX_E_CUDA;
+    }
+    h->ws_cap = need + need / 8;
+  }
+  uint8_t* wp = static_cast<uint8_t*>(h->ws);
+  auto take = [&](size_t bytes) { uint8_t* q = wp; wp += al(bytes); return q; };
+  __half* MEL = reinterpret_cast<__half*>(take(frames * kPeMel * 2));
+  __half* A[2] = {reinterpret_cast<__half*>(take(frames * C * 2)), reinterpret_cast<__half*>(take(frames * C * 2))};
+  float* X = reinterpret_cast<float*>(take(frames * H * 4));
+  float* Y = reinterpret_cast<float*>(take(frames * H * 4));
+  uint8_t* PAD = take(frames);
+  int* POS = reinterpret_cast<int*>(take(frames * 4));
+  float* ST = reinterpret_cast<float*>(take(static_cast<size_t>(B) * mtiles * (H / 16) * 3 * 4));
+
+  k_pe_pack_mel<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(mel, ms, B, T, MEL, PAD);
+  DSX_TRY(pe_ck("k_pe_pack_mel"));
+
+  PeConvArgs base{};
+  base.T = T;
+  base.pad = PAD;
+  PeConvArgs a = base;
+  // Prenet (pe.py:23-41): 3 x [conv k5, ReLU, BatchNorm, * nonpadding], then out_proj * nonpadding
+  const __half* in = MEL;
+  int cur = 0;
+  for (int i = 0; i < kPePrenetLayers; ++i) {
+    a = base;
+    a.x = in;
+    a.mode = PE_PRENET;
+    a.flags = PE_MASK | PE_OUT16;
+    a.scale = h->prenet[i].s;
+    a.shift = h->prenet[i].t;
+    a.o16 = A[cur];
+    DSX_TRY(pe_run(h->prenet[i], a, B, s));
+    in = A[cur];
+    cur ^= 1;
+  }
+  a = base;
+  a.x = in;
+  a.mode = PE_LINEAR;
+  a.flags = PE_MASK | (L > 0 ? PE_OUT16 : PE_OUT32);
+  a.o16 = A[cur];
+  a.o32 = X;
+  DSX_TRY(pe_run(h->prenet_out, a, B, s));
+  if (L > 0) {
+    // ConvStacks (pe.py:98-116): in_proj, conv_layers x [x += relu(GroupNorm(conv(x)))], out_proj; no masking
+    in = A[cur];
+    cur ^= 1;
+    a = base;
+    a.x = in;
+    a.mode = PE_LINEAR;
+    a.flags = PE_OUT32 | PE_OUT16;
+    a.o32 = X;
+    a.o16 = A[cur];
+    DSX_TRY(pe_run(h->enc_in, a, B, s));
+    for (int i = 0; i < L; ++i) {
+      a = base;
+      a.x = A[cur];
+      a.mode = PE_GN;
+      a.flags = PE_OUT32;
+      a.o32 = Y;
+      a.stats = ST;
+      DSX_TRY(pe_run(h->enc[i], a, B, s));
+      k_pe_gn<<<dim3((T + kGnRows - 1) / kGnRows, B), 256, 0, s>>>(Y, ST, mtiles, h->enc[i].s, h->enc[i].t, T, H, X,
+                                                                   A[cur ^ 1]);
+      DSX_TRY(pe_ck("k_pe_gn"));
+      cur ^= 1;
+    }
+    a = base;
+    a.x = A[cur];
+    a.mode = PE_LINEAR;
+    a.flags = PE_OUT32;
+    a.o32 = Y;
+    DSX_TRY(pe_run(h->enc_out, a, B, s));
+  }
+  // PitchPredictor (tts_modules.py:222-235): + alpha * position embedding, 4 x [conv, ReLU, LayerNorm], the head
+  const float* xs = L > 0 ? Y : X;
+  k_pe_scan<<<B, kScanThreads, 0, s>>>(xs, T, H, POS);
+  DSX_TRY(pe_ck("k_pe_scan"));
+  const float neg_emb = -static_cast<float>(log(10000.0) / (H / 2 - 1));
+  const size_t ne = frames * H;
+  k_pe_posadd<<<static_cast<unsigned>((ne + 255) / 256), 256, 0, s>>>(xs, POS, h->alpha, static_cast<int>(frames), H,
+                                                                      neg_emb, A[0]);
+  DSX_TRY(pe_ck("k_pe_posadd"));
+  cur = 0;
+  for (int i = 0; i < kPePredLayers; ++i) {
+    a = base;
+    a.x = A[cur];
+    a.scale = h->pred[i].s;
+    a.shift = h->pred[i].t;
+    if (i + 1 < kPePredLayers) {
+      a.mode = PE_LN;
+      a.flags = PE_OUT16;
+      a.o16 = A[cur ^ 1];
+    } else {
+      a.mode = PE_HEAD;
+      a.hw = h->head;
+      a.hb = h->head + 2 * P;
+      a.pitch = pitch_pred;
+      a.f0 = f0;
+      a.pitch_norm = c.pitch_norm;
+      a.use_uv = c.use_uv;
+      a.f0_mean = c.f0_mean;
+      a.f0_std = c.f0_std;
+    }
+    DSX_TRY(pe_run(h->pred[i], a, B, s));
+    cur ^= 1;
+  }
+  return DSX_OK;
+}
+
+}  // extern "C"

@@ -16,6 +16,12 @@ are the reference's own, so the task files run unchanged.
 replaces ``modules.hifigan.hifigan.HifiGanGenerator`` -- and the name bound from it in ``vocoders.*`` modules already
 imported -- by ``diffsinger_b200.HifiGanGenerator``, so ``vocoders/hifigan.py:load_model`` (strict ``load_state_dict``,
 ``remove_weight_norm``, ``.to(device)``) and ``spec2wav`` run the vocoder on dsx unchanged.
+
+    dropin.install_pitch_extractor()
+
+replaces ``modules.fastspeech.pe.PitchExtractor`` -- and the name bound from it in ``inference.*`` / ``tasks.*`` /
+``usr.*`` modules already imported (inference/svs/ds_e2e.py binds it at import) -- by ``diffsinger_b200.PitchExtractor``,
+so the e2e inference's ``self.pe(mel_out)['f0_denorm_pred']`` runs on dsx after a strict ``load_ckpt``.
 """
 import importlib
 import sys
@@ -168,3 +174,28 @@ def _swap_vocoder(old, new):
             continue
         if getattr(mod, "HifiGanGenerator", None) is old:
             mod.HifiGanGenerator = new
+
+
+_pe = {}
+
+
+def install_pitch_extractor():
+    from .pitch import PitchExtractor
+    mod = importlib.import_module("modules.fastspeech.pe")
+    _pe.setdefault("ref", mod.PitchExtractor)
+    _swap_pitch_extractor(_pe["ref"], PitchExtractor)
+    return PitchExtractor
+
+
+def uninstall_pitch_extractor():
+    if _pe:
+        from .pitch import PitchExtractor
+        _swap_pitch_extractor(PitchExtractor, _pe["ref"])
+
+
+def _swap_pitch_extractor(old, new):
+    for name, mod in list(sys.modules.items()):
+        if mod is None or not (name == "modules.fastspeech.pe" or name.startswith(("inference.", "tasks.", "usr."))):
+            continue
+        if getattr(mod, "PitchExtractor", None) is old:
+            mod.PitchExtractor = new

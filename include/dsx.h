@@ -310,6 +310,75 @@ int dsx_hifigan_forward(dsx_hifigan* h, const float* mel, dsx_strides ms, const 
                         const float* phase0, const float* src_noise, uint64_t seed, int B, int T, float* wav,
                         void* stream);
 
+/* ---- Pitch extractor: mel -> f0 -------------------------------------------------------------------------------------
+ * Replaces: PitchExtractor (modules/fastspeech/pe.py:119-149) with its Prenet (:7-41), ConvStacks (:81-116, GroupNorm),
+ * PitchPredictor (modules/fastspeech/tts_modules.py:192-235, sinusoidal position embedding of
+ * modules/commons/common_layers.py:88-143) and denorm_f0 (utils/pitch_utils.py:63-76), in eval mode, as
+ * inference/svs/ds_e2e.py:26-45 runs it between the sampler and the vocoder.  Convolutions and linears run on tensor
+ * cores with fp16 operands and fp32 accumulation; normalisations, the residual stream and the outputs are fp32.
+ * A pitch-extractor handle is independent of the sampler and vocoder handles. */
+typedef struct dsx_pe dsx_pe;
+
+/* The hyper-parameters PitchExtractor reads (hparams + its constructor's conv_layers). */
+typedef struct {
+  int n_mel_bins;        /* 80                                                                          */
+  int hidden;            /* hidden_size H: a multiple of 16 in [16, 256]                                */
+  int predictor_hidden;  /* P (the reference's predictor_hidden, or H when that is <= 0): same range      */
+  int predictor_kernel;  /* odd, <= 31                                                                  */
+  int conv_layers;       /* mel_encoder GroupNorm conv blocks, 0..16 (0: no mel_encoder)                 */
+  int causal;            /* ffn_padding: 0 'SAME', 1 'LEFT'                                             */
+  int pitch_norm;        /* 0 'log' (f0 = 2^pred), 1 'standard' (f0 = pred * f0_std + f0_mean)           */
+  float f0_mean, f0_std;
+  int use_uv;            /* pitch_type == 'frame' and use_uv: f0 = 0 where pitch_pred[..., 1] > 0        */
+} dsx_pe_config;
+
+/* Parameters, fp32 device pointers, each tensor contiguous in the reference's state-dict layout.  Per-layer arrays are
+ * HOST arrays of device pointers.  num_batches_tracked and embed_positions._float_tensor are not needed. */
+typedef struct {
+  const float* const* prenet_w;      /* mel_prenet.layers.i.0.weight [H, C_in, 5], i < 3, C_in = 80 then H           */
+  const float* const* prenet_b;      /* mel_prenet.layers.i.0.bias [H]                                               */
+  const float* const* bn_w;          /* mel_prenet.layers.i.2.weight [H] (BatchNorm1d)                               */
+  const float* const* bn_b;          /* mel_prenet.layers.i.2.bias                                                   */
+  const float* const* bn_mean;       /* mel_prenet.layers.i.2.running_mean                                           */
+  const float* const* bn_var;        /* mel_prenet.layers.i.2.running_var                                            */
+  const float* prenet_out_w;         /* mel_prenet.out_proj.weight [H, H]                                            */
+  const float* prenet_out_b;
+  const float* enc_in_w;             /* mel_encoder.in_proj.weight [H, H] (conv_layers > 0)                          */
+  const float* enc_in_b;
+  const float* const* enc_w;         /* mel_encoder.conv.i.conv.conv.weight [H, H, 5], i < conv_layers               */
+  const float* const* enc_b;
+  const float* const* gn_w;          /* mel_encoder.conv.i.norm.weight [H] (GroupNorm(H / 16, H))                    */
+  const float* const* gn_b;
+  const float* enc_out_w;            /* mel_encoder.out_proj.weight [H, H]                                           */
+  const float* enc_out_b;
+  const float* const* pred_w;        /* pitch_predictor.conv.i.1.weight [P, C_in, k], i < 5, C_in = H then P         */
+  const float* const* pred_b;
+  const float* const* ln_w;          /* pitch_predictor.conv.i.3.weight [P] (LayerNorm, eps 1e-12)                   */
+  const float* const* ln_b;
+  const float* linear_w;             /* pitch_predictor.linear.weight [2, P]                                         */
+  const float* linear_b;             /* pitch_predictor.linear.bias [2]                                              */
+  const float* pos_embed_alpha;      /* pitch_predictor.pos_embed_alpha [1]                                          */
+} dsx_pe_params;
+
+/* Replaces: PitchExtractor(n_mel_bins, conv_layers) under the global hparams.  Validates the configuration
+ * (DSX_E_INVALID). */
+int dsx_pe_create(int device, const dsx_pe_config* cfg, dsx_pe** out);
+void dsx_pe_destroy(dsx_pe* h);
+
+/* Replaces: load_state_dict (utils/__init__.py:load_ckpt of the pe_ckpt).  Packs fp16 tensor-core tiles and folds each
+ * BatchNorm's running statistics and affine into a per-channel scale and shift.  Call again after every change of the
+ * weights. */
+int dsx_pe_load(dsx_pe* h, const dsx_pe_params* p, void* stream);
+
+/* Replaces: PitchExtractor.forward(mel_input) (pe.py:135-149).
+ *   mel         logically [B, T, 80], any element strides ms (b, c = bin, t): dsx_infer's mel_out as it is;
+ *   pitch_pred  [B, T, 2] contiguous, or NULL;
+ *   f0          [B, T] contiguous: f0_denorm_pred in Hz, 0 where uv says unvoiced and on padding frames, or NULL.
+ * A frame is padding when all 80 bins are exactly 0 (pe.py:29, :143).  The batch is computed as given: GroupNorm
+ * statistics and the position scan span all T frames of an utterance, padding included, exactly as in the reference, so
+ * an utterance with a zero-padded tail is not the same as that utterance alone; utterances of equal T are independent. */
+int dsx_pe_forward(dsx_pe* h, const float* mel, dsx_strides ms, int B, int T, float* pitch_pred, float* f0, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
