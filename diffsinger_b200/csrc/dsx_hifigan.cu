@@ -1,24 +1,22 @@
 // HiFi-GAN (NSF) generator on sm_90a: the vocoder that turns the sampler's mel spectrogram into a waveform
 // (modules/hifigan/hifigan.py:104-171 with the harmonic source of modules/parallel_wavegan/models/source.py).
 //
-// Every convolution with a tensor-core shape is one implicit GEMM on wgmma (k_conv).  Activations are frames-major
-// fp16 [B][L][C], channels zero-padded to a multiple of 16, the layout of the sampler's step kernel.  Row m of the GEMM
-// is an output position; the K axis is (tap j, input channel c), and tap j reads the input at row m + tap0 + j * tstep,
-// zero outside the utterance's valid rows [0, len_b), which is the conv's zero padding:
+// Every convolution with a tensor-core shape is one implicit GEMM on wgmma (k_conv, on the core of dsx_conv.cuh), over
+// activations padded to a multiple of 16 channels, the layout of the sampler's step kernel:
 //   Conv1d(k, dilation d, padding (k - 1) d / 2)        tap0 = -(k - 1) d / 2, tstep = d, N = C_out
 //   ConvTranspose1d(k, stride u, padding (k - u) / 2)   polyphase: out[m u + r - pad] = sum_{j < k/u} x[m - j] W[:, :, r + j u]
 //                                                       tap0 = 0, tstep = -1, N = u C_out (column n = r C_out + o); the
 //                                                       epilogue scatters the phases
 // The epilogue adds the bias and, by flags, the NSF branch's noise conv (ups), a fp32 residual, the fp32 multi-receptive-
 // field sum and its 1 / num_kernels, and writes fp32 and / or leaky_relu(., 0.1) in fp16 (the next conv's operand).
-// A 64-row tile is one warpgroup; operands reach shared memory by cp.async in the 128-byte-swizzled layout of dsx_ptx.cuh,
-// double buffered per 64-wide K chunk.  On stages of at most 64 channels a whole ResBlock runs as one chained launch
-// instead (k_chain, below).  The harmonic source and conv_post (N = 1) run on CUDA cores.
+// On stages of at most 64 channels a whole ResBlock runs as one chained launch instead (k_chain, below).  The harmonic
+// source and conv_post (N = 1) run on CUDA cores.
 #include <math.h>
 #include <stdio.h>
 
 #include <algorithm>
 
+#include "dsx_conv.cuh"
 #include "dsx_internal.h"
 #include "dsx_ptx.cuh"
 #include "dsx_rng.cuh"
@@ -30,29 +28,22 @@ constexpr int kMelBins = 80;
 constexpr int kHarmonics = 9;        // SineGen dim = harmonic_num + 1 (hifigan.py:112)
 constexpr float kLrelu = 0.1f;       // LRELU_SLOPE (hifigan.py:11)
 constexpr float kSineAmp = 0.1f, kNoiseStd = 0.003f;   // SineGen defaults (source.py)
-constexpr int kRowsPerCta = 64;
 
 inline int round16(int c) { return (c + 15) & ~15; }
 
-// one packed convolution
-struct PackedConv {
-  int cin = 0, cout = 0, k = 0;
-  int cin_p = 0, cout_p = 0;   // channel counts padded to 16
-  int taps = 0, tap0 = 0, tstep = 0;
+// one packed convolution: the GEMM (cin padded to 16, at most 128 columns per tile) and its output channels
+struct PackedConv : ConvGemm {
+  int cout = 0, cout_p = 0;    // cout_p: padded to 16
   int u = 1, pad = 0;          // ConvTranspose1d: stride and padding (u == 1, pad == 0 for Conv1d)
-  int n = 0, nt = 0, ntiles = 0, kc = 0;   // GEMM columns, columns per tile (16 / 32 / 64 / 128), tiles, 64-wide K chunks
-  __half* w = nullptr;         // [ntiles][kc][nt][64] fp16
-  float* b = nullptr;          // [ntiles * nt]
 };
 
 enum { EPI_OUT32 = 1, EPI_OUT16 = 2, EPI_RES = 4, EPI_SUM = 8, EPI_DIV = 16, EPI_NOISE = 32 };
 
 struct ConvArgs {
-  const __half* x;             // A source [B][lx][cin_p]
-  int lx, cin_p, taps, tap0, tstep, kc;
-  const __half* w;
-  const float* bias;
-  int n, cout_p, u, pad, ups;  // ups: polyphase ConvTranspose1d
+  ConvGemm g;
+  const __half* x;             // A source [B][lx][g.cin]
+  int lx;
+  int cout_p, u, pad, ups;     // ups: polyphase ConvTranspose1d
   const int* lens;             // [B] frames, or null (all T)
   int T, in_mul;               // valid input rows of utterance b = len_b * in_mul
   int flags;
@@ -75,65 +66,22 @@ template <int NT>
 __global__ void __launch_bounds__(128) k_conv(const ConvArgs p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr int kA = kRowsPerCta * 128, kB = NT * 128, kStage = kA + kB;
-  const int tid = threadIdx.x, b = blockIdx.z, nt = blockIdx.y, m0 = blockIdx.x * kRowsPerCta;
+  const int tid = threadIdx.x, b = blockIdx.z, nt = blockIdx.y, m0 = blockIdx.x * kConvRows;
   const int len_frames = utt_len(p.lens, b, p.T);
   const int len_in = len_frames * p.in_mul;
   const int len_out = len_in * p.u;
   const int rows = p.ups ? len_in + (p.pad + p.u - 1) / p.u : len_in;   // ups: the last output rows come from m >= len_in
   if (m0 >= rows) return;
 
-  auto load = [&](int s, uint8_t* buf) {
-    const uint32_t da = smem_u32(buf), db = smem_u32(buf + kA);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int i = tid + q * 128, r = i >> 3, c = i & 7;
-      const int kk = s * 64 + c * 8, j = kk / p.cin_p, ch = kk - j * p.cin_p;
-      const int src = m0 + r + p.tap0 + j * p.tstep;
-      const bool valid = j < p.taps && src >= 0 && src < len_in;
-      cp16(da + sw128(r, c), p.x + (static_cast<size_t>(b) * p.lx + (valid ? src : 0)) * p.cin_p + (valid ? ch : 0), valid);
-    }
-    const __half* wsrc = p.w + (static_cast<size_t>(nt) * p.kc + s) * NT * 64;
-    for (int i = tid; i < NT * 8; i += 128) {
-      const int r = i >> 3, c = i & 7;
-      cp16(db + sw128(r, c), wsrc + r * 64 + c * 8, true);
-    }
-  };
-
   float acc[NT / 2];
-#pragma unroll
-  for (int e = 0; e < NT / 2; ++e) acc[e] = 0.f;
-  load(0, smem);
-  cp_commit();
-#pragma unroll 1
-  for (int s = 0; s < p.kc; ++s) {
-    uint8_t* cur = smem + (s & 1) * kStage;
-    if (s + 1 < p.kc) {
-      load(s + 1, smem + ((s + 1) & 1) * kStage);
-      cp_commit();
-      cp_wait<1>();
-    } else {
-      cp_wait<0>();
-    }
-    fence_proxy_async_smem();
-    __syncthreads();
-    const uint64_t da = wg_desc(smem_u32(cur)), db = wg_desc(smem_u32(cur + kA));
-    wg_fence();
-#pragma unroll
-    for (int k4 = 0; k4 < 4; ++k4) wgmma_f16<NT>(acc, da + 2 * k4, db + 2 * k4, 1);
-    wg_commit();
-    wg_wait0();
-#pragma unroll
-    for (int e = 0; e < NT / 2; ++e) asm volatile("" : "+f"(acc[e])::"memory");
-    __syncthreads();
-  }
+  conv_k_loop<NT, 1>(p.g, p.x, p.lx, len_in, b, m0, nt, smem, acc);
 
   // epilogue: element pairs (n, n + 1) share the phase r (cout_p is even) and are adjacent in memory
   const int len_h = len_frames * p.hop;
 #pragma unroll
   for (int e = 0; e < NT / 2; e += 2) {
     const int m = m0 + acc_row(tid, e), n = nt * NT + acc_col(tid, e);
-    if (n >= p.n || m >= rows) continue;
+    if (n >= p.g.n || m >= rows) continue;
     int row = m, o = n;
     if (p.ups) {
       const int r = n / p.cout_p;
@@ -141,7 +89,7 @@ __global__ void __launch_bounds__(128) k_conv(const ConvArgs p) {
       row = m * p.u + r - p.pad;
     }
     if (row < 0 || row >= len_out) continue;
-    float v0 = acc[e] + p.bias[n], v1 = acc[e + 1] + p.bias[n + 1];
+    float v0 = acc[e] + p.g.b[n], v1 = acc[e + 1] + p.g.b[n + 1];
     if (p.flags & EPI_NOISE) {         // noise_convs[i](har): stride ns, nks taps, padding npad, zero outside [0, len_h)
       const float* hb = p.har + static_cast<size_t>(b) * p.lh;
       const float* w0 = p.nw + static_cast<size_t>(o) * p.nks;
@@ -198,45 +146,6 @@ __global__ void k_wnorm(const float* v, const float* g, int inner, float* scale)
     float t = 0.f;
     for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) t += red[w];
     scale[i] = g ? g[i] / sqrtf(t) : 1.f;
-  }
-}
-
-struct PackArgs {
-  const float* v;
-  const float* scale;
-  const float* bias;
-  int cin, cout, k, u, transposed;
-  int cin_p, cout_p, taps, n, nt, kc, ntiles;
-  __half* w;
-  float* b;
-};
-
-// W (Conv1d [C_out][C_in][k] or ConvTranspose1d [C_in][C_out][k]) * scale -> fp16 [ntiles][kc][nt][64], zero padded
-__global__ void k_pack_conv(const PackArgs p) {
-  const size_t total = static_cast<size_t>(p.ntiles) * p.kc * p.nt * 64;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int q = static_cast<int>(i & 63);
-    size_t t = i >> 6;
-    const int rr = static_cast<int>(t % p.nt);
-    t /= p.nt;
-    const int s = static_cast<int>(t % p.kc);
-    const int tile = static_cast<int>(t / p.kc);
-    const int n = tile * p.nt + rr, kk = s * 64 + q, j = kk / p.cin_p, c = kk - j * p.cin_p;
-    float val = 0.f;
-    if (n < p.n && j < p.taps && c < p.cin) {
-      if (p.transposed) {
-        const int r = n / p.cout_p, o = n - r * p.cout_p;
-        if (o < p.cout) val = p.v[(static_cast<size_t>(c) * p.cout + o) * p.k + r + j * p.u] * p.scale[c];
-      } else if (n < p.cout) {
-        val = p.v[(static_cast<size_t>(n) * p.cin + c) * p.k + j] * p.scale[n];
-      }
-    }
-    p.w[i] = __float2half_rn(val);
-    if (i < static_cast<size_t>(p.ntiles) * p.nt) {
-      const int nn = static_cast<int>(i), o = nn % p.cout_p;
-      p.b[nn] = (nn < p.n && o < p.cout) ? p.bias[o] : 0.f;
-    }
   }
 }
 
@@ -376,18 +285,6 @@ __global__ void k_post(const float* x, int lo, int cp, int c, const float* w, co
   }
   wav[i] = acc;
 }
-
-int ck(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("%s: %s", what, cudaGetErrorString(e));
-    return DSX_E_CUDA;
-  }
-  return DSX_OK;
-}
-
-template <int NT>
-constexpr int conv_smem() { return 2 * (kRowsPerCta * 128 + NT * 128) + 1024; }
 
 // ---- one ResBlock as a chain of convs over one tile -----------------------------------------------
 // Stages of at most 64 (padded) channels are bandwidth-bound one conv per launch, so k_chain runs a whole ResBlock per
@@ -545,29 +442,15 @@ struct dsx_hifigan {
   std::vector<int> noise_ks, noise_s;
   float* src_w = nullptr;                 // [9] + bias [1]
   float* post_w = nullptr;                // [cp][7] + bias at [cp * 7]
-  std::vector<void*> owned;
-  float* scale = nullptr;                 // weight-norm scratch
-  size_t scale_cap = 0;
-  // workspace (grow-only)
-  void* ws = nullptr;
-  size_t ws_cap = 0;
+  DevAllocs mem;                          // the packs above
+  GrowBuffer scale;                       // weight-norm scratch
+  GrowBuffer ws;                          // workspace of a forward call
 };
 
 namespace {
 
-int halloc(dsx_hifigan* h, void** p, size_t bytes) {
-  cudaError_t e = cudaMalloc(p, bytes ? bytes : 1);
-  if (e != cudaSuccess) {
-    set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
-    return e == cudaErrorMemoryAllocation ? DSX_E_NOMEM : DSX_E_CUDA;
-  }
-  h->owned.push_back(*p);
-  return DSX_OK;
-}
-
 void free_model(dsx_hifigan* h) {
-  for (void* p : h->owned) cudaFree(p);
-  h->owned.clear();
+  h->mem.free_all();
   h->ups.clear();
   h->rb.clear();
   h->noise_w.clear();
@@ -580,10 +463,8 @@ int stage_cin(const dsx_hifigan_config& c, int i) { return c.upsample_initial_ch
 int pack_conv(dsx_hifigan* h, PackedConv& pc, const float* v, const float* g, const float* bias, int cin, int cout,
               int k, int dil, int u, bool transposed, cudaStream_t s) {
   DSX_CHECK(v && bias, DSX_E_INVALID, "missing conv weight or bias");
-  pc.cin = cin;
+  pc.cin = round16(cin);
   pc.cout = cout;
-  pc.k = k;
-  pc.cin_p = round16(cin);
   pc.cout_p = round16(cout);
   if (transposed) {
     pc.u = u;
@@ -600,48 +481,24 @@ int pack_conv(dsx_hifigan* h, PackedConv& pc, const float* v, const float* g, co
     pc.tstep = dil;
     pc.n = pc.cout_p;
   }
-  pc.nt = pc.n <= 16 ? 16 : pc.n <= 32 ? 32 : pc.n <= 64 ? 64 : 128;
-  pc.ntiles = (pc.n + pc.nt - 1) / pc.nt;
-  pc.kc = (pc.taps * pc.cin_p + 63) / 64;
-  const size_t nw = static_cast<size_t>(pc.ntiles) * pc.kc * pc.nt * 64;
-  DSX_TRY(halloc(h, reinterpret_cast<void**>(&pc.w), nw * sizeof(__half)));
-  DSX_TRY(halloc(h, reinterpret_cast<void**>(&pc.b), static_cast<size_t>(pc.ntiles) * pc.nt * sizeof(float)));
-  const int d0 = transposed ? cin : cout;
-  k_wnorm<<<d0, 256, 0, s>>>(v, g, (transposed ? cout : cin) * k, h->scale);
-  DSX_TRY(ck("k_wnorm"));
-  PackArgs a{v, h->scale, bias, cin, cout, k, u, transposed ? 1 : 0, pc.cin_p, pc.cout_p, pc.taps, pc.n, pc.nt, pc.kc,
-             pc.ntiles, pc.w, pc.b};
-  const int blocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 4096));
-  k_pack_conv<<<blocks, 256, 0, s>>>(a);
-  return ck("k_pack_conv");
-}
-
-template <int NT>
-int launch_conv_nt(const ConvArgs& a, int mtiles, int ntiles, int B, cudaStream_t s) {
-  k_conv<NT><<<dim3(mtiles, ntiles, B), 128, conv_smem<NT>(), s>>>(a);
-  return ck("k_conv");
+  float* scale = static_cast<float*>(h->scale.ptr);
+  k_wnorm<<<transposed ? cin : cout, 256, 0, s>>>(v, g, (transposed ? cout : cin) * k, scale);
+  DSX_TRY(launch_check("k_wnorm"));
+  return conv_pack(h->mem, pc, 128, PackArgs{v, scale, bias, cin, cout, pc.cout_p, k, u, transposed ? 1 : 0}, s);
 }
 
 // one conv over the batch; rows_max = GEMM rows of the longest utterance
 int run_conv(const PackedConv& pc, ConvArgs a, int B, int rows_max, cudaStream_t s) {
-  a.cin_p = pc.cin_p;
-  a.taps = pc.taps;
-  a.tap0 = pc.tap0;
-  a.tstep = pc.tstep;
-  a.kc = pc.kc;
-  a.w = pc.w;
-  a.bias = pc.b;
-  a.n = pc.n;
+  a.g = pc;
   a.cout_p = pc.cout_p;
   a.u = pc.u;
   a.pad = pc.pad;
-  const int mtiles = (rows_max + kRowsPerCta - 1) / kRowsPerCta;
-  switch (pc.nt) {
-    case 16: return launch_conv_nt<16>(a, mtiles, pc.ntiles, B, s);
-    case 32: return launch_conv_nt<32>(a, mtiles, pc.ntiles, B, s);
-    case 64: return launch_conv_nt<64>(a, mtiles, pc.ntiles, B, s);
-    default: return launch_conv_nt<128>(a, mtiles, pc.ntiles, B, s);
-  }
+  const dim3 grid((rows_max + kConvRows - 1) / kConvRows, pc.ntiles, B);
+  return conv_dispatch<128>(pc.nt, [&](auto c) {
+    constexpr int NT = decltype(c)::value;
+    k_conv<NT><<<grid, 128, conv_smem<NT>(), s>>>(a);
+    return launch_check("k_conv");
+  });
 }
 
 // chain order of a block's convs: ResBlock1 convs1.0, convs2.0, convs1.1, ... (packed as convs1.*, convs2.*)
@@ -676,7 +533,7 @@ bool chain_usable(const dsx_hifigan* h, int stage) {
 template <int NT>
 int launch_chain_nt(const ChainArgs& a, int taps_max, int tiles, int B, cudaStream_t s) {
   k_chain<NT><<<dim3(tiles, B), 512, chain_smem<NT>(taps_max), s>>>(a);
-  return ck("k_chain");
+  return launch_check("k_chain");
 }
 
 int run_chain(const dsx_hifigan* h, int blk, const float* X, float* S, __half* P, const int* lens, int T, int mul,
@@ -757,22 +614,8 @@ int dsx_hifigan_create(int device, const dsx_hifigan_config* cfg, dsx_hifigan** 
   DSX_CHECK(out, DSX_E_INVALID, "out is NULL");
   *out = nullptr;
   DSX_TRY(validate(cfg));
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) {
-    set_error("no CUDA device available (%s); dsx has no CPU fallback", cudaGetErrorString(e));
-    return DSX_E_CUDA;
-  }
-  DSX_CHECK(device >= 0 && device < ndev, DSX_E_INVALID, "device %d out of range (%d devices)", device, ndev);
-  cudaDeviceProp prop;
-  DSX_CUDA(cudaGetDeviceProperties(&prop, device));
-  DSX_CHECK(prop.major == 9 && prop.minor == 0, DSX_E_CUDA,
-            "the vocoder's kernels are built for sm_90a; device %d is sm_%d%d", device, prop.major, prop.minor);
-  DSX_CUDA(cudaSetDevice(device));
-  DSX_CUDA(cudaFuncSetAttribute(k_conv<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv_smem<16>()));
-  DSX_CUDA(cudaFuncSetAttribute(k_conv<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv_smem<32>()));
-  DSX_CUDA(cudaFuncSetAttribute(k_conv<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv_smem<64>()));
-  DSX_CUDA(cudaFuncSetAttribute(k_conv<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv_smem<128>()));
+  DSX_TRY(select_sm90_device(device, "vocoder"));
+  DSX_TRY(conv_opt_in<128>([](auto c) { return k_conv<decltype(c)::value>; }));
   DSX_CUDA(cudaFuncSetAttribute(k_chain<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChainSmemMax));
   DSX_CUDA(cudaFuncSetAttribute(k_chain<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChainSmemMax));
   DSX_CUDA(cudaFuncSetAttribute(k_chain<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChainSmemMax));
@@ -790,8 +633,8 @@ void dsx_hifigan_destroy(dsx_hifigan* h) {
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();
   free_model(h);
-  if (h->scale) cudaFree(h->scale);
-  if (h->ws) cudaFree(h->ws);
+  h->scale.release();
+  h->ws.release();
   delete h;
 }
 
@@ -807,14 +650,7 @@ int dsx_hifigan_load(dsx_hifigan* h, const dsx_hifigan_params* p, void* stream) 
   DSX_CHECK(p->conv_post_w && p->conv_post_b, DSX_E_INVALID, "missing conv_post parameters");
   DSX_CUDA(cudaStreamSynchronize(s));   // the old packs may still be read by queued work
   free_model(h);
-  const size_t scale_need = static_cast<size_t>(std::max(c.upsample_initial_channel, kMelBins)) * sizeof(float);
-  if (h->scale_cap < scale_need) {
-    if (h->scale) cudaFree(h->scale);
-    h->scale = nullptr;
-    h->scale_cap = 0;
-    DSX_CUDA(cudaMalloc(&h->scale, scale_need));
-    h->scale_cap = scale_need;
-  }
+  DSX_TRY(h->scale.reserve(static_cast<size_t>(std::max(c.upsample_initial_channel, kMelBins)) * sizeof(float), s));
   const int c0 = c.upsample_initial_channel;
   DSX_TRY(pack_conv(h, h->pre, p->conv_pre_w, p->conv_pre_g, p->conv_pre_b, kMelBins, c0, 7, 1, 1, false, s));
   h->ups.resize(nu);
@@ -848,21 +684,22 @@ int dsx_hifigan_load(dsx_hifigan* h, const dsx_hifigan_params* p, void* stream) 
       DSX_CHECK(p->noise_w[i] && p->noise_b[i], DSX_E_INVALID, "missing noise_convs.%d", i);
       h->noise_s[i] = static_cast<int>(stride);
       h->noise_ks[i] = ks;
-      DSX_TRY(halloc(h, reinterpret_cast<void**>(&h->noise_w[i]), static_cast<size_t>(cp) * ks * sizeof(float)));
-      DSX_TRY(halloc(h, reinterpret_cast<void**>(&h->noise_b[i]), cp * sizeof(float)));
+      DSX_TRY(h->mem.alloc(&h->noise_w[i], static_cast<size_t>(cp) * ks * sizeof(float)));
+      DSX_TRY(h->mem.alloc(&h->noise_b[i], cp * sizeof(float)));
       k_pack_rows<<<(cp * ks + 255) / 256, 256, 0, s>>>(h->noise_w[i], p->noise_w[i], nullptr, cout, cp, ks);
       k_pack_rows<<<1, 256, 0, s>>>(h->noise_b[i], p->noise_b[i], nullptr, cout, cp, 1);
-      DSX_TRY(ck("k_pack_rows"));
+      DSX_TRY(launch_check("k_pack_rows"));
     }
-    DSX_TRY(halloc(h, reinterpret_cast<void**>(&h->src_w), (kHarmonics + 1) * sizeof(float)));
+    DSX_TRY(h->mem.alloc(&h->src_w, (kHarmonics + 1) * sizeof(float)));
     DSX_CUDA(cudaMemcpyAsync(h->src_w, p->source_w, kHarmonics * sizeof(float), cudaMemcpyDeviceToDevice, s));
     DSX_CUDA(cudaMemcpyAsync(h->src_w + kHarmonics, p->source_b, sizeof(float), cudaMemcpyDeviceToDevice, s));
   }
-  DSX_TRY(halloc(h, reinterpret_cast<void**>(&h->post_w), (static_cast<size_t>(cp_last) * 7 + 1) * sizeof(float)));
-  k_wnorm<<<1, 256, 0, s>>>(p->conv_post_w, p->conv_post_g, clast * 7, h->scale);
-  k_pack_rows<<<(cp_last * 7 + 255) / 256, 256, 0, s>>>(h->post_w, p->conv_post_w, h->scale, clast, cp_last, 7);
+  DSX_TRY(h->mem.alloc(&h->post_w, (static_cast<size_t>(cp_last) * 7 + 1) * sizeof(float)));
+  float* scale = static_cast<float*>(h->scale.ptr);
+  k_wnorm<<<1, 256, 0, s>>>(p->conv_post_w, p->conv_post_g, clast * 7, scale);
+  k_pack_rows<<<(cp_last * 7 + 255) / 256, 256, 0, s>>>(h->post_w, p->conv_post_w, scale, clast, cp_last, 7);
   DSX_CUDA(cudaMemcpyAsync(h->post_w + cp_last * 7, p->conv_post_b, sizeof(float), cudaMemcpyDeviceToDevice, s));
-  DSX_TRY(ck("conv_post pack"));
+  DSX_TRY(launch_check("conv_post pack"));
   h->loaded = true;
   return DSX_OK;
 }
@@ -892,51 +729,31 @@ int dsx_hifigan_forward(dsx_hifigan* h, const float* mel, dsx_strides ms, const 
   }
   act *= B;
   const size_t mel_e = static_cast<size_t>(B) * T * kMelBins;
-  auto al = [](size_t bytes) { return (bytes + 255) & ~size_t(255); };
-  const size_t b16 = al(act * 2), b32 = al(act * 4);
-  const size_t need = al(mel_e * 2) + 5 * b16 + 3 * b32 + (f0 ? al(static_cast<size_t>(B) * lh * 4) +
-                                                                 al(static_cast<size_t>(B) * T * kHarmonics * 8) : 0);
-  if (h->ws_cap < need) {
-    if (h->ws) {
-      DSX_CUDA(cudaStreamSynchronize(s));
-      cudaFree(h->ws);
-    }
-    h->ws = nullptr;
-    h->ws_cap = 0;
-    cudaError_t e = cudaMalloc(&h->ws, need + need / 8);
-    if (e != cudaSuccess) {
-      set_error("cudaMalloc(%zu) failed: %s", need + need / 8, cudaGetErrorString(e));
-      return e == cudaErrorMemoryAllocation ? DSX_E_NOMEM : DSX_E_CUDA;
-    }
-    h->ws_cap = need + need / 8;
-  }
-  uint8_t* wp = static_cast<uint8_t*>(h->ws);
-  auto take = [&](size_t bytes) { uint8_t* q = wp; wp += bytes; return q; };
-  __half* MEL = reinterpret_cast<__half*>(take(al(mel_e * 2)));
-  __half* P = reinterpret_cast<__half*>(take(b16));    // leaky_relu(stage input) -> ups
-  __half* Q = reinterpret_cast<__half*>(take(b16));    // leaky_relu(ups output) -> first conv of every block
-  __half* Tm = reinterpret_cast<__half*>(take(b16));   // ResBlock1: leaky_relu(convs1 output)
-  __half* U[2] = {reinterpret_cast<__half*>(take(b16)), reinterpret_cast<__half*>(take(b16))};
-  float* X = reinterpret_cast<float*>(take(b32));      // ups output (+ noise conv)
-  float* R = reinterpret_cast<float*>(take(b32));      // the running residual inside a block
-  float* S = reinterpret_cast<float*>(take(b32));      // multi-receptive-field sum
-  float* HAR = nullptr;
-  double* PH = nullptr;
-  if (f0) {
-    HAR = reinterpret_cast<float*>(take(al(static_cast<size_t>(B) * lh * 4)));
-    PH = reinterpret_cast<double*>(take(al(static_cast<size_t>(B) * T * kHarmonics * 8)));
-  }
+  const size_t har_b = static_cast<size_t>(B) * lh * 4, ph_b = static_cast<size_t>(B) * T * kHarmonics * 8;
+  DSX_TRY(h->ws.reserve(align256(mel_e * 2) + 5 * align256(act * 2) + 3 * align256(act * 4) +
+                        (f0 ? align256(har_b) + align256(ph_b) : 0), s));
+  Bump ws{static_cast<uint8_t*>(h->ws.ptr)};
+  __half* MEL = ws.take<__half>(mel_e * 2);
+  __half* P = ws.take<__half>(act * 2);    // leaky_relu(stage input) -> ups
+  __half* Q = ws.take<__half>(act * 2);    // leaky_relu(ups output) -> first conv of every block
+  __half* Tm = ws.take<__half>(act * 2);   // ResBlock1: leaky_relu(convs1 output)
+  __half* U[2] = {ws.take<__half>(act * 2), ws.take<__half>(act * 2)};
+  float* X = ws.take<float>(act * 4);      // ups output (+ noise conv)
+  float* R = ws.take<float>(act * 4);      // the running residual inside a block
+  float* S = ws.take<float>(act * 4);      // multi-receptive-field sum
+  float* HAR = f0 ? ws.take<float>(har_b) : nullptr;
+  double* PH = f0 ? ws.take<double>(ph_b) : nullptr;
 
   k_pack_mel<<<static_cast<unsigned>((mel_e + 255) / 256), 256, 0, s>>>(mel, ms, B, T, MEL);
-  DSX_TRY(ck("k_pack_mel"));
+  DSX_TRY(launch_check("k_pack_mel"));
   const float sr = static_cast<float>(c.audio_sample_rate);
   if (f0) {
     k_nsf_phase<<<B * kHarmonics, 256, 0, s>>>(f0, phase0, seed, T, h->hop, sr, PH);
-    DSX_TRY(ck("k_nsf_phase"));
+    DSX_TRY(launch_check("k_nsf_phase"));
     const size_t ns = static_cast<size_t>(B) * lh;
     k_nsf_source<<<static_cast<unsigned>((ns + 255) / 256), 256, 0, s>>>(f0, PH, src_noise, seed, h->src_w,
                                                                          h->src_w + kHarmonics, B, T, h->hop, sr, HAR);
-    DSX_TRY(ck("k_nsf_source"));
+    DSX_TRY(launch_check("k_nsf_source"));
   }
 
   ConvArgs base{};
@@ -1028,7 +845,7 @@ int dsx_hifigan_forward(dsx_hifigan* h, const float* mel, dsx_strides ms, const 
   k_post<<<static_cast<unsigned>((nwav + 255) / 256), 256, 0, s>>>(S, lh, round16(clast), clast, h->post_w,
                                                                    h->post_w + round16(clast) * 7, lengths, T, h->hop, B,
                                                                    wav);
-  return ck("k_post");
+  return launch_check("k_post");
 }
 
 }  // extern "C"

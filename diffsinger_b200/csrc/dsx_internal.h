@@ -34,6 +34,96 @@ void set_error(const char* fmt, ...);
     if (_r != DSX_OK) return _r; \
   } while (0)
 
+// ---- handle plumbing of the vocoder and the pitch extractor --------------------------------------
+// the error of the last launch, if any, as DSX_E_CUDA naming the kernel
+inline int launch_check(const char* what) {
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("%s: %s", what, cudaGetErrorString(e));
+    return DSX_E_CUDA;
+  }
+  return DSX_OK;
+}
+
+// cudaMalloc of at least one byte; out of memory is DSX_E_NOMEM, any other failure DSX_E_CUDA
+inline int checked_malloc(void** p, size_t bytes) {
+  cudaError_t e = cudaMalloc(p, bytes ? bytes : 1);
+  if (e != cudaSuccess) {
+    set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? DSX_E_NOMEM : DSX_E_CUDA;
+  }
+  return DSX_OK;
+}
+
+// device allocations freed together (a model's packed weights)
+struct DevAllocs {
+  std::vector<void*> ptrs;
+  template <typename T>
+  int alloc(T** p, size_t bytes) {
+    DSX_TRY(checked_malloc(reinterpret_cast<void**>(p), bytes));
+    ptrs.push_back(*p);
+    return DSX_OK;
+  }
+  void free_all() {
+    for (void* p : ptrs) cudaFree(p);
+    ptrs.clear();
+  }
+};
+
+// grow-only device buffer: when `need` bytes do not fit, waits for the queued work on s that may still read it, frees
+// it and allocates need + need / 8
+struct GrowBuffer {
+  void* ptr = nullptr;
+  size_t cap = 0;
+  int reserve(size_t need, cudaStream_t s) {
+    if (cap >= need) return DSX_OK;
+    if (ptr) {
+      DSX_CUDA(cudaStreamSynchronize(s));
+      cudaFree(ptr);
+    }
+    ptr = nullptr;
+    cap = 0;
+    DSX_TRY(checked_malloc(&ptr, need + need / 8));
+    cap = need + need / 8;
+    return DSX_OK;
+  }
+  void release() {
+    if (ptr) cudaFree(ptr);
+    ptr = nullptr;
+    cap = 0;
+  }
+};
+
+inline size_t align256(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+
+// hands out consecutive 256-byte-aligned pieces of a buffer of at least the sum of their align256 sizes
+struct Bump {
+  uint8_t* p;
+  template <typename T>
+  T* take(size_t bytes) {
+    T* q = reinterpret_cast<T*>(p);
+    p += align256(bytes);
+    return q;
+  }
+};
+
+// makes `device` current after checking that it exists and is sm_90, the only target of the kernels of `what`
+inline int select_sm90_device(int device, const char* what) {
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0) {
+    set_error("no CUDA device available (%s); dsx has no CPU fallback", cudaGetErrorString(e));
+    return DSX_E_CUDA;
+  }
+  DSX_CHECK(device >= 0 && device < ndev, DSX_E_INVALID, "device %d out of range (%d devices)", device, ndev);
+  cudaDeviceProp prop;
+  DSX_CUDA(cudaGetDeviceProperties(&prop, device));
+  DSX_CHECK(prop.major == 9 && prop.minor == 0, DSX_E_CUDA, "the %s's kernels are built for sm_90a; device %d is sm_%d%d",
+            what, device, prop.major, prop.minor);
+  DSX_CUDA(cudaSetDevice(device));
+  return DSX_OK;
+}
+
 constexpr int kTile = 128;  // frames per tile: the frame axis of every utterance is padded to a multiple of it
 
 // Geometry of one call: B utterances of T frames, stored frames-major with the frame axis

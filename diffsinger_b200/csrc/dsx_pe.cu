@@ -1,13 +1,12 @@
 // Pitch extractor on sm_90a: mel [B, T, 80] -> pitch_pred [B, T, 2] and the denormalised f0 [B, T]
 // (modules/fastspeech/pe.py:119-149: Prenet, ConvStacks with GroupNorm, PitchPredictor, utils/pitch_utils.py:denorm_f0).
 //
-// Every conv and linear is one implicit GEMM on wgmma (k_pe_conv).  Activations are frames-major fp16 [B][T][C]; row m of
-// the GEMM is a frame, the K axis is (tap j, input channel c), and tap j reads frame m + tap0 + j, zero outside [0, T).
-// That one rule is the prenet's zero padding (tap0 = -2), the PitchPredictor's ConstantPad1d 'SAME' (tap0 = -(k-1)/2) and
-// 'LEFT' (tap0 = -(k-1)), and a linear (one tap).  A CTA covers 64 frames x ALL output channels (N <= 256), so a row's
-// normalisation and the head's P -> 2 linear run in the epilogue from registers: one warpgroup up to N = 128; at N = 256
-// two warpgroups share the A tile, each with its 128 columns (m64n128) and a row reduction through shared memory.  Operands reach shared memory by cp.async in the 128-byte-swizzled layout of dsx_ptx.cuh, double buffered per
-// 64-wide K chunk.  Epilogues by mode:
+// Every conv and linear is one implicit GEMM on wgmma (k_pe_conv, on the core of dsx_conv.cuh) over frames-major fp16
+// [B][T][C]: tap j reads frame m + tap0 + j, zero outside [0, T).  That one rule is the prenet's zero padding (tap0 = -2),
+// the PitchPredictor's ConstantPad1d 'SAME' (tap0 = -(k-1)/2) and 'LEFT' (tap0 = -(k-1)), and a linear (one tap).  A CTA
+// covers 64 frames x ALL output channels (N <= 256), so a row's normalisation and the head's P -> 2 linear run in the
+// epilogue from registers: one warpgroup up to N = 128; at N = 256 two warpgroups share the A tile, each with its 128
+// columns (m64n128) and a row reduction through shared memory.  Epilogues by mode:
 //   PE_PRENET  bias, ReLU, BatchNorm (eval: per-channel scale and shift packed at load), padding mask -> fp16
 //   PE_LINEAR  bias, optional padding mask -> fp32 and / or fp16
 //   PE_GN      bias -> fp32 pre-norm values, plus per-tile, per-16-channel-group (count, mean, M2) partials
@@ -21,6 +20,7 @@
 
 #include <algorithm>
 
+#include "dsx_conv.cuh"
 #include "dsx_internal.h"
 #include "dsx_ptx.cuh"
 
@@ -28,7 +28,6 @@ namespace dsx {
 namespace {
 
 constexpr int kPeMel = 80;
-constexpr int kPeRows = 64;           // frames per CTA
 constexpr int kPePrenetLayers = 3, kPePredLayers = 5, kPeEncKernel = 5, kPePrenetKernel = 5;
 constexpr int kPeMaxConvLayers = 16;
 constexpr float kBnEps = 1e-5f, kGnEps = 1e-5f, kLnEps = 1e-12f;
@@ -36,20 +35,16 @@ constexpr float kBnEps = 1e-5f, kGnEps = 1e-5f, kLnEps = 1e-12f;
 enum { PE_PRENET = 0, PE_LINEAR = 1, PE_GN = 2, PE_LN = 3, PE_HEAD = 4 };
 enum { PE_MASK = 1, PE_OUT32 = 2, PE_OUT16 = 4 };
 
-struct PePacked {
-  int cin = 0, n = 0, taps = 0, tap0 = 0, nt = 0, kc = 0;
-  __half* w = nullptr;         // [kc][nt][64] fp16, K index = tap * cin + channel, zero padded
-  float* b = nullptr;          // [nt]
+// one conv or linear: its GEMM (one column tile) and the per-channel affine of its epilogue
+struct PePacked : ConvGemm {
   float* s = nullptr;          // per-channel scale (BatchNorm, GroupNorm / LayerNorm weight) [n], or null
   float* t = nullptr;          // per-channel shift [n], or null
 };
 
 struct PeConvArgs {
-  const __half* x;             // [B][T][cin]
-  int cin, taps, tap0, kc;
-  const __half* w;
-  const float* bias;
-  int n, T, mode, flags;
+  ConvGemm g;
+  const __half* x;             // [B][T][g.cin]
+  int T, mode, flags;
   const float* scale;          // PE_PRENET: BN scale; PE_LN / PE_HEAD: LayerNorm weight
   const float* shift;          // PE_PRENET: BN shift; PE_LN / PE_HEAD: LayerNorm bias
   const uint8_t* pad;          // [B][T] 1 = padding frame
@@ -71,9 +66,6 @@ struct PeShape {
   static constexpr int NH = NT / WG;
 };
 
-template <int NT>
-constexpr int pe_smem() { return 2 * (kPeRows * 128 + NT * 128) + 1024; }
-
 // sum over the 4 threads of an accumulator quad (they hold the same two rows)
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
@@ -83,62 +75,20 @@ __device__ __forceinline__ float quad_sum(float v) {
 
 template <int NT>
 __global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvArgs p) {
-  constexpr int NH = PeShape<NT>::NH, WG = PeShape<NT>::WG, NTHR = 128 * WG;
+  constexpr int NH = PeShape<NT>::NH, WG = PeShape<NT>::WG;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr int kA = kPeRows * 128, kB = NT * 128, kStage = kA + kB;
   __shared__ float red[4 * WG][16];
   __shared__ float gmean[16];
-  __shared__ float xrow[WG][kPeRows];   // per-warpgroup row partials of the LayerNorm / head reductions
-  const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127, b = blockIdx.y, m0 = blockIdx.x * kPeRows;
+  __shared__ float xrow[WG][kConvRows];   // per-warpgroup row partials of the LayerNorm / head reductions
+  const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127, b = blockIdx.y, m0 = blockIdx.x * kConvRows;
   const int T = p.T;
 
-  auto load = [&](int s, uint8_t* buf) {
-    const uint32_t da = smem_u32(buf), db = smem_u32(buf + kA);
-    for (int i = tid; i < kPeRows * 8; i += NTHR) {
-      const int r = i >> 3, c = i & 7;
-      const int kk = s * 64 + c * 8, j = kk / p.cin, ch = kk - j * p.cin;
-      const int src = m0 + r + p.tap0 + j;
-      const bool valid = j < p.taps && src >= 0 && src < T;
-      cp16(da + sw128(r, c), p.x + (static_cast<size_t>(b) * T + (valid ? src : 0)) * p.cin + (valid ? ch : 0), valid);
-    }
-    const __half* wsrc = p.w + static_cast<size_t>(s) * NT * 64;
-    for (int i = tid; i < NT * 8; i += NTHR) {
-      const int r = i >> 3, c = i & 7;
-      cp16(db + sw128(r, c), wsrc + r * 64 + c * 8, true);
-    }
-  };
-
   float acc[NH / 2];
-#pragma unroll
-  for (int e = 0; e < NH / 2; ++e) acc[e] = 0.f;
-  load(0, smem);
-  cp_commit();
-#pragma unroll 1
-  for (int s = 0; s < p.kc; ++s) {
-    uint8_t* cur = smem + (s & 1) * kStage;
-    if (s + 1 < p.kc) {
-      load(s + 1, smem + ((s + 1) & 1) * kStage);
-      cp_commit();
-      cp_wait<1>();
-    } else {
-      cp_wait<0>();
-    }
-    fence_proxy_async_smem();
-    __syncthreads();
-    const uint64_t da = wg_desc(smem_u32(cur)), db = wg_desc(smem_u32(cur + kA + wg * NH * 128));
-    wg_fence();
-#pragma unroll
-    for (int k4 = 0; k4 < 4; ++k4) wgmma_f16<NH>(acc, da + 2 * k4, db + 2 * k4, 1);
-    wg_commit();
-    wg_wait0();
-#pragma unroll
-    for (int e = 0; e < NH / 2; ++e) asm volatile("" : "+f"(acc[e])::"memory");
-    __syncthreads();
-  }
+  conv_k_loop<NT, WG>(p.g, p.x, T, T, b, m0, 0, smem, acc);
 
   // ---- epilogue: thread wtid holds rows r0 = acc_row(wtid, 0) (e & 2 == 0) and r0 + 8 (e & 2 != 0) ----
-  const int n = p.n, c0 = wg * NH;
+  const int n = p.g.n, c0 = wg * NH;
   const int r0 = acc_row(wtid, 0);
   const int mrow[2] = {m0 + r0, m0 + r0 + 8};
   const size_t rbase = static_cast<size_t>(b) * T;
@@ -161,7 +111,7 @@ __global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvA
 #pragma unroll
   for (int e = 0; e < NH / 2; ++e) {
     const int col = c0 + acc_col(wtid, e);
-    float v = col < n ? acc[e] + __ldg(p.bias + col) : 0.f;
+    float v = col < n ? acc[e] + __ldg(p.g.b + col) : 0.f;
     if (p.mode == PE_PRENET || p.mode == PE_LN || p.mode == PE_HEAD) v = fmaxf(v, 0.f);
     acc[e] = v;
   }
@@ -169,7 +119,7 @@ __global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvA
   if (p.mode == PE_GN) {
     // per 16-channel group: count, mean and M2 over the tile's valid rows, two passes, fixed reduction order.  Local
     // group gl of this warpgroup (global group c0 / 16 + gl) is elements e in [8 gl, 8 gl + 8).
-    const int rows = min(kPeRows, T - m0);
+    const int rows = min(kConvRows, T - m0);
     const bool ok0 = r0 < rows, ok1 = r0 + 8 < rows;
     const int warp = tid >> 5, lane = tid & 31;
     const int groups = n / 16;
@@ -380,24 +330,6 @@ __global__ void k_pe_posadd(const float* x, const int* pos, const float* alpha, 
   out[i] = __float2half_rn(x[i] + alpha[0] * tab);
 }
 
-// ---- weight packing ------------------------------------------------------------------------------
-// Conv1d [n][cin][k] (Linear: k = 1) -> fp16 [kc][nt][64], K index kk = tap * cin + channel, zero padded; bias -> [nt]
-__global__ void k_pe_pack(const float* w, const float* bias, int cin, int n, int k, int nt, int kc, __half* wp,
-                          float* bp) {
-  const size_t total = static_cast<size_t>(kc) * nt * 64;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int q = static_cast<int>(i & 63);
-    const size_t t = i >> 6;
-    const int r = static_cast<int>(t % nt), s = static_cast<int>(t / nt);
-    const int kk = s * 64 + q, j = kk / cin, c = kk - j * cin;
-    float v = 0.f;
-    if (r < n && j < k) v = w[(static_cast<size_t>(r) * cin + c) * k + j];
-    wp[i] = __float2half_rn(v);
-    if (i < static_cast<size_t>(nt)) bp[i] = static_cast<int>(i) < n ? bias[i] : 0.f;
-  }
-}
-
 // BatchNorm1d in eval mode as y = x * scale + shift: scale = w / sqrt(var + eps), shift = b - mean * scale
 __global__ void k_pe_bn(const float* w, const float* b, const float* mean, const float* var, int n, float* scale,
                         float* shift) {
@@ -407,17 +339,6 @@ __global__ void k_pe_bn(const float* w, const float* b, const float* mean, const
   scale[i] = s;
   shift[i] = b[i] - mean[i] * s;
 }
-
-int pe_ck(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("%s: %s", what, cudaGetErrorString(e));
-    return DSX_E_CUDA;
-  }
-  return DSX_OK;
-}
-
-int pe_nt(int n) { return n <= 16 ? 16 : n <= 32 ? 32 : n <= 64 ? 64 : n <= 128 ? 128 : 256; }
 
 }  // namespace
 }  // namespace dsx
@@ -433,38 +354,26 @@ struct dsx_pe {
   std::vector<PePacked> enc;
   float* head = nullptr;       // linear.weight [2][P], bias [2]
   float* alpha = nullptr;      // pos_embed_alpha [1]
-  std::vector<void*> owned;
-  void* ws = nullptr;
-  size_t ws_cap = 0;
+  DevAllocs mem;               // the packs above
+  GrowBuffer ws;               // workspace of a forward call
 };
 
 namespace {
 
-int pe_alloc(dsx_pe* h, void** p, size_t bytes) {
-  cudaError_t e = cudaMalloc(p, bytes ? bytes : 1);
-  if (e != cudaSuccess) {
-    set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
-    return e == cudaErrorMemoryAllocation ? DSX_E_NOMEM : DSX_E_CUDA;
-  }
-  h->owned.push_back(*p);
-  return DSX_OK;
-}
-
 void pe_free_model(dsx_pe* h) {
-  for (void* p : h->owned) cudaFree(p);
-  h->owned.clear();
+  h->mem.free_all();
   h->enc.clear();
   h->loaded = false;
 }
 
 int pe_copy(dsx_pe* h, float** dst, const float* src, int n, const char* what, cudaStream_t s) {
   DSX_CHECK(src, DSX_E_INVALID, "missing %s", what);
-  DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(dst), static_cast<size_t>(n) * sizeof(float)));
+  DSX_TRY(h->mem.alloc(dst, static_cast<size_t>(n) * sizeof(float)));
   DSX_CUDA(cudaMemcpyAsync(*dst, src, static_cast<size_t>(n) * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return DSX_OK;
 }
 
-// pack one conv (k taps starting at tap0) or linear (k = 1, tap0 = 0) of cin -> n channels
+// pack one conv (k taps starting at tap0) or linear (k = 1, tap0 = 0) of cin -> n channels, all n in one column tile
 int pe_pack(dsx_pe* h, PePacked& pc, const float* w, const float* b, int cin, int n, int k, int tap0, const char* what,
             cudaStream_t s) {
   DSX_CHECK(w && b, DSX_E_INVALID, "missing %s weight or bias", what);
@@ -472,38 +381,17 @@ int pe_pack(dsx_pe* h, PePacked& pc, const float* w, const float* b, int cin, in
   pc.n = n;
   pc.taps = k;
   pc.tap0 = tap0;
-  pc.nt = pe_nt(n);
-  pc.kc = (k * cin + 63) / 64;
-  const size_t nw = static_cast<size_t>(pc.kc) * pc.nt * 64;
-  DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(&pc.w), nw * sizeof(__half)));
-  DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(&pc.b), static_cast<size_t>(pc.nt) * sizeof(float)));
-  const int blocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 4096));
-  k_pe_pack<<<blocks, 256, 0, s>>>(w, b, cin, n, k, pc.nt, pc.kc, pc.w, pc.b);
-  return pe_ck("k_pe_pack");
-}
-
-template <int NT>
-int pe_launch(const PeConvArgs& a, int mtiles, int B, cudaStream_t s) {
-  k_pe_conv<NT><<<dim3(mtiles, B), 128 * PeShape<NT>::WG, pe_smem<NT>(), s>>>(a);
-  return pe_ck("k_pe_conv");
+  return conv_pack(h->mem, pc, 256, PackArgs{w, nullptr, b, cin, n, n, k, 1, 0}, s);
 }
 
 int pe_run(const PePacked& pc, PeConvArgs a, int B, cudaStream_t s) {
-  a.cin = pc.cin;
-  a.taps = pc.taps;
-  a.tap0 = pc.tap0;
-  a.kc = pc.kc;
-  a.w = pc.w;
-  a.bias = pc.b;
-  a.n = pc.n;
-  a.mtiles = (a.T + kPeRows - 1) / kPeRows;
-  switch (pc.nt) {
-    case 16: return pe_launch<16>(a, a.mtiles, B, s);
-    case 32: return pe_launch<32>(a, a.mtiles, B, s);
-    case 64: return pe_launch<64>(a, a.mtiles, B, s);
-    case 128: return pe_launch<128>(a, a.mtiles, B, s);
-    default: return pe_launch<256>(a, a.mtiles, B, s);
-  }
+  a.g = pc;
+  a.mtiles = (a.T + kConvRows - 1) / kConvRows;
+  return conv_dispatch<256>(pc.nt, [&](auto c) {
+    constexpr int NT = decltype(c)::value;
+    k_pe_conv<NT><<<dim3(a.mtiles, B), 128 * PeShape<NT>::WG, conv_smem<NT>(), s>>>(a);
+    return launch_check("k_pe_conv");
+  });
 }
 
 int pe_validate(const dsx_pe_config* c) {
@@ -533,23 +421,8 @@ int dsx_pe_create(int device, const dsx_pe_config* cfg, dsx_pe** out) {
   DSX_CHECK(out, DSX_E_INVALID, "out is NULL");
   *out = nullptr;
   DSX_TRY(pe_validate(cfg));
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) {
-    set_error("no CUDA device available (%s); dsx has no CPU fallback", cudaGetErrorString(e));
-    return DSX_E_CUDA;
-  }
-  DSX_CHECK(device >= 0 && device < ndev, DSX_E_INVALID, "device %d out of range (%d devices)", device, ndev);
-  cudaDeviceProp prop;
-  DSX_CUDA(cudaGetDeviceProperties(&prop, device));
-  DSX_CHECK(prop.major == 9 && prop.minor == 0, DSX_E_CUDA,
-            "the pitch extractor's kernels are built for sm_90a; device %d is sm_%d%d", device, prop.major, prop.minor);
-  DSX_CUDA(cudaSetDevice(device));
-  DSX_CUDA(cudaFuncSetAttribute(k_pe_conv<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, pe_smem<16>()));
-  DSX_CUDA(cudaFuncSetAttribute(k_pe_conv<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, pe_smem<32>()));
-  DSX_CUDA(cudaFuncSetAttribute(k_pe_conv<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, pe_smem<64>()));
-  DSX_CUDA(cudaFuncSetAttribute(k_pe_conv<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, pe_smem<128>()));
-  DSX_CUDA(cudaFuncSetAttribute(k_pe_conv<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, pe_smem<256>()));
+  DSX_TRY(select_sm90_device(device, "pitch extractor"));
+  DSX_TRY(conv_opt_in<256>([](auto c) { return k_pe_conv<decltype(c)::value>; }));
   dsx_pe* h = new dsx_pe();
   h->device = device;
   h->cfg = *cfg;
@@ -563,7 +436,7 @@ void dsx_pe_destroy(dsx_pe* h) {
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();
   pe_free_model(h);
-  if (h->ws) cudaFree(h->ws);
+  h->ws.release();
   delete h;
 }
 
@@ -586,10 +459,10 @@ int dsx_pe_load(dsx_pe* h, const dsx_pe_params* p, void* stream) {
     DSX_TRY(pe_pack(h, pc, p->prenet_w[i], p->prenet_b[i], i ? H : kPeMel, H, kPePrenetKernel, -kPePrenetKernel / 2,
                     what, s));
     DSX_CHECK(p->bn_w[i] && p->bn_b[i] && p->bn_mean[i] && p->bn_var[i], DSX_E_INVALID, "missing mel_prenet.layers.%d.2", i);
-    DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(&pc.s), H * sizeof(float)));
-    DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(&pc.t), H * sizeof(float)));
+    DSX_TRY(h->mem.alloc(&pc.s, H * sizeof(float)));
+    DSX_TRY(h->mem.alloc(&pc.t, H * sizeof(float)));
     k_pe_bn<<<(H + 255) / 256, 256, 0, s>>>(p->bn_w[i], p->bn_b[i], p->bn_mean[i], p->bn_var[i], H, pc.s, pc.t);
-    DSX_TRY(pe_ck("k_pe_bn"));
+    DSX_TRY(launch_check("k_pe_bn"));
   }
   DSX_TRY(pe_pack(h, h->prenet_out, p->prenet_out_w, p->prenet_out_b, H, H, 1, 0, "mel_prenet.out_proj", s));
   if (L > 0) {
@@ -613,7 +486,7 @@ int dsx_pe_load(dsx_pe* h, const dsx_pe_params* p, void* stream) {
   }
   DSX_CHECK(p->linear_w && p->linear_b && p->pos_embed_alpha, DSX_E_INVALID,
             "missing pitch_predictor.linear or pos_embed_alpha");
-  DSX_TRY(pe_alloc(h, reinterpret_cast<void**>(&h->head), (2 * P + 2) * sizeof(float)));
+  DSX_TRY(h->mem.alloc(&h->head, (2 * P + 2) * sizeof(float)));
   DSX_CUDA(cudaMemcpyAsync(h->head, p->linear_w, 2 * P * sizeof(float), cudaMemcpyDeviceToDevice, s));
   DSX_CUDA(cudaMemcpyAsync(h->head + 2 * P, p->linear_b, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
   DSX_TRY(pe_copy(h, &h->alpha, p->pos_embed_alpha, 1, "pos_embed_alpha", s));
@@ -638,36 +511,21 @@ int dsx_pe_forward(dsx_pe* h, const float* mel, dsx_strides ms, int B, int T, fl
 
   // workspace: fp16 MEL / A0 / A1, fp32 X / Y, padding flags, positions, GroupNorm partials
   const size_t frames = static_cast<size_t>(B) * T;
-  const int mtiles = (T + kPeRows - 1) / kPeRows;
-  auto al = [](size_t bytes) { return (bytes + 255) & ~size_t(255); };
-  const size_t need = al(frames * kPeMel * 2) + 2 * al(frames * C * 2) + 2 * al(frames * H * 4) + al(frames) +
-                      al(frames * 4) + al(static_cast<size_t>(B) * mtiles * (H / 16) * 3 * 4);
-  if (h->ws_cap < need) {
-    if (h->ws) {
-      DSX_CUDA(cudaStreamSynchronize(s));
-      cudaFree(h->ws);
-    }
-    h->ws = nullptr;
-    h->ws_cap = 0;
-    cudaError_t e = cudaMalloc(&h->ws, need + need / 8);
-    if (e != cudaSuccess) {
-      set_error("cudaMalloc(%zu) failed: %s", need + need / 8, cudaGetErrorString(e));
-      return e == cudaErrorMemoryAllocation ? DSX_E_NOMEM : DSX_E_CUDA;
-    }
-    h->ws_cap = need + need / 8;
-  }
-  uint8_t* wp = static_cast<uint8_t*>(h->ws);
-  auto take = [&](size_t bytes) { uint8_t* q = wp; wp += al(bytes); return q; };
-  __half* MEL = reinterpret_cast<__half*>(take(frames * kPeMel * 2));
-  __half* A[2] = {reinterpret_cast<__half*>(take(frames * C * 2)), reinterpret_cast<__half*>(take(frames * C * 2))};
-  float* X = reinterpret_cast<float*>(take(frames * H * 4));
-  float* Y = reinterpret_cast<float*>(take(frames * H * 4));
-  uint8_t* PAD = take(frames);
-  int* POS = reinterpret_cast<int*>(take(frames * 4));
-  float* ST = reinterpret_cast<float*>(take(static_cast<size_t>(B) * mtiles * (H / 16) * 3 * 4));
+  const int mtiles = (T + kConvRows - 1) / kConvRows;
+  const size_t st_b = static_cast<size_t>(B) * mtiles * (H / 16) * 3 * 4;
+  DSX_TRY(h->ws.reserve(align256(frames * kPeMel * 2) + 2 * align256(frames * C * 2) + 2 * align256(frames * H * 4) +
+                        align256(frames) + align256(frames * 4) + align256(st_b), s));
+  Bump ws{static_cast<uint8_t*>(h->ws.ptr)};
+  __half* MEL = ws.take<__half>(frames * kPeMel * 2);
+  __half* A[2] = {ws.take<__half>(frames * C * 2), ws.take<__half>(frames * C * 2)};
+  float* X = ws.take<float>(frames * H * 4);
+  float* Y = ws.take<float>(frames * H * 4);
+  uint8_t* PAD = ws.take<uint8_t>(frames);
+  int* POS = ws.take<int>(frames * 4);
+  float* ST = ws.take<float>(st_b);
 
   k_pe_pack_mel<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(mel, ms, B, T, MEL, PAD);
-  DSX_TRY(pe_ck("k_pe_pack_mel"));
+  DSX_TRY(launch_check("k_pe_pack_mel"));
 
   PeConvArgs base{};
   base.T = T;
@@ -716,7 +574,7 @@ int dsx_pe_forward(dsx_pe* h, const float* mel, dsx_strides ms, int B, int T, fl
       DSX_TRY(pe_run(h->enc[i], a, B, s));
       k_pe_gn<<<dim3((T + kGnRows - 1) / kGnRows, B), 256, 0, s>>>(Y, ST, mtiles, h->enc[i].s, h->enc[i].t, T, H, X,
                                                                    A[cur ^ 1]);
-      DSX_TRY(pe_ck("k_pe_gn"));
+      DSX_TRY(launch_check("k_pe_gn"));
       cur ^= 1;
     }
     a = base;
@@ -729,12 +587,12 @@ int dsx_pe_forward(dsx_pe* h, const float* mel, dsx_strides ms, int B, int T, fl
   // PitchPredictor (tts_modules.py:222-235): + alpha * position embedding, 4 x [conv, ReLU, LayerNorm], the head
   const float* xs = L > 0 ? Y : X;
   k_pe_scan<<<B, kScanThreads, 0, s>>>(xs, T, H, POS);
-  DSX_TRY(pe_ck("k_pe_scan"));
+  DSX_TRY(launch_check("k_pe_scan"));
   const float neg_emb = -static_cast<float>(log(10000.0) / (H / 2 - 1));
   const size_t ne = frames * H;
   k_pe_posadd<<<static_cast<unsigned>((ne + 255) / 256), 256, 0, s>>>(xs, POS, h->alpha, static_cast<int>(frames), H,
                                                                       neg_emb, A[0]);
-  DSX_TRY(pe_ck("k_pe_posadd"));
+  DSX_TRY(launch_check("k_pe_posadd"));
   cur = 0;
   for (int i = 0; i < kPePredLayers; ++i) {
     a = base;

@@ -7,15 +7,13 @@ hold the parameters: ``forward`` packs them into the library (once per storage a
 ``load_state_dict`` or ``.to()``) and runs the whole extractor there, mel to denormalised f0.  There is no eager or CPU
 path and no training path: a CPU tensor or a module in training mode raises ``DsxError``.
 """
-import ctypes
-
 import torch
 import torch.nn as nn
 
 from . import _capi
 from ._capi import DsxError, check, lib
 from .modules import _get_hparams
-from .sampler import _need_cuda, _ptr, _stream, _strides_bct
+from .sampler import PackedModule, _need_cuda, _ptr, _stream, _strides_bct
 
 
 class Prenet(nn.Module):
@@ -121,7 +119,7 @@ def _pe_config(hp, n_mel_bins, conv_layers):
     return cfg
 
 
-class PitchExtractor(nn.Module):
+class PitchExtractor(PackedModule):
     def __init__(self, n_mel_bins=80, conv_layers=2, hparams=None):
         super().__init__()
         hp = _get_hparams(hparams)
@@ -135,48 +133,15 @@ class PitchExtractor(nn.Module):
         self.pitch_predictor = PitchPredictor(self.hidden_size, n_chans=self.predictor_hidden, n_layers=5,
                                               dropout_rate=0.1, odim=2, padding=hp['ffn_padding'],
                                               kernel_size=self._cfg.predictor_kernel)
-        self._dsx = None          # (handle, device)
-        self._wkey = None
-        self._keep = None
 
     # -- library handle ---------------------------------------------------------------------------
-    def close(self):
-        if self._dsx is not None:
-            lib.dsx_pe_destroy(self._dsx[0])
-            self._dsx, self._wkey, self._keep = None, None, None
+    _lib_create, _lib_load, _lib_destroy = lib.dsx_pe_create, lib.dsx_pe_load, lib.dsx_pe_destroy
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def _config(self):
+        return self._cfg
 
-    def _ensure(self, device):
-        if self._dsx is not None and self._dsx[1] != device:
-            self.close()
-        if self._dsx is None:
-            hnd = ctypes.c_void_p()
-            check(lib.dsx_pe_create(device.index if device.index is not None else torch.cuda.current_device(),
-                                    ctypes.byref(self._cfg), ctypes.byref(hnd)), "dsx_pe_create")
-            self._dsx = (hnd, device)
-        hnd = self._dsx[0]
-        sd = self.state_dict()
-        key = tuple((k, v.data_ptr(), v._version, tuple(v.shape)) for k, v in sd.items())
-        if key == self._wkey:
-            return hnd
-        keep = []
-
-        def t(name):
-            x = sd[name].detach().to(device=device, dtype=torch.float32).contiguous()
-            keep.append(x)
-            return x.data_ptr()
-
-        def arr(names):
-            a = (ctypes.c_void_p * len(names))(*[t(n) for n in names])
-            keep.append(a)
-            return ctypes.cast(a, ctypes.POINTER(ctypes.c_void_p))
-
-        pre = [f"mel_prenet.layers.{i}" for i in range(3)]
+    def _params(self, sd, t, arr):
+        pre =[f"mel_prenet.layers.{i}" for i in range(3)]
         enc = [f"mel_encoder.conv.{i}" for i in range(self.conv_layers)]
         pred = [f"pitch_predictor.conv.{i}" for i in range(5)]
         p = _capi.PeParams(
@@ -193,10 +158,7 @@ class PitchExtractor(nn.Module):
             p.enc_w, p.enc_b = arr([n + ".conv.conv.weight" for n in enc]), arr([n + ".conv.conv.bias" for n in enc])
             p.gn_w, p.gn_b = arr([n + ".norm.weight" for n in enc]), arr([n + ".norm.bias" for n in enc])
             p.enc_out_w, p.enc_out_b = t("mel_encoder.out_proj.weight"), t("mel_encoder.out_proj.bias")
-        with torch.cuda.device(device):
-            check(lib.dsx_pe_load(hnd, ctypes.byref(p), _stream(device)), "dsx_pe_load")
-        self._wkey, self._keep = key, keep
-        return hnd
+        return p
 
     def forward(self, mel_input=None):
         """mel_input: [B, T, n_mel_bins] (any strides; dsx_infer's mel_out as it is).  A frame whose bins are all 0 is

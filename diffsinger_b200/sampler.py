@@ -7,6 +7,7 @@ import ctypes
 import os
 
 import torch
+import torch.nn as nn
 
 from . import _capi
 from ._capi import DsxError, Strides, check, lib
@@ -30,6 +31,64 @@ def _need_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise DsxError("dsx runs on CUDA tensors only -- there is no CPU fallback (got a CPU tensor)")
+
+
+class PackedModule(nn.Module):
+    """A module that only holds parameters and runs in a dsx handle of its own (the vocoder, the pitch extractor).
+
+    Subclasses set ``_lib_create`` / ``_lib_load`` / ``_lib_destroy`` to their dsx_*_create / _load / _destroy and define
+    ``_config()`` (the create config) and ``_params(sd, t, arr)`` (the load params).  The handle is made per device, and
+    the parameters are packed again whenever a state-dict entry changes storage, version or shape."""
+
+    def __init__(self):
+        super().__init__()
+        self._dsx = None          # (handle, device)
+        self._wkey = None
+        self._keep = None
+
+    def close(self):
+        if self._dsx is not None:
+            self._lib_destroy(self._dsx[0])
+            self._dsx, self._wkey, self._keep = None, None, None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _ensure(self, device):
+        if self._dsx is not None and self._dsx[1] != device:
+            self.close()
+        if self._dsx is None:
+            hnd = ctypes.c_void_p()
+            check(self._lib_create(device.index if device.index is not None else torch.cuda.current_device(),
+                                   ctypes.byref(self._config()), ctypes.byref(hnd)), self._lib_create.__name__)
+            self._dsx = (hnd, device)
+        hnd = self._dsx[0]
+        sd = self.state_dict()
+        key = tuple((k, v.data_ptr(), v._version, tuple(v.shape)) for k, v in sd.items())
+        if key == self._wkey:
+            return hnd
+        keep = []
+
+        def t(name):
+            """Device pointer of state-dict entry `name` as contiguous fp32, kept alive until the next load."""
+            x = sd[name].detach().to(device=device, dtype=torch.float32).contiguous()
+            keep.append(x)
+            return x.data_ptr()
+
+        def arr(vals):
+            """C array of pointers: a str entry is a state-dict name (see t), anything else a pointer or None."""
+            a = (ctypes.c_void_p * len(vals))(*[t(v) if isinstance(v, str) else v for v in vals])
+            keep.append(a)
+            return ctypes.cast(a, ctypes.POINTER(ctypes.c_void_p))
+
+        p = self._params(sd, t, arr)
+        with torch.cuda.device(device):
+            check(self._lib_load(hnd, ctypes.byref(p), _stream(device)), self._lib_load.__name__)
+        self._wkey, self._keep = key, keep
+        return hnd
 
 
 def default_precision():

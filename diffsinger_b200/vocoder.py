@@ -6,8 +6,6 @@
 library (once per storage and version, so again after ``load_state_dict``, ``remove_weight_norm`` or ``.to()``) and
 runs the whole generator there.  There is no eager or CPU path: a CPU tensor raises ``DsxError``.
 """
-import ctypes
-
 import numpy as np
 import torch
 import torch.nn as nn
@@ -16,7 +14,7 @@ from torch.nn.utils import remove_weight_norm, weight_norm
 
 from . import _capi
 from ._capi import DsxError, check, lib
-from .sampler import _need_cuda, _ptr, _stream, _strides_bct
+from .sampler import PackedModule, _need_cuda, _ptr, _stream, _strides_bct
 
 HARMONIC_NUM = 8
 
@@ -68,7 +66,7 @@ class SourceModuleHnNSF(nn.Module):
         self.l_linear = nn.Linear(harmonic_num + 1, 1)
 
 
-class HifiGanGenerator(nn.Module):
+class HifiGanGenerator(PackedModule):
     def __init__(self, h, c_out=1):
         super().__init__()
         self.h = h
@@ -100,9 +98,6 @@ class HifiGanGenerator(nn.Module):
         self.conv_post = weight_norm(Conv1d(ch, c_out, 7, 1, padding=3))
         self.ups.apply(_init_weights)
         self.conv_post.apply(_init_weights)
-        self._dsx = None          # (handle, device)
-        self._wkey = None
-        self._keep = None
 
     def remove_weight_norm(self):
         for l in self.ups:
@@ -113,6 +108,8 @@ class HifiGanGenerator(nn.Module):
         remove_weight_norm(self.conv_post)
 
     # -- library handle ---------------------------------------------------------------------------
+    _lib_create, _lib_load, _lib_destroy = lib.dsx_hifigan_create, lib.dsx_hifigan_load, lib.dsx_hifigan_destroy
+
     def _config(self):
         h = self.h
         cfg = _capi.HifiganConfig()
@@ -135,48 +132,11 @@ class HifiGanGenerator(nn.Module):
         cfg.use_pitch_embed = 1 if h['use_pitch_embed'] else 0
         return cfg
 
-    def close(self):
-        if self._dsx is not None:
-            lib.dsx_hifigan_destroy(self._dsx[0])
-            self._dsx, self._wkey, self._keep = None, None, None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _ensure(self, device):
-        if self.c_out != 1:
-            raise DsxError(f"the dsx vocoder writes one waveform channel (c_out = {self.c_out})")
-        if self._dsx is not None and self._dsx[1] != device:
-            self.close()
-        if self._dsx is None:
-            hnd = ctypes.c_void_p()
-            check(lib.dsx_hifigan_create(device.index if device.index is not None else torch.cuda.current_device(),
-                                         ctypes.byref(self._config()), ctypes.byref(hnd)), "dsx_hifigan_create")
-            self._dsx = (hnd, device)
-        hnd = self._dsx[0]
-        sd = self.state_dict()
-        key = tuple((k, v.data_ptr(), v._version, tuple(v.shape)) for k, v in sd.items())
-        if key == self._wkey:
-            return hnd
-        keep = []
-
-        def t(name):
-            x = sd[name].detach().to(device=device, dtype=torch.float32).contiguous()
-            keep.append(x)
-            return x.data_ptr()
-
+    def _params(self, sd, t, arr):
         def conv(name):      # (w, g): weight_v / weight_g of a weight-normalised conv, or (weight, NULL)
             if name + ".weight_g" in sd:
                 return t(name + ".weight_v"), t(name + ".weight_g")
             return t(name + ".weight"), None
-
-        def arr(vals):
-            a = (ctypes.c_void_p * len(vals))(*vals)
-            keep.append(a)
-            return ctypes.cast(a, ctypes.POINTER(ctypes.c_void_p))
 
         nu, nk = self.num_upsamples, self.num_kernels
         per_block = ["convs1.0", "convs1.1", "convs1.2", "convs2.0", "convs2.1", "convs2.2"] \
@@ -188,17 +148,14 @@ class HifiGanGenerator(nn.Module):
         post_w, post_g = conv("conv_post")
         p = _capi.HifiganParams(
             conv_pre_w=pre_w, conv_pre_g=pre_g, conv_pre_b=t("conv_pre.bias"),
-            ups_w=arr([w for w, _ in ups]), ups_g=arr([g for _, g in ups]), ups_b=arr([t(f"ups.{i}.bias") for i in range(nu)]),
-            rb_w=arr([w for w, _ in rb]), rb_g=arr([g for _, g in rb]), rb_b=arr([t(n + ".bias") for n in rb_names]),
+            ups_w=arr([w for w, _ in ups]), ups_g=arr([g for _, g in ups]), ups_b=arr([f"ups.{i}.bias" for i in range(nu)]),
+            rb_w=arr([w for w, _ in rb]), rb_g=arr([g for _, g in rb]), rb_b=arr([n + ".bias" for n in rb_names]),
             conv_post_w=post_w, conv_post_g=post_g, conv_post_b=t("conv_post.bias"))
         if self.h['use_pitch_embed']:
-            p.noise_w = arr([t(f"noise_convs.{i}.weight") for i in range(nu)])
-            p.noise_b = arr([t(f"noise_convs.{i}.bias") for i in range(nu)])
+            p.noise_w = arr([f"noise_convs.{i}.weight" for i in range(nu)])
+            p.noise_b = arr([f"noise_convs.{i}.bias" for i in range(nu)])
             p.source_w, p.source_b = t("m_source.l_linear.weight"), t("m_source.l_linear.bias")
-        with torch.cuda.device(device):
-            check(lib.dsx_hifigan_load(hnd, ctypes.byref(p), _stream(device)), "dsx_hifigan_load")
-        self._wkey, self._keep = key, keep
-        return hnd
+        return p
 
     def forward(self, x, f0=None, *, lengths=None, phase0=None, src_noise=None, seed=0):
         """x: mel [B, 80, T] (any strides); f0: [B, T] Hz or None; lengths: [B] frames or None; phase0 [B, 9] and
@@ -207,6 +164,8 @@ class HifiGanGenerator(nn.Module):
             raise DsxError(f"mel must be [B, 80, T] (got {tuple(x.shape)}); pass dsx_infer's [B, T, 80] output as "
                            ".transpose(1, 2)")
         _need_cuda(x, f0, lengths, phase0, src_noise)
+        if self.c_out != 1:
+            raise DsxError(f"the dsx vocoder writes one waveform channel (c_out = {self.c_out})")
         dev = x.device
         hnd = self._ensure(dev)
         B, _, T = x.shape
