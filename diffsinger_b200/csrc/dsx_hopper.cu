@@ -16,11 +16,15 @@
 // global memory (frames-major [B][Tp][256], Tp = T rounded up to 128); the dilated taps read y at frame offsets -d, 0, +d
 // and the loads zero-fill frames outside [0, T), which is the conv's zero padding applied after the FiLM add.
 //
-// Operands reach shared memory by cp.async in the 128-byte-swizzled K-major layout wgmma reads (dsx_ptx.cuh), double
-// buffered: one stage = a 256-row x 64-k weight tile (32 KB, shared by the warpgroups) + one 64 x 64 activation block per
-// warpgroup.  Each warpgroup's rows go through the same instruction sequence whatever NWG is, so 64- and 128-frame CTAs
-// give bit-identical results.  While GEMM1 runs, the warpgroup prefetches the CP, x and skip rows its epilogues read
-// into L2, and the epilogues issue their global loads in batches ahead of their stores.
+// Operands reach shared memory in the 128-byte-swizzled K-major layout wgmma reads (dsx_ptx.cuh) through a ring of R
+// stages: one stage = a 256-row x 64-k weight tile (32 KB, shared by the warpgroups), packed already swizzled and moved
+// by one bulk copy, + one 64 x 64 activation block per warpgroup, copied by cp.async (the taps shift frames and
+// zero-fill).  Each slot has a full barrier (the bulk copy's bytes and every thread's cp.async) and an empty barrier (one
+// arrival per warpgroup when its MMAs of the slot are done).  The ring runs on across GEMM phases: before an epilogue
+// starts, the first R stages of the next phase are issued, so the weight stream does not stop while the epilogues run.
+// Each warpgroup's rows go through the same instruction sequence whatever NWG is, so 64- and 128-frame CTAs give
+// bit-identical results.  While GEMM1 runs, the warpgroup prefetches the CP, x and skip rows its epilogues read into L2,
+// and the epilogues issue their global loads in batches ahead of their stores.
 //
 // Precision (MMA passes P per k-block): P = 1 fp16 operands; P = 2 adds a W_lo pass (weights as hi+lo fp16 pairs);
 // P = 3 accumulates A_hi*W_hi + A_hi*W_lo + A_lo*W_hi (~2^-22 relative).  The conditioner projection is always 3-pass.
@@ -46,17 +50,29 @@ constexpr int kRowsPerLayer = 80 * 256;    // wpack rows (of 64 fp16) per layer:
 constexpr int kSrRowsPerLayer = 32 * 256;  // rows per layer of one stochastically rounded weight set: 24 W1 + 8 W2 tiles
 constexpr int kWBytes = 256 * 128;         // one weight tile: 256 rows x 64 fp16
 constexpr int kABytes = 64 * 128;          // one activation block: 64 rows x 64 fp16
-constexpr int kZBytes = 2 * 4 * kABytes;   // per warpgroup: z / h / x_in operand, [plane hi, lo][4 k-blocks]
+constexpr int kZBytes = 4 * kABytes;       // one plane (4 k-blocks) of a warpgroup's z / h / x_in operand
 constexpr int kEpiBatch = 8;               // accumulator pairs whose global loads a layer epilogue issues at once
 
-template <int NWG>
+// Shared memory of k_hp_step<NWG, R> from a 1024-aligned base (the dynamic allocation adds 1 KB for the alignment):
+//   R ring slots of STAGE bytes | full[R], empty[R] mbarriers (1 KB, keeps z aligned) | z hi plane, NWG x 32 KB | LO
+// R = 3 (P <= 2: fp16, fp16x2, fp16s): the residual layers never read z's lo plane; only the head does (HP = 3), and
+// during the head's H2 and input-projection GEMMs the ring carries weights only.  So lo k-block kb < 3 of warpgroup wg
+// lives in wg's activation block of slot kb, and LO holds k-block 3, NWG x 8 KB.
+// R = 2 (fp16x3, P = 3 inside the layers): LO is the whole lo plane, NWG x 32 KB.
+template <int NWG, int R>
 struct StepCfg {
+  static_assert(R == 2 || R == 3, "ring depth");
   static constexpr int THREADS = NWG * 128;
   static constexpr int STAGE = kWBytes + NWG * kABytes;
-  static constexpr int SMEM = 1024 + 2 * STAGE + NWG * kZBytes;
-  static_assert(SMEM <= 232448, "shared memory budget");
+  static constexpr int BARS = R * STAGE;
+  static constexpr int ZHI = BARS + 1024;
+  static constexpr int ZLO = ZHI + NWG * kZBytes;
+  static constexpr int SMEM = 1024 + ZLO + NWG * (R == 2 ? kZBytes : kABytes);
+  // NWG = 2: 1 + 3 x 48 + 1 + 64 + 16 KB (R = 3) or 1 + 2 x 48 + 1 + 128 KB (R = 2) = 226 KB, of 227 KB
+  static_assert(SMEM <= 232448, "shared memory budget (227 KB per block on sm_90)");
 };
-constexpr int kCondSmem = 1024 + 2 * StepCfg<2>::STAGE;
+// the conditioner projection: the ring and its barriers only
+constexpr int kCondSmem = 1024 + StepCfg<2, 3>::BARS + 2 * 3 * 8;
 
 struct HpParams {
   const __half* w;           // residual-layer weights: wpack (hi / lo planes) or one stochastically rounded set
@@ -114,7 +130,8 @@ __device__ __forceinline__ int head_slot(const HpParams& p, int k) { return 1 + 
 // ------------------------------------------------------------------------------------------
 // operand loads and the GEMM loop
 // ------------------------------------------------------------------------------------------
-// 256 (NROWS) weight rows -> swizzled tile; row r comes from src0 (r < 128) or src1 (r >= 128, may be src0 + 128 rows)
+// 256 (NROWS) weight rows of an unswizzled tile -> swizzled tile; row r comes from src0 (r < 128) or src1 (r >= 128).
+// Only the self-test uses it, to check the layout against a host product; the kernels bulk-copy pre-swizzled tiles.
 template <int NT>
 __device__ __forceinline__ void load_w(uint8_t* dst, const __half* src0, const __half* src1, int nrows, int tid) {
   const uint32_t d = smem_u32(dst);
@@ -147,53 +164,78 @@ struct NoPrefetch {
   __device__ __forceinline__ void operator()(int) const {}
 };
 
-// c0 (weight rows 0..127) [and c1 (rows 128..255) when NH == 2] = sum over nst stages of A_s . W_s^T.  load(s, buf) issues
-// the cp.async copies of stage s into buf; adesc(s, buf) is the descriptor of this warpgroup's A block of stage s;
-// pre(s) runs at stage s after the copies of stage s + 1 are issued (L2 prefetches of what the epilogues read, paced so
-// that they queue behind the operand copies).  Every thread of the CTA runs it (the weight tile is shared); it ends with
-// the accumulators complete and the stage buffers free.
-template <int NH, class Load, class ADesc, class Pre = NoPrefetch>
-__device__ __forceinline__ void gemm(float (&c0)[64], float (&c1)[64], int nst, Load load, ADesc adesc, uint8_t* buf0,
-                                     uint8_t* buf1, Pre pre = Pre()) {
-  load(0, buf0);
-  cp_commit();
-  fence_acc(c0);
-  if (NH == 2) fence_acc(c1);
-#pragma unroll 1
-  for (int s = 0; s < nst; ++s) {
-    uint8_t* cur = (s & 1) ? buf1 : buf0;
-    if (s + 1 < nst) {
-      load(s + 1, (s & 1) ? buf0 : buf1);
-      cp_commit();
-      pre(s);
-      cp_wait<1>();
-    } else {
-      pre(s);
-      cp_wait<0>();
-    }
-    fence_proxy_async_smem();
-    __syncthreads();
-    const uint64_t a = adesc(s, cur);
-    const uint64_t w = wg_desc(smem_u32(cur));
-    wg_fence();
-#pragma unroll
-    for (int k4 = 0; k4 < 4; ++k4) {
-      const int acc = (s > 0 || k4 > 0) ? 1 : 0;
-      wgmma_n128(c0, a + 2 * k4, w + 2 * k4, acc);
-      if (NH == 2) wgmma_n128(c1, a + 2 * k4, w + (16384 >> 4) + 2 * k4, acc);
-    }
-    wg_commit();
-    wg_wait0();
-    fence_acc(c0);
-    if (NH == 2) fence_acc(c1);
-    __syncthreads();
-  }
+__device__ __forceinline__ uint8_t* smem_base() {
+  extern __shared__ uint8_t smem_raw[];
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 }
 
-// byte offset of (row r, channel k) in a [4 k-blocks] K-major swizzled operand
-__device__ __forceinline__ uint32_t opnd_off(int r, int k) {
-  return static_cast<uint32_t>((k >> 6) * kABytes) + sw128(r, (k & 63) >> 3) + (k & 7) * 2;
+// The shared memory of one CTA, laid out as StepCfg says (the conditioner projection has no z): the operand ring, its
+// barriers, and this warpgroup's z operand.  Addresses are recomputed from the base where they are used, so only n
+// stays live: the stages consumed so far in the launch.  Every thread runs the same GEMM phases, so n is the same in
+// all of them; ring stage i uses slot i % R in barrier phase i / R.
+template <int NWG, int R>
+struct Smem {
+  using Cfg = StepCfg<NWG, R>;
+  uint32_t n;
+  __device__ __forceinline__ uint8_t* slot(uint32_t i) const { return smem_base() + (i % R) * Cfg::STAGE; }
+  __device__ __forceinline__ uint32_t full(uint32_t i) const { return smem_u32(smem_base() + Cfg::BARS) + (i % R) * 8; }
+  __device__ __forceinline__ uint32_t empty(uint32_t i) const { return full(i) + R * 8; }
+  __device__ __forceinline__ uint32_t parity(uint32_t i) const { return (i / R) & 1; }
+  // this warpgroup's activation block in slot j
+  __device__ __forceinline__ uint8_t* ablk(int j) const {
+    return smem_base() + j * Cfg::STAGE + kWBytes + (threadIdx.x >> 7) * kABytes;
+  }
+  // k-block kb of z plane 0 (hi) or 1 (lo).  With R = 3 the lo plane may only be used while no activation block is in
+  // flight in the ring (the head's H2 and input projection, StepCfg).
+  __device__ __forceinline__ uint8_t* zblk(int plane, int kb) const {
+    const int wg = threadIdx.x >> 7;
+    if (plane == 0) return smem_base() + Cfg::ZHI + wg * kZBytes + kb * kABytes;
+    if (R == 2) return smem_base() + Cfg::ZLO + wg * kZBytes + kb * kABytes;
+    return kb < R ? ablk(kb) : smem_base() + Cfg::ZLO + wg * kABytes;
+  }
+  // (row r, channel k) of z plane `plane`
+  __device__ __forceinline__ uint8_t* zat(int plane, int r, int k) const {
+    return zblk(plane, k >> 6) + sw128(r, (k & 63) >> 3) + (k & 7) * 2;
+  }
+  __device__ __forceinline__ void init() {
+    n = 0;
+    if (threadIdx.x == 0) {
+      for (int j = 0; j < R; ++j) {
+        mbar_init(full(j), 1 + NWG * 128);     // the bulk copy's arrive.expect_tx + every thread's cp.async arrival
+        mbar_init(empty(j), NWG);              // one release per warpgroup
+      }
+      fence_mbar_init();
+    }
+    __syncthreads();
+  }
+};
+
+// A GEMM phase of one tile; the stages of a phase are its k-blocks times MMA passes
+enum PhaseKind { PH_NONE, PH_G1, PH_G2, PH_H1, PH_H2, PH_IN, PH_COND };
+struct Phase {
+  int kind, l, u, hq;   // layer, tile, GEMM1 chunk / GEMM2 half / conditioner-projection chunk
+};
+// the first GEMM phase of the head of tile u (none past the last tile)
+__device__ __forceinline__ Phase head_phase(const HpParams& p, int u) {
+  const int kind = u >= p.units ? PH_NONE : (p.head_flags & TC_HEAD) ? PH_H1 : (p.head_flags & TC_INPROJ) ? PH_IN : PH_NONE;
+  return Phase{kind, 0, u, 0};
 }
+// what this CTA runs after layer l: the next layer or the head, from its first tile
+__device__ __forceinline__ Phase after_layer(const HpParams& p, int l) {
+  const int u0 = blockIdx.x;
+  if (l + 1 < p.l1) return Phase{PH_G1, l + 1, u0, 0};
+  return p.head_flags ? head_phase(p, u0) : Phase{PH_NONE, 0, 0, 0};
+}
+
+// The operands of one stage for this thread's warpgroup
+struct StageSrc {
+  const __half* w0;   // packed weight tile, or its rows 0..127 when w1 is set
+  const __half* w1;   // rows 128..255 from a second 128-row tile, or nullptr
+  uint32_t wbytes;    // bytes of each weight copy
+  const __half* a;    // plane whose 64 x 64 block is copied into the slot; nullptr: the A operand is z
+  int b, at, ach;     // that block: utterance, first frame (may lie outside [0, T)), first channel
+  int zplane, zkb;    // otherwise the plane and k-block of z
+};
 
 __device__ __forceinline__ const __half* w1_tile(const HpParams& p, int l, int plane, int h, int kb) {
   if (p.w_sr) return p.w + (static_cast<size_t>(l) * kSrRowsPerLayer + (h * 12 + kb) * 256) * 64;
@@ -210,33 +252,153 @@ __device__ __forceinline__ const __half* whead_tile(const HpParams& p, int idx) 
 __device__ __forceinline__ int pass_wplane(int ps) { return ps == 1 ? 1 : 0; }
 __device__ __forceinline__ int pass_aplane(int ps) { return ps == 2 ? 1 : 0; }
 
+__device__ __forceinline__ int phase_passes(const HpParams& p, int kind) {
+  return kind == PH_COND ? 3 : (kind >= PH_H1 ? p.HP : p.P);
+}
+__device__ __forceinline__ int phase_stages(const HpParams& p, const Phase& ph) {
+  // k-blocks: GEMM1 3 taps x 256 channels, input projection 128 mel bins, the others 256 channels
+  const int kbs = ph.kind == PH_G1 ? 12 : ph.kind == PH_IN ? 2 : ph.kind == PH_NONE ? 0 : 4;
+  return kbs * phase_passes(p, ph.kind);
+}
+
+template <int NWG>
+__device__ __forceinline__ StageSrc stage_src(const HpParams& p, const Phase& ph, int s) {
+  const int frame0 = ph.u * 64 * NWG;
+  const int P = phase_passes(p, ph.kind);
+  const int kb = s / P, ps = s % P, wp = pass_wplane(ps), ap = pass_aplane(ps);
+  StageSrc st;
+  st.w1 = nullptr;
+  st.wbytes = kWBytes;
+  st.a = nullptr;
+  st.b = frame0 / p.Tp;
+  st.at = frame0 % p.Tp + (threadIdx.x >> 7) * 64;
+  st.ach = kb * 64;
+  st.zplane = ap;
+  st.zkb = kb;
+  switch (ph.kind) {
+    case PH_G1:   // [y(t-d) | y(t) | y(t+d)]: k-block kb = tap * 4 + channel block
+      st.w0 = w1_tile(p, ph.l, wp, ph.hq, kb);
+      st.a = p.Y + static_cast<size_t>(ph.l & 1) * 2 * p.plane + ap * p.plane;
+      st.at += ((kb >> 2) - 1) * (1 << (ph.l % p.cycle));
+      st.ach = (kb & 3) * 64;
+      break;
+    case PH_G2:
+      st.w0 = w2_tile(p, ph.l, wp, ph.hq, kb);
+      break;
+    case PH_H1:
+      st.w0 = whead_tile(p, wp * 8 + kb);
+      st.w1 = whead_tile(p, wp * 8 + 4 + kb);
+      st.wbytes = kWBytes / 2;
+      st.a = p.S16 + ap * p.plane;
+      break;
+    case PH_H2:   // N = 128: one 128-row tile
+      st.w0 = whead_tile(p, 16 + wp * 4 + kb);
+      st.wbytes = kWBytes / 2;
+      break;
+    case PH_IN:
+      st.w0 = whead_tile(p, 24 + wp * 4 + kb);
+      st.w1 = whead_tile(p, 24 + wp * 4 + 2 + kb);
+      st.wbytes = kWBytes / 2;
+      break;
+    default:      // PH_COND: the conditioner k-blocks 12..15 of W1 chunk hq
+      st.w0 = p.w + (static_cast<size_t>(ph.l) * kRowsPerLayer + ((wp * 2 + ph.hq) * 16 + 12 + kb) * 256) * 64;
+      st.a = p.CONDH + ap * p.plane;
+      break;
+  }
+  return st;
+}
+
+enum { kIssueW = 1, kIssueA = 2 };
+// Issues the parts of ring stage i: the weight tile (thread 0, once the slot's previous stage is released by every
+// warpgroup) and this warpgroup's activation block (every thread; its own MMAs of the slot's previous stage are done).
+// Every thread arrives on the full barrier with its A part, block or not, so the stage completes only when both parts
+// have landed.
+template <int NWG, int R>
+__device__ __forceinline__ void issue(const HpParams& p, const Smem<NWG, R>& sm, const StageSrc& st, uint32_t i, int parts) {
+  const uint32_t full = sm.full(i);
+  uint8_t* slot = sm.slot(i);
+  if ((parts & kIssueW) && threadIdx.x == 0) {
+    mbar_wait(sm.empty(i), sm.parity(i) ^ 1);
+    mbar_arrive_expect_tx(full, st.w1 ? 2 * st.wbytes : st.wbytes);
+    bulk_g2s(smem_u32(slot), st.w0, st.wbytes, full);
+    if (st.w1) bulk_g2s(smem_u32(slot) + st.wbytes, st.w1, st.wbytes, full);
+  }
+  if (parts & kIssueA) {
+    if (st.a) load_a(slot + kWBytes + (threadIdx.x >> 7) * kABytes, st.a, st.b, st.at, st.ach, p.T, p.Tp, threadIdx.x & 127);
+    cp_arrive_noinc(full);
+  }
+}
+
+// Issues parts of the first R stages of phase ph, the next one the ring will run (all its slots are released).
+template <int NWG, int R>
+__device__ __forceinline__ void fill(const HpParams& p, const Smem<NWG, R>& sm, const Phase& ph, int parts) {
+  const int n = min(R, phase_stages(p, ph));
+#pragma unroll 1
+  for (int j = 0; j < n; ++j) issue(p, sm, stage_src<NWG>(p, ph, j), sm.n + j, parts);
+}
+
+// c0 (weight rows 0..127) [and c1 (rows 128..255) when NH == 2] = sum over the stages s of phase ph of A_s . W_s^T.  The
+// first R stages were issued by fill(); stage s + R - 1 is issued once the MMAs of stage s - 1 are done, which keeps one
+// wgmma group in flight behind the copies.  pre(s) runs after that (L2 prefetches of what the epilogues read, paced so
+// that they queue behind the operand copies).  Every thread of the CTA runs it; it ends with the accumulators complete
+// and every slot released by this warpgroup.
+template <int NH, int NWG, int R, class Pre = NoPrefetch>
+__device__ __forceinline__ void gemm(float (&c0)[64], float (&c1)[64], Smem<NWG, R>& sm, const HpParams& p, const Phase& ph,
+                                     Pre pre = Pre()) {
+  const int nst = phase_stages(p, ph);
+  const int wg = threadIdx.x >> 7;
+  // the epilogue before this phase wrote z with st.shared: visible to the warpgroup's wgmmas from here
+  fence_proxy_async_smem();
+  wg_bar_sync();
+  fence_acc(c0);
+  if (NH == 2) fence_acc(c1);
+#pragma unroll 1
+  for (int s = 0; s < nst; ++s) {
+    const uint32_t i = sm.n + s;
+    const StageSrc st = stage_src<NWG>(p, ph, s);
+    mbar_wait(sm.full(i), sm.parity(i));
+    fence_proxy_async_smem();   // the cp.async writes of the activation block -> the async proxy of wgmma
+    uint8_t* slot = sm.slot(i);
+    const uint64_t a = wg_desc(smem_u32(st.a ? slot + kWBytes + wg * kABytes : sm.zblk(st.zplane, st.zkb)));
+    const uint64_t w = wg_desc(smem_u32(slot));
+    wg_fence();
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4) {
+      const int acc = (s > 0 || k4 > 0) ? 1 : 0;
+      wgmma_n128(c0, a + 2 * k4, w + 2 * k4, acc);
+      if (NH == 2) wgmma_n128(c1, a + 2 * k4, w + (16384 >> 4) + 2 * k4, acc);
+    }
+    wg_commit();
+    if (s > 0) {
+      wg_wait1();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(sm.empty(i - 1));
+      if (s - 1 + R < nst) issue(p, sm, stage_src<NWG>(p, ph, s - 1 + R), i - 1 + R, kIssueW | kIssueA);
+    }
+    pre(s);
+  }
+  wg_wait0();
+  fence_acc(c0);
+  if (NH == 2) fence_acc(c1);
+  if ((threadIdx.x & 127) == 0) mbar_arrive(sm.empty(sm.n + nst - 1));
+  sm.n += nst;
+}
+
 // ------------------------------------------------------------------------------------------
 // one residual layer of one tile
 // ------------------------------------------------------------------------------------------
-template <int NWG>
-__device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, uint8_t* buf0, uint8_t* buf1, uint8_t* zb) {
-  constexpr int NT = NWG * 128;
+template <int NWG, int R>
+__device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem<NWG, R>& sm) {
   const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
   const int frame0 = u * 64 * NWG;
   const int b = frame0 / p.Tp, t0 = frame0 % p.Tp + wg * 64;
   const size_t fbase = static_cast<size_t>(b) * p.Tp + t0;     // global frame of row 0 of this warpgroup
-  const int d = 1 << (l % p.cycle);
   const int P = p.P;
-  const __half* Yin = p.Y + static_cast<size_t>(l & 1) * 2 * p.plane;
   const size_t NF = p.plane / kC;
   float c0[64], c1[64];
 
   // ---- GEMM1 + gate, chunk by chunk ----
 #pragma unroll 1
   for (int h = 0; h < 2; ++h) {
-    auto load = [&](int s, uint8_t* bf) {
-      const int kb = s / P, ps = s % P;
-      const __half* wt = w1_tile(p, l, pass_wplane(ps), h, kb);
-      load_w<NT>(bf, wt, wt + 128 * 64, 256, tid);
-      const int tap = kb >> 2, cb = kb & 3;
-      load_a(bf + kWBytes + wg * kABytes, Yin + pass_aplane(ps) * p.plane, b, t0 + (tap - 1) * d, cb * 64, p.T, p.Tp, wtid);
-    };
-    auto adesc = [&](int, uint8_t* bf) { return wg_desc(smem_u32(bf + kWBytes + wg * kABytes)); };
     // L2 prefetch of this warpgroup's epilogue operands, 16 KB per stage: its CP rows (64 x 2 KB, both chunks) during
     // chunk 0, its X and SKIP rows (64 x 1 KB each) during chunk 1
     auto pre = [&](int s) {
@@ -245,7 +407,9 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, uint
       else if (s < 4) prefetch_l2(p.X + fbase * kC + s * 4096, 16384);
       else if (l > 0) prefetch_l2(p.SKIP + fbase * kC + (s - 4) * 4096, 16384);
     };
-    gemm<2>(c0, c1, 12 * P, load, adesc, buf0, buf1, pre);
+    gemm<2>(c0, c1, sm, p, Phase{PH_G1, l, u, h}, pre);
+    // chunk 1's weights and taps do not depend on this epilogue; GEMM2's weights do not depend on either
+    fill(p, sm, h == 0 ? Phase{PH_G1, l, u, 1} : Phase{PH_G2, l, u, 0}, kIssueW | kIssueA);
     stamp(p, layer_slot(p, l, 2 * h));
     const float* cp = p.CP + (static_cast<size_t>(l) * NF + fbase) * 512 + h * 256;
     // the loads of kEpiBatch accumulator pairs are issued together, ahead of the stores that use them
@@ -270,11 +434,10 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, uint
           z1 = gate_acc(c0[e + 1] + cgv[j].y, c1[e + 1] + cfv[j].y);
         }
         const __half2 hh = __floats2half2_rn(z0, z1);
-        const uint32_t off = opnd_off(r, 128 * h + n);
-        *reinterpret_cast<__half2*>(zb + off) = hh;
-        if (P == 3) {
+        *reinterpret_cast<__half2*>(sm.zat(0, r, 128 * h + n)) = hh;
+        if (R == 2 && P == 3) {
           const float2 hf = __half22float2(hh);
-          *reinterpret_cast<__half2*>(zb + 4 * kABytes + off) = __floats2half2_rn(z0 - hf.x, z1 - hf.y);
+          *reinterpret_cast<__half2*>(sm.zat(1, r, 128 * h + n)) = __floats2half2_rn(z0 - hf.x, z1 - hf.y);
         }
       }
     }
@@ -287,16 +450,10 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, uint
   __half* Yout = p.Y + static_cast<size_t>((l + 1) & 1) * 2 * p.plane;
 #pragma unroll 1
   for (int q = 0; q < 2; ++q) {
-    auto load = [&](int s, uint8_t* bf) {
-      const int kb = s / P, ps = s % P;
-      const __half* wt = w2_tile(p, l, pass_wplane(ps), q, kb);
-      load_w<NT>(bf, wt, wt + 128 * 64, 256, tid);
-    };
-    auto adesc = [&](int s, uint8_t*) {
-      const int kb = s / P, ps = s % P;
-      return wg_desc(smem_u32(zb + (pass_aplane(ps) * 4 + kb) * kABytes));
-    };
-    gemm<2>(c0, c1, 4 * P, load, adesc, buf0, buf1);
+    gemm<2>(c0, c1, sm, p, Phase{PH_G2, l, u, q});
+    if (q == 0) fill(p, sm, Phase{PH_G2, l, u, 1}, kIssueW | kIssueA);
+    else if (u + static_cast<int>(gridDim.x) < p.units) fill(p, sm, Phase{PH_G1, l, u + static_cast<int>(gridDim.x), 0}, kIssueW | kIssueA);
+    else fill(p, sm, after_layer(p, l), kIssueW);   // its activation blocks are issued after the grid barrier
     stamp(p, layer_slot(p, l, 4 + 2 * q));
     // This thread's accumulators cover rows row0 and row0 + 8 and columns colb + 8 i + {0, 1} of each 128-column half
     // (acc_row / acc_col), so every address below is a per-thread base plus a compile-time offset; with the offsets
@@ -368,28 +525,23 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, uint
 // ------------------------------------------------------------------------------------------
 // head of one tile: eps = W_out . relu(W_s . s16 + b_s) + b_out, sampler update, next input projection
 // ------------------------------------------------------------------------------------------
-template <int NWG>
-__device__ __forceinline__ void head_tile(const HpParams& p, int u, uint8_t* buf0, uint8_t* buf1, uint8_t* zb) {
-  constexpr int NT = NWG * 128;
+template <int NWG, int R>
+__device__ __forceinline__ void head_tile(const HpParams& p, int u, Smem<NWG, R>& sm) {
   const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
   const int frame0 = u * 64 * NWG;
   const int b = frame0 / p.Tp, t0 = frame0 % p.Tp + wg * 64;
   const size_t fbase = static_cast<size_t>(b) * p.Tp + t0;
-  const int flags = p.head_flags, HP = p.HP;
+  const int flags = p.head_flags;
   const bool do_head = flags & TC_HEAD, do_in = flags & TC_INPROJ;
   float c0[64], c1[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) c0[i] = 0.f;
 
   if (do_head) {
-    // H1: h = relu(s16 . W_s^T + b_s) -> fp16 hi / lo operand
-    auto load1 = [&](int s, uint8_t* bf) {
-      const int kb = s / HP, ps = s % HP, wp = pass_wplane(ps);
-      load_w<NT>(bf, whead_tile(p, wp * 8 + kb), whead_tile(p, wp * 8 + 4 + kb), 256, tid);
-      load_a(bf + kWBytes + wg * kABytes, p.S16 + pass_aplane(ps) * p.plane, b, t0, kb * 64, p.T, p.Tp, wtid);
-    };
-    auto adesc1 = [&](int, uint8_t* bf) { return wg_desc(smem_u32(bf + kWBytes + wg * kABytes)); };
-    gemm<2>(c0, c1, 4 * HP, load1, adesc1, buf0, buf1);
+    // H1: h = relu(s16 . W_s^T + b_s) -> fp16 hi / lo operand.  H2 carries weights only, so h's lo plane may take the
+    // ring's activation blocks (StepCfg).
+    gemm<2>(c0, c1, sm, p, Phase{PH_H1, 0, u, 0});
+    fill(p, sm, Phase{PH_H2, 0, u, 0}, kIssueW | kIssueA);
     stamp(p, head_slot(p, 0));
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
@@ -399,24 +551,15 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, uint8_t* buf
         const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bs + col));
         const float a0 = fmaxf((hh ? c1[e] : c0[e]) + bb.x, 0.f), a1 = fmaxf((hh ? c1[e + 1] : c0[e + 1]) + bb.y, 0.f);
         const __half2 hv = __floats2half2_rn(a0, a1);
-        const uint32_t off = opnd_off(r, col);
-        *reinterpret_cast<__half2*>(zb + off) = hv;
+        *reinterpret_cast<__half2*>(sm.zat(0, r, col)) = hv;
         const float2 hf = __half22float2(hv);
-        *reinterpret_cast<__half2*>(zb + 4 * kABytes + off) = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
+        *reinterpret_cast<__half2*>(sm.zat(1, r, col)) = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
       }
     }
     stamp(p, head_slot(p, 1));
     // H2: eps (before bias) = h . W_out^T, N = 128 (rows >= M of the packed tile are zero)
-    auto load2 = [&](int s, uint8_t* bf) {
-      const int kb = s / HP, ps = s % HP;
-      const __half* wt = whead_tile(p, 16 + pass_wplane(ps) * 4 + kb);
-      load_w<NT>(bf, wt, wt, 128, tid);
-    };
-    auto adesc2 = [&](int s, uint8_t*) {
-      const int kb = s / HP, ps = s % HP;
-      return wg_desc(smem_u32(zb + (pass_aplane(ps) * 4 + kb) * kABytes));
-    };
-    gemm<1>(c0, c1, 4 * HP, load2, adesc2, buf0, buf1);
+    gemm<1>(c0, c1, sm, p, Phase{PH_H2, 0, u, 0});
+    fill(p, sm, do_in ? Phase{PH_IN, 0, u, 0} : head_phase(p, u + gridDim.x), kIssueW | kIssueA);
     stamp(p, head_slot(p, 2));
   }
 
@@ -475,25 +618,17 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, uint8_t* buf
     if (do_in) {
       // K = 128 operand: bins >= M and frames >= T are zero
       const __half2 hv = __floats2half2_rn(xv[0], xv[1]);
-      const uint32_t off = opnd_off(r, m);
-      *reinterpret_cast<__half2*>(zb + off) = hv;
+      *reinterpret_cast<__half2*>(sm.zat(0, r, m)) = hv;
       const float2 hf = __half22float2(hv);
-      *reinterpret_cast<__half2*>(zb + 4 * kABytes + off) = __floats2half2_rn(xv[0] - hf.x, xv[1] - hf.y);
+      *reinterpret_cast<__half2*>(sm.zat(1, r, m)) = __floats2half2_rn(xv[0] - hf.x, xv[1] - hf.y);
     }
   }
   stamp(p, head_slot(p, 3));
   if (!do_in) return;
 
   // ---- input projection: x0 = relu(x_in . W_in^T + b_in) -> X ; y0 = split(x0 + d_0) -> Y buffer 0 ----
-  auto load3 = [&](int s, uint8_t* bf) {
-    const int kb = s / HP, wp = pass_wplane(s % HP);
-    load_w<NT>(bf, whead_tile(p, 24 + wp * 4 + kb), whead_tile(p, 24 + wp * 4 + 2 + kb), 256, tid);
-  };
-  auto adesc3 = [&](int s, uint8_t*) {
-    const int kb = s / HP, ps = s % HP;
-    return wg_desc(smem_u32(zb + (pass_aplane(ps) * 4 + kb) * kABytes));
-  };
-  gemm<2>(c0, c1, 2 * HP, load3, adesc3, buf0, buf1);
+  gemm<2>(c0, c1, sm, p, Phase{PH_IN, 0, u, 0});
+  fill(p, sm, head_phase(p, u + gridDim.x), kIssueW | kIssueA);
   stamp(p, head_slot(p, 4));
   const float* d0 = p.d0 + static_cast<size_t>(b) * p.d0_row_stride;
 #pragma unroll
@@ -519,32 +654,31 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, uint8_t* buf
   stamp(p, head_slot(p, 5));
 }
 
-template <int NWG>
+template <int NWG, int R>
 __global__ void __launch_bounds__(NWG * 128, 1) k_hp_step(const __grid_constant__ HpParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* buf0 = base;
-  uint8_t* buf1 = base + StepCfg<NWG>::STAGE;
-  uint8_t* zb = base + 2 * StepCfg<NWG>::STAGE + (threadIdx.x >> 7) * kZBytes;
+  Smem<NWG, R> sm;
+  sm.init();
   stamp(p, 0);
+  fill(p, sm, p.l0 < p.l1 ? Phase{PH_G1, p.l0, static_cast<int>(blockIdx.x), 0} : head_phase(p, blockIdx.x),
+       kIssueW | kIssueA);
   for (int l = p.l0; l < p.l1; ++l) {
-    for (int u = blockIdx.x; u < p.units; u += gridDim.x) layer_tile<NWG>(p, l, u, buf0, buf1, zb);
+    for (int u = blockIdx.x; u < p.units; u += gridDim.x) layer_tile<NWG, R>(p, l, u, sm);
     if (l + 1 < p.l1 || p.head_flags) {
+      // every thread gets here with its ring copies issued and none of its barrier waits pending
       cg::this_grid().sync();
       stamp(p, layer_slot(p, l, 8));
+      fill(p, sm, after_layer(p, l), kIssueA);
     }
   }
   if (p.head_flags)
-    for (int u = blockIdx.x; u < p.units; u += gridDim.x) head_tile<NWG>(p, u, buf0, buf1, zb);
+    for (int u = blockIdx.x; u < p.units; u += gridDim.x) head_tile<NWG, R>(p, u, sm);
 }
 
 // CP[l][frame][h * 256 + n] = cond . W1cond^T (hi / lo operands, 3 passes) + dilated_conv.bias + conditioner_projection.bias,
 // for job (tile of 128 frames, layer) = (blockIdx.x, blockIdx.y)
 __global__ void __launch_bounds__(256, 1) k_hp_condproj(const __grid_constant__ HpParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* buf0 = base;
-  uint8_t* buf1 = base + StepCfg<2>::STAGE;
+  Smem<2, 3> sm;   // the ring only: no z operand
+  sm.init();
   const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
   const int u = blockIdx.x, l = blockIdx.y;
   const int frame0 = u * 128;
@@ -552,16 +686,11 @@ __global__ void __launch_bounds__(256, 1) k_hp_condproj(const __grid_constant__ 
   const size_t fbase = static_cast<size_t>(b) * p.Tp + t0;
   const size_t NF = p.plane / kC;
   float c0[64], c1[64];
+  fill(p, sm, Phase{PH_COND, l, u, 0}, kIssueW | kIssueA);
 #pragma unroll 1
   for (int h = 0; h < 2; ++h) {
-    auto load = [&](int s, uint8_t* bf) {
-      const int kb = s / 3, ps = s % 3;
-      const __half* wt = p.w + (static_cast<size_t>(l) * kRowsPerLayer + ((pass_wplane(ps) * 2 + h) * 16 + 12 + kb) * 256) * 64;
-      load_w<256>(bf, wt, wt + 128 * 64, 256, tid);
-      load_a(bf + kWBytes + wg * kABytes, p.CONDH + pass_aplane(ps) * p.plane, b, t0, kb * 64, p.T, p.Tp, wtid);
-    };
-    auto adesc = [&](int, uint8_t* bf) { return wg_desc(smem_u32(bf + kWBytes + wg * kABytes)); };
-    gemm<2>(c0, c1, 12, load, adesc, buf0, buf1);
+    gemm<2>(c0, c1, sm, p, Phase{PH_COND, l, u, h});
+    if (h == 0) fill(p, sm, Phase{PH_COND, l, u, 1}, kIssueW | kIssueA);
     float* cp = p.CP + (static_cast<size_t>(l) * NF + fbase) * 512 + h * 256;
     const float* bias = p.b1p + (static_cast<size_t>(l) * 2 + h) * 256;
 #pragma unroll
@@ -578,7 +707,8 @@ __global__ void __launch_bounds__(256, 1) k_hp_condproj(const __grid_constant__ 
 }
 
 // ------------------------------------------------------------------------------------------
-// weight packing (tiles of 64 fp16 per row, in the order the K loops consume them)
+// weight packing (tiles of 64 fp16 per row, in the order the K loops consume them).  Each row is stored in the
+// 128-byte-swizzled order of its shared-memory slot (sw128_elem), so one bulk copy moves a tile.
 // ------------------------------------------------------------------------------------------
 // whead tile order (128 rows x 64 k each): skip_projection [plane][row half][kb 0..3] (16 tiles),
 // output_projection [plane][kb 0..3] with rows >= M zero (8 tiles), input_projection [plane][row half][kb 0..1]
@@ -587,7 +717,7 @@ __global__ void k_pack_whead(const float* __restrict__ skip_w, const float* __re
                              const float* __restrict__ in_w, __half* __restrict__ whead, int M) {
   const int tileidx = blockIdx.x, n = threadIdx.x;   // 128 threads = rows
   int plane;
-  __half* dst = whead + (static_cast<size_t>(tileidx) * 128 + n) * 64;
+  __half* dst = whead + static_cast<size_t>(tileidx) * 128 * 64;
   for (int kk = 0; kk < 64; ++kk) {
     float v = 0.f;
     if (tileidx < 16) {
@@ -607,7 +737,7 @@ __global__ void k_pack_whead(const float* __restrict__ skip_w, const float* __re
       v = (k < M) ? in_w[static_cast<size_t>(nh * 128 + n) * M + k] : 0.f;
     }
     const __half hi = __float2half_rn(v);
-    dst[kk] = plane == 0 ? hi : __float2half_rn(v - __half2float(hi));
+    dst[sw128_elem(n, kk)] = plane == 0 ? hi : __float2half_rn(v - __half2float(hi));
   }
 }
 
@@ -643,11 +773,11 @@ __global__ void k_pack_wtc(const float* __restrict__ w1f, const float* __restric
     plane = u / 8;
     src = w_src(w1f, w2f, l, false, (u / 4) & 1, u & 3, n);
   }
-  __half* dst = wpack + (static_cast<size_t>(l) * kRowsPerLayer + static_cast<size_t>(tileidx) * 256 + n) * 64;
+  __half* dst = wpack + (static_cast<size_t>(l) * kRowsPerLayer + static_cast<size_t>(tileidx) * 256) * 64;
   for (int kk = 0; kk < 64; ++kk) {
     const float v = src[kk];
     const __half hi = __float2half_rn(v);
-    dst[kk] = plane == 0 ? hi : __float2half_rn(v - __half2float(hi));
+    dst[sw128_elem(n, kk)] = plane == 0 ? hi : __float2half_rn(v - __half2float(hi));
   }
 }
 
@@ -660,8 +790,7 @@ __global__ void k_pack_wsr(const float* __restrict__ w1f, const float* __restric
   const int l = blockIdx.y, tileidx = blockIdx.x, set = blockIdx.z, n = threadIdx.x;
   const float* src = (tileidx < 24) ? w_src(w1f, w2f, l, true, tileidx / 12, tileidx % 12, n)
                                     : w_src(w1f, w2f, l, false, (tileidx - 24) / 4, (tileidx - 24) & 3, n);
-  const size_t row = ((static_cast<size_t>(set) * L + l) * 32 + tileidx) * 256 + n;
-  __half* dst = wsr + row * 64;
+  __half* dst = wsr + ((static_cast<size_t>(set) * L + l) * 32 + tileidx) * 256 * 64;
   const uint2 key = make_uint2(static_cast<uint32_t>(seed) ^ (0x9E3779B9u * static_cast<uint32_t>(set + 1)),
                                static_cast<uint32_t>(seed >> 32) + static_cast<uint32_t>(set));
   for (int k4 = 0; k4 < 16; ++k4) {
@@ -686,7 +815,7 @@ __global__ void k_pack_wsr(const float* __restrict__ w1f, const float* __restric
       // P(take the other neighbour) = |v - fn| / |fo - fn|
       const float pr = (fo != fn) ? fabsf(v - fn) / fabsf(fo - fn) : 0.f;
       const float uu = static_cast<float>(u4[e] >> 8) * (1.0f / 16777216.0f);
-      dst[k4 * 4 + e] = (uu < pr) ? ho : hn;
+      dst[sw128_elem(n, k4 * 4 + e)] = (uu < pr) ? ho : hn;
     }
   }
 }
@@ -731,14 +860,15 @@ int tc_pack_model(dsx_handle* h, cudaStream_t s) {
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-// co-resident CTAs of k_hp_step<NWG> on this device (cached per handle)
-template <int NWG>
+// co-resident CTAs of k_hp_step<NWG, R> on this device (cached per handle)
+template <int NWG, int R>
 static int step_capacity(dsx_handle* h) {
-  int& cache = h->step_occ[NWG - 1];
+  int& cache = h->step_occ[NWG == 1 ? 0 : R == 3 ? 1 : 2];
   if (cache == 0) {
-    cudaFuncSetAttribute(k_hp_step<NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, StepCfg<NWG>::SMEM);
+    using Cfg = StepCfg<NWG, R>;
+    cudaFuncSetAttribute(k_hp_step<NWG, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
     int n = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_hp_step<NWG>, StepCfg<NWG>::THREADS, StepCfg<NWG>::SMEM);
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_hp_step<NWG, R>, Cfg::THREADS, Cfg::SMEM);
     if (e != cudaSuccess) cudaGetLastError();
     cache = (e == cudaSuccess && n >= 1) ? n * h->sm_count : -1;
   }
@@ -790,13 +920,14 @@ static void set_head(dsx_handle* h, HpParams& prm, int flags, float* x, dsx_stri
   prm.d0_row_stride = row_per_b * h->m.L * kC;
 }
 
-static int launch_step(dsx_handle* h, const HpParams& prm, int rows, cudaStream_t s) {
-  const int cap = rows == 64 ? step_capacity<1>(h) : step_capacity<2>(h);
-  DSX_CHECK(cap > 0, DSX_E_CUDA, "k_hp_step<%d> cannot be resident on this device", rows / 64);
+template <int NWG, int R>
+static int launch_step(dsx_handle* h, const HpParams& prm, cudaStream_t s) {
+  const int cap = step_capacity<NWG, R>(h);
+  DSX_CHECK(cap > 0, DSX_E_CUDA, "k_hp_step<%d, %d> cannot be resident on this device", NWG, R);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(static_cast<unsigned>(std::min(prm.units, cap)));
-  cfg.blockDim = dim3(rows == 64 ? StepCfg<1>::THREADS : StepCfg<2>::THREADS);
-  cfg.dynamicSmemBytes = rows == 64 ? StepCfg<1>::SMEM : StepCfg<2>::SMEM;
+  cfg.blockDim = dim3(StepCfg<NWG, R>::THREADS);
+  cfg.dynamicSmemBytes = StepCfg<NWG, R>::SMEM;
   cfg.stream = s;
   // cooperative: the layers of one launch are separated by grid-wide barriers, so every CTA must be resident
   cudaLaunchAttribute attr[1];
@@ -804,10 +935,18 @@ static int launch_step(dsx_handle* h, const HpParams& prm, int rows, cudaStream_
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  if (rows == 64) DSX_CUDA(cudaLaunchKernelEx(&cfg, k_hp_step<1>, prm));
-  else DSX_CUDA(cudaLaunchKernelEx(&cfg, k_hp_step<2>, prm));
+  DSX_CUDA(cudaLaunchKernelEx(&cfg, k_hp_step<NWG, R>, prm));
   h->launches++;
   return DSX_OK;
+}
+
+// Layers that read z's lo plane (P = 3) keep it out of the ring and run a two-stage ring; every other launch runs three.
+static int launch_step(dsx_handle* h, const HpParams& prm, int rows, cudaStream_t s) {
+  if (prm.P == 3) {
+    DSX_CHECK(rows == 128, DSX_E_INVALID, "three-pass layers run in 128-frame tiles");
+    return launch_step<2, 2>(h, prm, s);
+  }
+  return rows == 64 ? launch_step<1, 3>(h, prm, s) : launch_step<2, 3>(h, prm, s);
 }
 
 static int gate_mode(const dsx_handle* h, int P) { return h->gate_approx >= 0 ? h->gate_approx : (P == 3 ? 0 : 1); }
@@ -857,7 +996,7 @@ int launch_tc_head(dsx_handle* h, const Geom& g, int flags, float* x_state, dsx_
 // tile at once, i.e. for small batches that would otherwise leave most SMs idle; 128 otherwise.
 static int stack_rows(dsx_handle* h, const Geom& g) {
   if (h->stack_rows == 64 || h->stack_rows == 128) return h->stack_rows;      // DSX_OPT_STACK_ROWS
-  const int cap64 = step_capacity<1>(h);
+  const int cap64 = step_capacity<1, 3>(h);
   return (cap64 > 0 && g.frames_padded() / 64 <= static_cast<size_t>(cap64)) ? 64 : 128;
 }
 
@@ -899,22 +1038,53 @@ int launch_tc_stack(dsx_handle* h, int nl, const Geom& g, int row0, int row_per_
 // ------------------------------------------------------------------------------------------
 struct SelfParams {
   const __half* a;   // [T][256] fp16, one utterance
-  const __half* w;   // [256 rows][64]
+  const __half* w;   // [256 rows][64], plain (BULK = false) or packed as the kernels' weights (sw128_elem)
   float* out;        // [64][256]
   int t0, T;
 };
 
+// BULK = false: cp.async of the plain tile into the swizzled layout; true: one bulk copy of the packed tile, completing
+// on an mbarrier together with the activation block's cp.async, as in the kernels' ring
+template <bool BULK>
 __global__ void __launch_bounds__(128, 1) k_selftest(const __grid_constant__ SelfParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int wtid = threadIdx.x;
   float c0[64], c1[64];
-  auto load = [&](int s, uint8_t* bf) {
-    load_w<128>(bf, p.w, p.w + 128 * 64, 256, wtid);
-    load_a(bf + kWBytes, p.a, 0, p.t0, s * 64, p.T, p.T, wtid);
-  };
-  auto adesc = [&](int, uint8_t* bf) { return wg_desc(smem_u32(bf + kWBytes)); };
-  gemm<2>(c0, c1, 1, load, adesc, base, base + kWBytes + kABytes);
+  if (BULK) {
+    const uint32_t full = smem_u32(base + kWBytes + kABytes);
+    if (wtid == 0) {
+      mbar_init(full, 1 + 128);
+      fence_mbar_init();
+    }
+    __syncthreads();
+    if (wtid == 0) {
+      mbar_arrive_expect_tx(full, kWBytes);
+      bulk_g2s(smem_u32(base), p.w, kWBytes, full);
+    }
+    load_a(base + kWBytes, p.a, 0, p.t0, 0, p.T, p.T, wtid);
+    cp_arrive_noinc(full);
+    mbar_wait(full, 0);
+    fence_proxy_async_smem();
+  } else {
+    load_w<128>(base, p.w, p.w + 128 * 64, 256, wtid);
+    load_a(base + kWBytes, p.a, 0, p.t0, 0, p.T, p.T, wtid);
+    cp_commit();
+    cp_wait<0>();
+    fence_proxy_async_smem();
+    __syncthreads();
+  }
+  const uint64_t a = wg_desc(smem_u32(base + kWBytes)), w = wg_desc(smem_u32(base));
+  wg_fence();
+#pragma unroll
+  for (int k4 = 0; k4 < 4; ++k4) {
+    wgmma_n128(c0, a + 2 * k4, w + 2 * k4, k4 > 0);
+    wgmma_n128(c1, a + 2 * k4, w + (16384 >> 4) + 2 * k4, k4 > 0);
+  }
+  wg_commit();
+  wg_wait0();
+  fence_acc(c0);
+  fence_acc(c1);
   for (int e = 0; e < 64; ++e) {
     const int r = acc_row(wtid, e), n = acc_col(wtid, e);
     p.out[r * 256 + n] = c0[e];
@@ -926,49 +1096,59 @@ static int run_selftest(std::string& report) {
   const int T = 150;
   auto aval = [](int t, int c) { return static_cast<float>((t * 131 + c * 71) % 61 - 30) / 64.f; };
   auto wval = [](int n, int k) { return static_cast<float>((n * 37 + k * 11) % 53 - 26) / 128.f; };
-  std::vector<__half> ha(static_cast<size_t>(T) * 256), hw(256 * 64);
+  std::vector<__half> ha(static_cast<size_t>(T) * 256), hw(256 * 64), hwp(256 * 64);
   for (int t = 0; t < T; ++t)
     for (int c = 0; c < 256; ++c) ha[static_cast<size_t>(t) * 256 + c] = __float2half(aval(t, c));
   for (int n = 0; n < 256; ++n)
-    for (int k = 0; k < 64; ++k) hw[static_cast<size_t>(n) * 64 + k] = __float2half(wval(n, k));
-  __half *da = nullptr, *dw = nullptr;
+    for (int k = 0; k < 64; ++k) {
+      hw[static_cast<size_t>(n) * 64 + k] = __float2half(wval(n, k));
+      hwp[sw128_elem(n, k)] = __float2half(wval(n, k));
+    }
+  __half *da = nullptr, *dw = nullptr, *dwp = nullptr;
   float* dout = nullptr;
   DSX_CUDA(cudaMalloc(&da, ha.size() * 2));
   DSX_CUDA(cudaMalloc(&dw, hw.size() * 2));
+  DSX_CUDA(cudaMalloc(&dwp, hwp.size() * 2));
   DSX_CUDA(cudaMalloc(&dout, 64 * 256 * 4));
   DSX_CUDA(cudaMemcpy(da, ha.data(), ha.size() * 2, cudaMemcpyHostToDevice));
   DSX_CUDA(cudaMemcpy(dw, hw.data(), hw.size() * 2, cudaMemcpyHostToDevice));
-  const int smem = 1024 + 2 * (kWBytes + kABytes);
-  DSX_CUDA(cudaFuncSetAttribute(k_selftest, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  DSX_CUDA(cudaMemcpy(dwp, hwp.data(), hwp.size() * 2, cudaMemcpyHostToDevice));
+  const int smem = 1024 + kWBytes + kABytes + 8;
+  DSX_CUDA(cudaFuncSetAttribute(k_selftest<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  DSX_CUDA(cudaFuncSetAttribute(k_selftest<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   int failures = 0;
   const int starts[] = {0, -8, 37, 120};     // interior, leading zero fill, unaligned, trailing zero fill
-  for (int t0 : starts) {
-    SelfParams prm{da, dw, dout, t0, T};
-    DSX_CUDA(cudaMemset(dout, 0xff, 64 * 256 * 4));
-    k_selftest<<<1, 128, smem>>>(prm);
-    DSX_CUDA(cudaGetLastError());
-    DSX_CUDA(cudaDeviceSynchronize());
-    std::vector<float> out(64 * 256);
-    DSX_CUDA(cudaMemcpy(out.data(), dout, out.size() * 4, cudaMemcpyDeviceToHost));
-    int bad = 0;
-    double maxerr = 0;
-    for (int m = 0; m < 64; ++m)
-      for (int n = 0; n < 256; ++n) {
-        double ref = 0;
-        const int t = t0 + m;
-        if (t >= 0 && t < T)
-          for (int k = 0; k < 64; ++k) ref += static_cast<double>(aval(t, k)) * wval(n, k);
-        const double e = fabs(ref - out[static_cast<size_t>(m) * 256 + n]);
-        if (!(e <= 1e-4)) bad++;
-        if (e > maxerr || e != e) maxerr = e;
-      }
-    char line[160];
-    snprintf(line, sizeof(line), "wgmma_m64n128k16 t0=%d: bad=%d/16384 maxerr=%.3g\n", t0, bad, maxerr);
-    report += line;
-    if (bad) failures++;
-  }
+  for (int bulk = 0; bulk < 2; ++bulk)
+    for (int t0 : starts) {
+      SelfParams prm{da, bulk ? dwp : dw, dout, t0, T};
+      DSX_CUDA(cudaMemset(dout, 0xff, 64 * 256 * 4));
+      if (bulk) k_selftest<true><<<1, 128, smem>>>(prm);
+      else k_selftest<false><<<1, 128, smem>>>(prm);
+      DSX_CUDA(cudaGetLastError());
+      DSX_CUDA(cudaDeviceSynchronize());
+      std::vector<float> out(64 * 256);
+      DSX_CUDA(cudaMemcpy(out.data(), dout, out.size() * 4, cudaMemcpyDeviceToHost));
+      int bad = 0;
+      double maxerr = 0;
+      for (int m = 0; m < 64; ++m)
+        for (int n = 0; n < 256; ++n) {
+          double ref = 0;
+          const int t = t0 + m;
+          if (t >= 0 && t < T)
+            for (int k = 0; k < 64; ++k) ref += static_cast<double>(aval(t, k)) * wval(n, k);
+          const double e = fabs(ref - out[static_cast<size_t>(m) * 256 + n]);
+          if (!(e <= 1e-4)) bad++;
+          if (e > maxerr || e != e) maxerr = e;
+        }
+      char line[160];
+      snprintf(line, sizeof(line), "wgmma_m64n128k16 %s t0=%d: bad=%d/16384 maxerr=%.3g\n",
+               bulk ? "bulk-copied packed tile" : "cp.async tile", t0, bad, maxerr);
+      report += line;
+      if (bad) failures++;
+    }
   cudaFree(da);
   cudaFree(dw);
+  cudaFree(dwp);
   cudaFree(dout);
   return failures ? DSX_E_KERNEL : DSX_OK;
 }

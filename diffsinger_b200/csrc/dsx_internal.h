@@ -160,7 +160,8 @@ struct ModelDev {
   const float* skip_b;
   const float* fin_w;  // [M][C]
   const float* fin_b;
-  // tensor-core packs (fp16, 128-byte rows of 64 k-values; see dsx_hopper.cu for the tile order)
+  // tensor-core packs (fp16, 128-byte rows of 64 k-values, each row in its 128-byte-swizzled order; see dsx_hopper.cu
+  // for the tile order)
   const __half* wpack; // [L][20480 rows][64]
   const float* b1p;    // [L][2 chunks][256]  gate(128) | filter(128) per chunk
   const __half* whead; // [32 tiles][128 rows][64]: skip_projection, output_projection, input_projection packs
@@ -215,7 +216,7 @@ struct dsx_handle {
   void* stage[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // dsx_infer_host device staging
   size_t stage_cap[7] = {0, 0, 0, 0, 0, 0, 0};
   int stack_kernel = 1;                // DSX_OPT_STACK_KERNEL: 1 = layers and head of a step in one launch where it applies
-  int step_occ[2] = {};                // co-resident CTAs of k_hp_step<NWG> [NWG - 1] on the device (0 unknown, -1 none)
+  int step_occ[3] = {};                // co-resident CTAs of k_hp_step<NWG, R> <1, 3> / <2, 3> / <2, 2> on the device (0 unknown, -1 none)
   int fused_head = 1;                  // DSX_OPT_FUSED_HEAD: the head / sampler update / next input projection run inside the stack launch
   int stack_rows = 0;                  // DSX_OPT_STACK_ROWS: 0 = automatic, 64 / 128 forced
   int stack_rows_used = 0;             // rows per CTA of the last stack launch

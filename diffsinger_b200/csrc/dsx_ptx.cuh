@@ -14,6 +14,9 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 // K-major operand tile, 128-byte swizzle: rows of 64 fp16 (128 B), 8-row swizzle atoms 1024 B apart.  The 16-byte chunk c
 // of row r lives at r * 128 + ((c ^ (r & 7)) << 4); tiles start on 1024-byte boundaries.
 __device__ __forceinline__ uint32_t sw128(int r, int c) { return static_cast<uint32_t>(r * 128 + ((c ^ (r & 7)) << 4)); }
+// The same layout in fp16 elements: where (row r, k) of a tile goes when it is packed in global memory already swizzled,
+// so that one bulk copy of the tile into a 1024-aligned shared-memory slot lands it as sw128 places it.
+__host__ __device__ __forceinline__ int sw128_elem(int r, int k) { return r * 64 + ((((k >> 3) ^ r) & 7) << 3) + (k & 7); }
 
 // wgmma shared-memory matrix descriptor (sm_90): start >> 4 in bits [0,14), leading byte offset >> 4 in [16,30) (unused by
 // swizzled K-major layouts, 1 by convention), stride byte offset >> 4 in [32,46) = 1024 B between 8-row atoms, swizzle mode
@@ -26,6 +29,13 @@ __device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr) {
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the most recent wgmma group of this warpgroup complete
+__device__ __forceinline__ void wg_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// barrier over the 128 threads of this thread's warpgroup, of at most two (ids 1 and 2; 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar_sync() {
+  if (threadIdx.x < 128) asm volatile("bar.sync 1, 128;" ::: "memory");
+  else asm volatile("bar.sync 2, 128;" ::: "memory");
+}
 // generic-proxy writes to shared memory (st.shared, cp.async) -> visible to the async proxy that wgmma reads through
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
@@ -101,6 +111,40 @@ __device__ __forceinline__ void cp16(uint32_t dst, const void* src, bool valid) 
 __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// ---- mbarriers and bulk copies ------------------------------------------------------------------
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+// makes mbarrier.init visible to the other threads and to the async proxy (bulk copies); a __syncthreads must follow
+__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// spins until the phase of parity `parity` of the barrier has completed (returns at once for the phase before the current)
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n"
+      "WAIT:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@!p bra WAIT;\n\t}" ::"r"(bar),
+      "r"(parity)
+      : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// one arrival, and `bytes` more transaction bytes that bulk copies must complete before the phase can
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// one arrival (counted in the barrier's init count) once every cp.async this thread issued so far has landed
+__device__ __forceinline__ void cp_arrive_noinc(uint32_t bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
+}
+// bytes (a multiple of 16) global -> shared, completing as transaction bytes on the barrier bar
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
+               "l"(src), "r"(bytes), "r"(bar)
+               : "memory");
+}
 
 // ---- global memory hints ------------------------------------------------------------------------
 // bytes (a multiple of 16) at a 16-byte aligned global address -> L2, asynchronously; nothing waits for it

@@ -238,7 +238,8 @@ int dsx_debug_trace(dsx_handle* h, int enable, int64_t* out_host);
 int dsx_debug_set_layer_limit(dsx_handle* h, int n_layers);
 
 /* Hardware self-test of the encodings the tensor-core kernels rely on: the swizzled cp.async operand loads (row shifts,
- * zero fill outside [0, T)) and the wgmma shared-memory descriptors, on a small GEMM checked against a host product.
+ * zero fill outside [0, T)), the bulk copy of a pre-swizzled packed weight tile completing on an mbarrier, and the wgmma
+ * shared-memory descriptors, on a small GEMM checked against a host product.
  * which = -1 or 0 runs it; returns 0 when it passes, otherwise DSX_E_KERNEL with the report in dsx_last_error().
  * report (may be NULL): host buffer receiving a text report. */
 int dsx_selftest(int device, int which, char* report, int report_bytes);
