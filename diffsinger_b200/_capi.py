@@ -25,8 +25,9 @@ SYMBOLS = (
     "dsx_set_option", "dsx_set_cond", "dsx_plms_update", "dsx_debug_read", "dsx_debug_trace", "dsx_debug_set_layer_limit", "dsx_selftest",
     "dsx_hifigan_create", "dsx_hifigan_destroy", "dsx_hifigan_load", "dsx_hifigan_forward",
     "dsx_pe_create", "dsx_pe_destroy", "dsx_pe_load", "dsx_pe_forward",
+    "dsx_fs2dec_create", "dsx_fs2dec_destroy", "dsx_fs2dec_load", "dsx_fs2dec_forward",
 )
-_VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy")
+_VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy", "dsx_fs2dec_destroy")
 
 
 class DsxError(RuntimeError):
@@ -77,6 +78,17 @@ class PeParams(ctypes.Structure):
                 ("pos_embed_alpha", _fp)]
 
 
+class Fs2DecConfig(ctypes.Structure):
+    _fields_ = [("hidden", ctypes.c_int), ("layers", ctypes.c_int), ("kernel", ctypes.c_int), ("heads", ctypes.c_int),
+                ("padding", ctypes.c_int), ("act", ctypes.c_int)]
+
+
+class Fs2DecParams(ctypes.Structure):
+    _fields_ = [("ln1_w", _fpp), ("ln1_b", _fpp), ("in_proj_w", _fpp), ("out_proj_w", _fpp), ("ln2_w", _fpp),
+                ("ln2_b", _fpp), ("ffn1_w", _fpp), ("ffn1_b", _fpp), ("ffn2_w", _fpp), ("ffn2_b", _fpp), ("ln_w", _fp),
+                ("ln_b", _fp), ("pos_embed_alpha", _fp)]
+
+
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"dsx CUDA library not found at {LIB_PATH}; build it with `python diffsinger_b200/build.py` "
@@ -114,6 +126,11 @@ lib.dsx_pe_destroy.argtypes = [_vp]
 lib.dsx_pe_destroy.restype = None
 lib.dsx_pe_load.argtypes = [_vp, ctypes.POINTER(PeParams), _vp]
 lib.dsx_pe_forward.argtypes = [_vp, _vp, Strides, _i, _i, _vp, _vp, _vp]
+lib.dsx_fs2dec_create.argtypes = [_i, ctypes.POINTER(Fs2DecConfig), ctypes.POINTER(_vp)]
+lib.dsx_fs2dec_destroy.argtypes = [_vp]
+lib.dsx_fs2dec_destroy.restype = None
+lib.dsx_fs2dec_load.argtypes = [_vp, ctypes.POINTER(Fs2DecParams), _vp]
+lib.dsx_fs2dec_forward.argtypes = [_vp, _vp, Strides, _i, _i, _vp, _vp]
 for _n in SYMBOLS:
     if _n not in _VOID:
         getattr(lib, _n).restype = _i

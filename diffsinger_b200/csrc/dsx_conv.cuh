@@ -1,5 +1,6 @@
-// Implicit-GEMM convolution core of the vocoder (dsx_hifigan.cu) and the pitch extractor (dsx_pe.cu): the packed weight
-// layout, its pack kernel and the K loop of one 64-row tile.  The epilogues are the callers' own.
+// Implicit-GEMM convolution core of the vocoder (dsx_hifigan.cu), the pitch extractor (dsx_pe.cu) and the FastSpeech2
+// decoder (dsx_fs2dec.cu): the packed weight layout, its pack kernel and the K loop of one 64-row tile.  The epilogues
+// are the callers' own.
 //
 // Activations are frames-major fp16 [B][L][cin], cin 80 or a multiple of 16.  Row m of the GEMM is an output position; the
 // K axis is (tap j, input channel c), kk = j * cin + c, and tap j reads input row m + tap0 + j * tstep, zero outside the
@@ -18,6 +19,13 @@ namespace dsx {
 namespace {   // every translation unit has its own k_pack_conv
 
 constexpr int kConvRows = 64;   // GEMM rows per CTA
+
+// sum over the 4 threads of an accumulator quad (they hold the same two rows)
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
+}
 
 // one convolution packed for the implicit GEMM
 struct ConvGemm {
@@ -123,7 +131,7 @@ __device__ __forceinline__ void conv_k_loop(const ConvGemm& g, const __half* x, 
 struct PackArgs {
   const float* v;              // Conv1d [cout][cin][k], or ConvTranspose1d [cin][cout][k] in polyphase form
   const float* scale;          // per index of dim 0 (weight norm), or null: unscaled
-  const float* bias;           // [cout]
+  const float* bias;           // [cout], or null: no bias
   int cin, cout, cout_p, k, u, transposed;   // cout_p: columns per ConvTranspose1d phase (column n = r cout_p + o)
 };
 
@@ -155,7 +163,7 @@ __global__ void k_pack_conv(const ConvGemm g, const PackArgs p) {
     g.w[i] = __float2half_rn(val);
     if (i < static_cast<size_t>(g.ntiles) * g.nt) {
       const int nn = static_cast<int>(i), o = nn % p.cout_p;
-      g.b[nn] = (nn < g.n && o < p.cout) ? p.bias[o] : 0.f;
+      g.b[nn] = (nn < g.n && o < p.cout && p.bias) ? p.bias[o] : 0.f;
     }
   }
 }

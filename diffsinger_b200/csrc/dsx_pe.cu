@@ -13,8 +13,8 @@
 //   PE_LN      bias, ReLU, LayerNorm over the row (two-pass, reduced over the accumulator quad) -> fp16
 //   PE_HEAD    PE_LN, then Linear(P, 2) from registers -> pitch_pred, and f0 with the uv and padding rules
 // GroupNorm statistics span a whole utterance, so k_pe_gn merges the tile partials in a fixed order (Chan's formula, no
-// atomics: deterministic) and applies x += relu(gn(y)).  The position embedding's positions are a scan per utterance
-// (k_pe_scan); k_pe_posadd adds alpha * table[pos] with the table evaluated in fp32 on the fly.
+// atomics: deterministic) and applies x += relu(gn(y)).  The position embedding is dsx_posemb.cuh's: a scan per utterance
+// (k_pos_scan), then k_pos_add adds alpha * table[pos] with the table evaluated in fp32 on the fly.
 #include <math.h>
 #include <stdio.h>
 
@@ -22,6 +22,7 @@
 
 #include "dsx_conv.cuh"
 #include "dsx_internal.h"
+#include "dsx_posemb.cuh"
 #include "dsx_ptx.cuh"
 
 namespace dsx {
@@ -65,13 +66,6 @@ struct PeShape {
   static constexpr int WG = NT > 128 ? 2 : 1;      // warpgroups per CTA; each owns NH columns of the same 64 rows
   static constexpr int NH = NT / WG;
 };
-
-// sum over the 4 threads of an accumulator quad (they hold the same two rows)
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  v += __shfl_xor_sync(0xffffffffu, v, 2);
-  return v;
-}
 
 template <int NT>
 __global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvArgs p) {
@@ -279,55 +273,6 @@ __global__ void __launch_bounds__(256) k_pe_gn(const float* y, const float* stat
     x[base + i] = r;
     x16[base + i] = __float2half_rn(r);
   }
-}
-
-// ---- position embedding ------------------------------------------------------------------------
-// pos[b][t] = cumsum(x[b, :, 0] != 0)[t] * (x[b, t, 0] != 0) (utils/__init__.py:145-157, padding_idx 0).  One block per
-// utterance, kScanChunk frames per thread per pass.
-constexpr int kScanThreads = 1024, kScanChunk = 8;
-__global__ void __launch_bounds__(kScanThreads) k_pe_scan(const float* x, int T, int n, int* pos) {
-  __shared__ int sh[kScanThreads];
-  const int b = blockIdx.x, tid = threadIdx.x;
-  const float* xb = x + static_cast<size_t>(b) * T * n;
-  int carry = 0;
-  for (int base = 0; base < T; base += kScanThreads * kScanChunk) {
-    const int t0 = base + tid * kScanChunk, t1 = min(T, t0 + kScanChunk);
-    int local = 0;
-    for (int t = t0; t < t1; ++t) local += xb[static_cast<size_t>(t) * n] != 0.f;
-    sh[tid] = local;
-    __syncthreads();
-    for (int off = 1; off < kScanThreads; off <<= 1) {
-      const int v = tid >= off ? sh[tid - off] : 0;
-      __syncthreads();
-      sh[tid] += v;
-      __syncthreads();
-    }
-    int s = carry + sh[tid] - local;
-    for (int t = t0; t < t1; ++t) {
-      const bool nz = xb[static_cast<size_t>(t) * n] != 0.f;
-      s += nz;
-      pos[static_cast<size_t>(b) * T + t] = nz ? s : 0;
-    }
-    carry += sh[kScanThreads - 1];
-    __syncthreads();
-  }
-}
-
-// out = fp16(x + alpha * table[pos]) (tts_modules.py:228-229).  table[p] = [sin(p f_i), cos(p f_i)], f_i = exp(-i ln(1e4) /
-// (n/2 - 1)), row 0 = 0 (common_layers.py:106-122), evaluated in fp32 with the full-range sinf / cosf.
-__global__ void k_pe_posadd(const float* x, const int* pos, const float* alpha, int total_rows, int n, float neg_emb,
-                            __half* out) {
-  const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
-  if (i >= static_cast<size_t>(total_rows) * n) return;
-  const int c = static_cast<int>(i % n), half = n / 2;
-  const int ps = pos[i / n];
-  float tab = 0.f;
-  if (ps != 0) {
-    const int fi = c < half ? c : c - half;
-    const float arg = static_cast<float>(ps) * expf(static_cast<float>(fi) * neg_emb);
-    tab = c < half ? sinf(arg) : cosf(arg);
-  }
-  out[i] = __float2half_rn(x[i] + alpha[0] * tab);
 }
 
 // BatchNorm1d in eval mode as y = x * scale + shift: scale = w / sqrt(var + eps), shift = b - mean * scale
@@ -586,13 +531,12 @@ int dsx_pe_forward(dsx_pe* h, const float* mel, dsx_strides ms, int B, int T, fl
   }
   // PitchPredictor (tts_modules.py:222-235): + alpha * position embedding, 4 x [conv, ReLU, LayerNorm], the head
   const float* xs = L > 0 ? Y : X;
-  k_pe_scan<<<B, kScanThreads, 0, s>>>(xs, T, H, POS);
-  DSX_TRY(launch_check("k_pe_scan"));
-  const float neg_emb = -static_cast<float>(log(10000.0) / (H / 2 - 1));
+  k_pos_scan<<<B, kScanThreads, 0, s>>>(xs, T, H, POS);
+  DSX_TRY(launch_check("k_pos_scan"));
   const size_t ne = frames * H;
-  k_pe_posadd<<<static_cast<unsigned>((ne + 255) / 256), 256, 0, s>>>(xs, POS, h->alpha, static_cast<int>(frames), H,
-                                                                      neg_emb, A[0]);
-  DSX_TRY(launch_check("k_pe_posadd"));
+  k_pos_add<<<static_cast<unsigned>((ne + 255) / 256), 256, 0, s>>>(xs, POS, h->alpha, static_cast<int>(frames), H,
+                                                                    pos_neg_emb(H), A[0]);
+  DSX_TRY(launch_check("k_pos_add"));
   cur = 0;
   for (int i = 0; i < kPePredLayers; ++i) {
     a = base;

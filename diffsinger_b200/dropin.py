@@ -22,6 +22,14 @@ imported -- by ``diffsinger_b200.HifiGanGenerator``, so ``vocoders/hifigan.py:lo
 replaces ``modules.fastspeech.pe.PitchExtractor`` -- and the name bound from it in ``inference.*`` / ``tasks.*`` /
 ``usr.*`` modules already imported (inference/svs/ds_e2e.py binds it at import) -- by ``diffsinger_b200.PitchExtractor``,
 so the e2e inference's ``self.pe(mel_out)['f0_denorm_pred']`` runs on dsx after a strict ``load_ckpt``.
+
+    dropin.install_fs2_decoder()      # before the model is built
+
+rebinds ``FastspeechDecoder`` in ``modules.fastspeech.fs2`` and ``modules.diffsinger_midi.fs2`` to
+``diffsinger_b200.FastspeechDecoder``.  Their ``FS_DECODERS['fft']`` looks the name up when it is called, so the next
+``FastSpeech2`` / ``FastSpeech2MIDI`` gets the dsx decoder; ``mel_out`` stays the reference's ``nn.Linear``.
+``modules.fastspeech.tts_modules`` keeps the reference's class, so subclasses of it (usr/diff/candidate_decoder.py) are
+untouched.
 """
 import importlib
 import sys
@@ -199,3 +207,30 @@ def _swap_pitch_extractor(old, new):
             continue
         if getattr(mod, "PitchExtractor", None) is old:
             mod.PitchExtractor = new
+
+
+_fs2 = {}
+_FS2_MODULES = ("modules.fastspeech.fs2", "modules.diffsinger_midi.fs2")
+
+
+def install_fs2_decoder():
+    from .fs2dec import FastspeechDecoder
+    for name in _FS2_MODULES:
+        try:
+            mod = importlib.import_module(name)
+        except ModuleNotFoundError as e:
+            if e.name is None or not name.startswith(e.name):      # a missing dependency, not a missing module
+                raise
+            continue
+        cur = mod.FastspeechDecoder
+        _fs2.setdefault(name, cur)
+        mod.FastspeechDecoder = FastspeechDecoder
+    return FastspeechDecoder
+
+
+def uninstall_fs2_decoder():
+    for name, ref in list(_fs2.items()):
+        mod = sys.modules.get(name)
+        if mod is not None:
+            mod.FastspeechDecoder = ref
+        del _fs2[name]

@@ -380,6 +380,61 @@ int dsx_pe_load(dsx_pe* h, const dsx_pe_params* p, void* stream);
  * an utterance with a zero-padded tail is not the same as that utterance alone; utterances of equal T are independent. */
 int dsx_pe_forward(dsx_pe* h, const float* mel, dsx_strides ms, int B, int T, float* pitch_pred, float* f0, void* stream);
 
+/* ---- FastSpeech2 decoder: decoder_inp -> decoder output -------------------------------------------------------------
+ * Replaces: FastspeechDecoder (modules/fastspeech/tts_modules.py:350-357), i.e. FFTBlocks.forward (:282-307) with the
+ * sinusoidal position embedding (modules/commons/common_layers.py:88-143) and L EncSALayers (:542-588: LayerNorm,
+ * bias-free MultiheadAttention with key padding mask, TransformerFFNLayer :486-522), in eval mode, as
+ * FastSpeech2.forward runs it at inference (modules/fastspeech/fs2.py, FS_DECODERS['fft']).  GEMMs and the attention run
+ * on tensor cores with fp16 operands and fp32 accumulation; the residual stream, LayerNorm statistics, the softmax state
+ * and the output are fp32.  A decoder handle is independent of the other handles. */
+typedef struct dsx_fs2dec dsx_fs2dec;
+
+/* The hyper-parameters FastspeechDecoder reads (hidden_size, dec_layers, dec_ffn_kernel_size, num_heads, ffn_padding,
+ * ffn_act). */
+typedef struct {
+  int hidden;            /* H: a multiple of 64 in [64, 256]                                    */
+  int layers;            /* L: 1..64                                                            */
+  int kernel;            /* ffn_1 kernel size k: odd for SAME, any k >= 1 for LEFT (k <= 255)   */
+  int heads;             /* H / heads must be 64 or 128                                         */
+  int padding;           /* ffn_padding: 0 'SAME' (k // 2 each side), 1 'LEFT' (k - 1 on the left) */
+  int act;               /* ffn_act: 0 'gelu' (exact erf form), 1 'relu'                        */
+} dsx_fs2dec_config;
+
+/* Parameters, fp32 device pointers, each tensor contiguous in the reference's state-dict layout.  Per-layer arrays are
+ * HOST arrays of L device pointers, entry i for layers.i.op.*.  embed_positions._float_tensor is not needed. */
+typedef struct {
+  const float* const* ln1_w;         /* layer_norm1.weight [H]                                                      */
+  const float* const* ln1_b;         /* layer_norm1.bias [H]                                                        */
+  const float* const* in_proj_w;     /* self_attn.in_proj_weight [3H, H] (no bias)                                  */
+  const float* const* out_proj_w;    /* self_attn.out_proj.weight [H, H] (no bias)                                  */
+  const float* const* ln2_w;         /* layer_norm2.weight [H]                                                      */
+  const float* const* ln2_b;         /* layer_norm2.bias [H]                                                        */
+  const float* const* ffn1_w;        /* ffn.ffn_1.weight (SAME) or ffn.ffn_1.1.weight (LEFT) [4H, H, k]             */
+  const float* const* ffn1_b;        /* its bias [4H]                                                               */
+  const float* const* ffn2_w;        /* ffn.ffn_2.weight [H, 4H]                                                    */
+  const float* const* ffn2_b;        /* ffn.ffn_2.bias [H]                                                          */
+  const float* ln_w;                 /* layer_norm.weight [H] (the final LayerNorm)                                 */
+  const float* ln_b;                 /* layer_norm.bias [H]                                                         */
+  const float* pos_embed_alpha;      /* pos_embed_alpha [1]                                                         */
+} dsx_fs2dec_params;
+
+/* Replaces: FastspeechDecoder(hidden_size, num_layers, kernel_size, num_heads) (tts_modules.py:351-356).  Validates the
+ * configuration (DSX_E_INVALID, "unsupported ..."). */
+int dsx_fs2dec_create(int device, const dsx_fs2dec_config* cfg, dsx_fs2dec** out);
+void dsx_fs2dec_destroy(dsx_fs2dec* h);
+
+/* Replaces: load_state_dict of the decoder's parameters (fs2.decoder.* of a FastSpeech2 checkpoint,
+ * utils/__init__.py:178-203).  Packs fp16 tensor-core tiles.  Call again after every change of the weights. */
+int dsx_fs2dec_load(dsx_fs2dec* h, const dsx_fs2dec_params* p, void* stream);
+
+/* Replaces: FFTBlocks.forward(x) with padding_mask = attn_mask = None and return_hiddens = False (tts_modules.py:282-307).
+ *   x    logically [B, T, H], any element strides xs (b, c = channel, t);
+ *   out  [B, T, H] contiguous fp32.
+ * A frame is padding when all H channels are exactly 0 (:288).  Nothing crosses utterances: each utterance of a batch,
+ * padded tail included, gives the same bits as that utterance alone.  An utterance whose frames are all padding gives 0
+ * (the reference's softmax over no key gives NaN there).  The workspace grows to the largest B * T seen. */
+int dsx_fs2dec_forward(dsx_fs2dec* h, const float* x, dsx_strides xs, int B, int T, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
