@@ -2,7 +2,7 @@
 
 The compute lives in ``lib/libdsx.so`` (hand-written CUDA behind the C ABI of ``include/dsx.h``);
 this package is the thin host side that mirrors the reference's ``DiffNet`` / ``GaussianDiffusion``
-class surface, ``HifiGanGenerator`` mirrors the reference's HiFi-GAN (NSF) vocoder, ``PitchExtractor`` its mel-to-f0 pitch extractor and ``FastspeechDecoder`` the FastSpeech2 decoder.  Importing it requires the built library -- there is no Python or CPU fallback.
+class surface, ``HifiGanGenerator`` mirrors the reference's HiFi-GAN (NSF) vocoder, ``PitchExtractor`` its mel-to-f0 pitch extractor, ``FastspeechDecoder`` the FastSpeech2 decoder and ``FFT`` the FFT diffusion denoiser.  Importing it requires the built library -- there is no Python or CPU fallback.
 """
 from ._capi import DsxError, LIB_PATH, PRECISIONS  # noqa: F401  (raises ImportError when libdsx.so is missing)
 from .sampler import DsxSampler, selftest  # noqa: F401
@@ -10,6 +10,7 @@ from .modules import DiffNet, GaussianDiffusion, Mish, SinusoidalPosEmb  # noqa:
 from .vocoder import HifiGanGenerator  # noqa: F401
 from .pitch import PitchExtractor  # noqa: F401
 from .fs2dec import FastspeechDecoder  # noqa: F401
+from .fftdiff import FFT  # noqa: F401
 
 __all__ = ["DiffNet", "GaussianDiffusion", "DsxSampler", "DsxError", "HifiGanGenerator", "PitchExtractor", "FastspeechDecoder",
-           "selftest"]
+           "FFT", "selftest"]

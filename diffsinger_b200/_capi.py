@@ -25,7 +25,7 @@ SYMBOLS = (
     "dsx_set_option", "dsx_set_cond", "dsx_plms_update", "dsx_debug_read", "dsx_debug_trace", "dsx_debug_set_layer_limit", "dsx_selftest",
     "dsx_hifigan_create", "dsx_hifigan_destroy", "dsx_hifigan_load", "dsx_hifigan_forward",
     "dsx_pe_create", "dsx_pe_destroy", "dsx_pe_load", "dsx_pe_forward",
-    "dsx_fs2dec_create", "dsx_fs2dec_destroy", "dsx_fs2dec_load", "dsx_fs2dec_forward",
+    "dsx_fs2dec_create", "dsx_fs2dec_destroy", "dsx_fs2dec_load", "dsx_fs2dec_forward", "dsx_load_fft",
 )
 _VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy", "dsx_fs2dec_destroy")
 
@@ -89,6 +89,15 @@ class Fs2DecParams(ctypes.Structure):
                 ("ln_b", _fp), ("pos_embed_alpha", _fp)]
 
 
+class FftConfig(ctypes.Structure):
+    _fields_ = [("dec", Fs2DecConfig), ("residual_channels", ctypes.c_int), ("mel_bins", ctypes.c_int)]
+
+
+class FftParams(ctypes.Structure):
+    _fields_ = [("dec", Fs2DecParams), ("in_w", _fp), ("in_b", _fp), ("mlp0_w", _fp), ("mlp0_b", _fp), ("mlp2_w", _fp),
+                ("mlp2_b", _fp), ("decode_inp_w", _fp), ("decode_inp_b", _fp), ("mel_out_w", _fp), ("mel_out_b", _fp)]
+
+
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"dsx CUDA library not found at {LIB_PATH}; build it with `python diffsinger_b200/build.py` "
@@ -131,6 +140,7 @@ lib.dsx_fs2dec_destroy.argtypes = [_vp]
 lib.dsx_fs2dec_destroy.restype = None
 lib.dsx_fs2dec_load.argtypes = [_vp, ctypes.POINTER(Fs2DecParams), _vp]
 lib.dsx_fs2dec_forward.argtypes = [_vp, _vp, Strides, _i, _i, _vp, _vp]
+lib.dsx_load_fft.argtypes = [_vp, ctypes.POINTER(FftConfig), ctypes.POINTER(FftParams), _vp]
 for _n in SYMBOLS:
     if _n not in _VOID:
         getattr(lib, _n).restype = _i

@@ -65,29 +65,34 @@ int ensure_workspace(dsx_handle* h, const Geom& g, int rows, cudaStream_t s) {
     return DSX_OK;
   };
 #define NEED(field, bytes) DSX_TRY(need(reinterpret_cast<void**>(&w.field), w.cap_##field, (bytes)))
-  NEED(X, nf * m.C * 4);
-  NEED(SKIP, nf * m.C * 4);
-  if (tc) {
-    const void* cond_before[2] = {w.CONDH, w.CP};
-    NEED(Y, nf * m.C * 2 * 4);
-    NEED(CONDH, nf * m.H * 2 * 2);
-    NEED(S16, nf * m.C * 2 * 2);
-    NEED(CP, static_cast<size_t>(m.L) * nf * 2 * m.C * 4);
-    if (cond_before[0] != w.CONDH || cond_before[1] != w.CP) h->cond_ready = false;
-  } else {
-    const void* cond_before = w.CONDF;
-    NEED(G1, nf * 2 * m.C * 4);
-    NEED(Zf, nf * m.C * 4);
-    NEED(CONDF, nf * m.H * 4);
-    if (cond_before != w.CONDF) h->cond_ready = false;
+  if (!h->fft) {   // the FFT denoiser keeps its own per-evaluation buffers (fft_workspace)
+    NEED(X, nf * m.C * 4);
+    NEED(SKIP, nf * m.C * 4);
+    if (tc) {
+      const void* cond_before[2] = {w.CONDH, w.CP};
+      NEED(Y, nf * m.C * 2 * 4);
+      NEED(CONDH, nf * m.H * 2 * 2);
+      NEED(S16, nf * m.C * 2 * 2);
+      NEED(CP, static_cast<size_t>(m.L) * nf * 2 * m.C * 4);
+      if (cond_before[0] != w.CONDH || cond_before[1] != w.CP) h->cond_ready = false;
+    } else {
+      const void* cond_before = w.CONDF;
+      NEED(G1, nf * 2 * m.C * 4);
+      NEED(Zf, nf * m.C * 4);
+      NEED(CONDF, nf * m.H * 4);
+      if (cond_before != w.CONDF) h->cond_ready = false;
+    }
   }
   if (w.rows_cap < rows) {
     const int keep_rows = std::max(rows, w.rows_cap + w.rows_cap / 2);
-    NEED(DTAB, static_cast<size_t>(keep_rows) * m.L * m.C * 4);
-    NEED(EMB, static_cast<size_t>(keep_rows) * m.C * 4);
+    if (!h->fft) {
+      NEED(DTAB, static_cast<size_t>(keep_rows) * m.L * m.C * 4);
+      NEED(EMB, static_cast<size_t>(keep_rows) * m.C * 4);
+    }
     NEED(TVALS, static_cast<size_t>(keep_rows) * 8);
     w.rows_cap = keep_rows;
   }
+  if (h->fft) DSX_TRY(fft_workspace(h, g, w.rows_cap, s));
   const size_t mel = static_cast<size_t>(g.B) * m.M * g.T;
   NEED(EPS, 5 * mel * 4);
   NEED(XTMP, mel * 4);
@@ -147,6 +152,7 @@ static int run_layers(dsx_handle* h, const Geom& g, int row0, int row_per_b, int
 // One DiffNet evaluation: x (any strides) -> eps (contiguous [B,1,M,T]).
 static int run_eval(dsx_handle* h, const float* x, dsx_strides xs, const Geom& g, int row0, int row_per_b, float* eps,
                     cudaStream_t s) {
+  if (h->fft) return fft_eval(h, x, xs, g, row0, row_per_b, eps, s);
   const bool tc = h->precision != DSX_PREC_FP32_SIMT;
   const int nl = (h->layer_limit >= 0) ? std::min(h->layer_limit, h->m.L) : h->m.L;
   const DdpmCoef none{};
@@ -187,12 +193,25 @@ static int prepare(dsx_handle* h, const float* cond, dsx_strides cs, int B, int 
     return DSX_OK;
   }
   h->cond_ready = false;
-  DSX_TRY(launch_pack_cond(h, cond, cs, g, s));
-  if (h->precision != DSX_PREC_FP32_SIMT) DSX_TRY(launch_tc_condproj(h, g, s));
+  if (h->fft) {
+    DSX_TRY(fft_set_cond(h, cond, cs, g, s));
+  } else {
+    DSX_TRY(launch_pack_cond(h, cond, cs, g, s));
+    if (h->precision != DSX_PREC_FP32_SIMT) DSX_TRY(launch_tc_condproj(h, g, s));
+  }
   h->cond_ready = true;
   h->cond_geom = g;
   return DSX_OK;
 }
+
+// step table of the loaded denoiser: rows of t_dev -> DiffNet's FiLM vectors or the FFT's get_decode_inp step part
+static int embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream_t s) {
+  return h->fft ? fft_embed_table(h, t_dev, rows, s) : launch_embed_table(h, t_dev, rows, s);
+}
+
+// the tensor-core DiffNet kernels (fused heads, updates and input projections); the FFT denoiser runs run_eval + the
+// fp32 update kernels
+static bool tc_diffnet(const dsx_handle* h) { return !h->fft && h->precision != DSX_PREC_FP32_SIMT; }
 
 static dsx_strides contiguous_mel(int M, int T) {
   dsx_strides xs;
@@ -209,9 +228,9 @@ static int sample_ddpm_impl(dsx_handle* h, float* x, const Geom& g, int t_start,
   for (int j = 0; j < n_steps; ++j) tv[j] = t_start - 1 - j;
   DSX_CUDA(cudaMemcpyAsync(h->ws.TVALS, tv.data(), n_steps * sizeof(int64_t), cudaMemcpyHostToDevice, s));
   DSX_CUDA(cudaStreamSynchronize(s));   // tv is a stack-owned staging buffer
-  DSX_TRY(launch_embed_table(h, h->ws.TVALS, n_steps, s));
+  DSX_TRY(embed_table(h, h->ws.TVALS, n_steps, s));
   const dsx_strides xs = contiguous_mel(h->m.M, g.T);
-  const bool tc = h->precision != DSX_PREC_FP32_SIMT;
+  const bool tc = tc_diffnet(h);
   if (tc) DSX_TRY(launch_tc_head(h, g, TC_INPROJ, x, xs, nullptr, nullptr, 0, 0, DdpmCoef{}, 0, 0, s));
   for (int j = 0; j < n_steps; ++j) {
     const int t = t_start - 1 - j;
@@ -277,14 +296,14 @@ static int sample_plms_impl(dsx_handle* h, float* x, const Geom& g, int t_start,
   tv[n] = std::max(steps[0] - interval, 0);
   DSX_CUDA(cudaMemcpyAsync(h->ws.TVALS, tv.data(), (n + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
   DSX_CUDA(cudaStreamSynchronize(s));
-  DSX_TRY(launch_embed_table(h, h->ws.TVALS, n + 1, s));
+  DSX_TRY(embed_table(h, h->ws.TVALS, n + 1, s));
   const dsx_strides xs = contiguous_mel(h->m.M, g.T);
   float* E[5];
   for (int i = 0; i < 5; ++i) E[i] = h->ws.EPS + static_cast<size_t>(i) * mel;
   // history ring: hist[0] = most recent eps_t
   float* hist[4] = {nullptr, nullptr, nullptr, nullptr};
   int nh = 0, slot = 0;
-  const bool tc = h->precision != DSX_PREC_FP32_SIMT;
+  const bool tc = tc_diffnet(h);
   const DdpmCoef none{};
   if (tc) {
     // tcgen05 path: per evaluation the residual stack + ONE head kernel that also does the multistep combination, the
@@ -413,6 +432,7 @@ void dsx_destroy(dsx_handle* h) {
   cudaDeviceSynchronize();
   free_model(h);
   free_ws(h->ws);
+  fft_destroy(h->fft);
   for (cudaEvent_t e : h->prof_events) cudaEventDestroy(e);
   for (void* p : h->stage)
     if (p) cudaFree(p);
@@ -434,6 +454,8 @@ int dsx_load_diffnet(dsx_handle* h, const dsx_diffnet_params* p, int M, int C, i
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   free_model(h);
   free_ws(h->ws);
+  fft_destroy(h->fft);
+  h->fft = nullptr;
   h->ws_epoch++;
   h->cond_ready = false;
   memset(&h->m, 0, sizeof(h->m));
@@ -448,6 +470,26 @@ int dsx_load_diffnet(dsx_handle* h, const dsx_diffnet_params* p, int M, int C, i
   DSX_TRY(simt_pack_model(h, p, s));
   if (precision != DSX_PREC_FP32_SIMT) DSX_TRY(tc_pack_model(h, s));
   DSX_CUDA(cudaStreamSynchronize(s));
+  h->loaded = true;
+  return DSX_OK;
+}
+
+int dsx_load_fft(dsx_handle* h, const dsx_fft_config* cfg, const dsx_fft_params* p, void* stream) {
+  DSX_CHECK(h && cfg && p, DSX_E_INVALID, "null handle, config or params");
+  DSX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  FftDenoiser* f = nullptr;
+  DSX_TRY(fft_create(h->device, cfg, p, s, &f));   // validates and packs before the old denoiser is let go
+  free_model(h);
+  free_ws(h->ws);
+  fft_destroy(h->fft);
+  h->fft = f;
+  h->ws_epoch++;
+  h->cond_ready = false;
+  memset(&h->m, 0, sizeof(h->m));
+  h->m.M = cfg->mel_bins;
+  h->m.H = cfg->dec.hidden;
+  h->precision = DSX_PREC_FP16;
   h->loaded = true;
   return DSX_OK;
 }
@@ -468,7 +510,7 @@ int dsx_diffnet_forward(dsx_handle* h, const float* x, dsx_strides xs, const int
   DSX_CHECK(x && t && eps, DSX_E_INVALID, "null tensor pointer");
   Geom g;
   DSX_TRY(prepare(h, cond, cs, B, T, B, g, s));
-  DSX_TRY(launch_embed_table(h, t, B, s));
+  DSX_TRY(embed_table(h, t, B, s));
   DSX_TRY(run_eval(h, x, xs, g, 0, 1, eps, s));
   return check_status(h, s, "dsx_diffnet_forward");
 }
@@ -682,6 +724,7 @@ int dsx_set_option(dsx_handle* h, int what, int64_t value) {
 
 int dsx_debug_read(dsx_handle* h, int which, float* out, int B, int T, void* stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  DSX_CHECK(!(h && h->fft), DSX_E_STATE, "dsx_debug_read taps DiffNet buffers; the loaded denoiser is the FFT");
   DSX_CHECK(h && out && h->ws.X, DSX_E_STATE, "no workspace");
   DSX_CHECK(B == h->ws.g.B && T == h->ws.g.T, DSX_E_INVALID, "geometry mismatch");
   const float* src = which == 0 ? h->ws.X : h->ws.SKIP;
@@ -693,6 +736,7 @@ int dsx_debug_read(dsx_handle* h, int which, float* out, int B, int T, void* str
 
 int dsx_debug_trace(dsx_handle* h, int enable, int64_t* out_host) {
   DSX_CHECK(h, DSX_E_INVALID, "null handle");
+  DSX_CHECK(!h->fft, DSX_E_STATE, "dsx_debug_trace records the DiffNet step kernel; the loaded denoiser is the FFT");
   DSX_CUDA(cudaSetDevice(h->device));
   const size_t bytes = static_cast<size_t>(2) * h->sm_count * DSX_TRACE_SLOTS * sizeof(int64_t);
   if (enable) {
@@ -713,6 +757,7 @@ int dsx_debug_trace(dsx_handle* h, int enable, int64_t* out_host) {
 
 int dsx_debug_set_layer_limit(dsx_handle* h, int n_layers) {
   DSX_CHECK(h, DSX_E_INVALID, "null handle");
+  DSX_CHECK(!h->fft, DSX_E_STATE, "dsx_debug_set_layer_limit applies to DiffNet; the loaded denoiser is the FFT");
   h->layer_limit = n_layers;
   return DSX_OK;
 }

@@ -14,7 +14,8 @@
 //     k_fs2_conv<F2_RES>   F . ffn_2^T + bias + X, * !pad -> X; LN1 of the next layer -> A, or after the last layer
 //                          the final LayerNorm * !pad -> the fp32 output
 // GEMMs use the implicit-GEMM core of dsx_conv.cuh (fp16 operands, fp32 accumulation).  The residual stream, LayerNorm
-// statistics and the softmax state are fp32.
+// statistics and the softmax state are fp32.  Everything after k_fs2_pack is fs2_stack_run, which the FFT diffusion
+// denoiser (dsx_fftdiff.cu) runs on its own buffers.
 //
 // Padded rows: a padding frame is 0 after each mask, but LN2(0) = beta2 is what the FFN conv's taps read from it, as in
 // the reference, so LN2 is written for every row < T; only rows at or past T read as the conv's zero padding.
@@ -57,6 +58,7 @@ struct Fs2ConvArgs {
   const float* ln_b;
   __half* ln16;                // [B][T][n] LayerNorm output, every row < T
   float* out;                  // non-null: LayerNorm * !pad -> out [B][T][n] fp32 instead of ln16
+  int mask16;                  // with ln16: LayerNorm * !pad (the FFT denoiser's get_mel_out operand)
 };
 
 template <int NT>
@@ -178,6 +180,8 @@ __global__ void __launch_bounds__(128 * Fs2Shape<NT>::WG) k_fs2_conv(const Fs2Co
     const size_t idx = (rbase + m) * n + col;
     if (p.out) {
       *reinterpret_cast<float2*>(p.out + idx) = keep[r] ? make_float2(y0, y1) : make_float2(0.f, 0.f);
+    } else if (p.mask16 && !keep[r]) {
+      *reinterpret_cast<__half2*>(p.ln16 + idx) = __floats2half2_rn(0.f, 0.f);
     } else {
       *reinterpret_cast<__half2*>(p.ln16 + idx) = __floats2half2_rn(y0, y1);
     }
@@ -463,6 +467,109 @@ int attn_opt_in() {
 
 }  // namespace
 
+namespace dsx {
+
+// fp32 X, fp16 A (LayerNorm outputs), O (attention), Q, K, F (FFN hidden), V^T, pad flags, positions
+size_t fs2_workspace_bytes(const dsx_fs2dec* h, int B, int T) {
+  const int H = h->cfg.hidden, Tp = (T + kConvRows - 1) / kConvRows * kConvRows;
+  const size_t frames = static_cast<size_t>(B) * T;
+  return align256(frames * H * 4) + 4 * align256(frames * H * 2) + align256(frames * 4 * H * 2) +
+         align256(static_cast<size_t>(B) * Tp * H * 2) + align256(frames) + align256(frames * 4);
+}
+
+Fs2Bufs fs2_carve(const dsx_fs2dec* h, void* base, int B, int T) {
+  const int H = h->cfg.hidden, Tp = (T + kConvRows - 1) / kConvRows * kConvRows;
+  const size_t frames = static_cast<size_t>(B) * T;
+  Bump ws{static_cast<uint8_t*>(base)};
+  Fs2Bufs w;
+  w.X = ws.take<float>(frames * H * 4);
+  w.A = ws.take<__half>(frames * H * 2);
+  w.O = ws.take<__half>(frames * H * 2);
+  w.Q = ws.take<__half>(frames * H * 2);
+  w.K = ws.take<__half>(frames * H * 2);
+  w.F = ws.take<__half>(frames * 4 * H * 2);
+  w.VT = ws.take<__half>(static_cast<size_t>(B) * Tp * H * 2);
+  w.PAD = ws.take<uint8_t>(frames);
+  w.POS = ws.take<int>(frames * 4);
+  return w;
+}
+
+int fs2_layers(const dsx_fs2dec* h) { return h->cfg.layers; }
+
+int fs2_stack_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s) {
+  const dsx_fs2dec_config& c = h->cfg;
+  const int H = c.hidden, L = c.layers, heads = c.heads, D = H / heads;
+  const int mtiles = (T + kConvRows - 1) / kConvRows, Tp = mtiles * kConvRows;
+  const size_t frames = static_cast<size_t>(B) * T;
+  const unsigned row_blocks = static_cast<unsigned>((frames * 32 + 255) / 256);
+  k_pos_scan<<<B, kScanThreads, 0, s>>>(w.X, T, H, w.POS);
+  DSX_TRY(launch_check("k_pos_scan"));
+  k_fs2_embed<<<row_blocks, 256, 0, s>>>(w.X, w.POS, w.PAD, h->alpha, static_cast<int>(frames), H, pos_neg_emb(H),
+                                         h->layers[0].ln1_w, h->layers[0].ln1_b, w.A);
+  DSX_TRY(launch_check("k_fs2_embed"));
+
+  Fs2ConvArgs base{};
+  base.T = T;
+  base.Tp = Tp;
+  base.H = H;
+  base.heads = heads;
+  base.D = D;
+  base.pad = w.PAD;
+  base.xres = w.X;
+  for (int i = 0; i < L; ++i) {
+    const dsx_fs2dec::Layer& l = h->layers[i];
+    // self-attention block (common_layers.py:569-580): x = (x + out_proj(MHA(LN1(x)))) * !pad
+    Fs2ConvArgs a = base;
+    a.x = w.A;
+    a.mode = F2_QKV;
+    a.qscale = static_cast<float>(sqrt(1.0 / D));   // math.sqrt(1 / head_dim) of F.multi_head_attention_forward
+    a.q = w.Q;
+    a.k = w.K;
+    a.vt = w.VT;
+    DSX_TRY(f2_run(l.qkv, a, B, s));
+    const dim3 agrid(mtiles, heads, B);
+    if (D == 64) {
+      k_fs2_attn<64><<<agrid, 128, attn_smem<64>(), s>>>(w.Q, w.K, w.VT, w.PAD, T, Tp, heads, w.O);
+    } else {
+      k_fs2_attn<128><<<agrid, 128, attn_smem<128>(), s>>>(w.Q, w.K, w.VT, w.PAD, T, Tp, heads, w.O);
+    }
+    DSX_TRY(launch_check("k_fs2_attn"));
+    a = base;
+    a.x = w.O;
+    a.mode = F2_RES;
+    a.ln_w = l.ln2_w;
+    a.ln_b = l.ln2_b;
+    a.ln16 = w.A;
+    DSX_TRY(f2_run(l.out, a, B, s));
+    // FFN block (:582-587, TransformerFFNLayer :503-522): x = (x + ffn_2(act(ffn_1(LN2(x)) * k^-0.5))) * !pad
+    a = base;
+    a.x = w.A;
+    a.mode = F2_FFN1;
+    a.ffn_scale = static_cast<float>(pow(static_cast<double>(c.kernel), -0.5));
+    a.relu = c.act;
+    a.o16 = w.F;
+    DSX_TRY(f2_run(l.ffn1, a, B, s));
+    a = base;
+    a.x = w.F;
+    a.mode = F2_RES;
+    if (i + 1 < L) {
+      a.ln_w = h->layers[i + 1].ln1_w;
+      a.ln_b = h->layers[i + 1].ln1_b;
+      a.ln16 = w.A;
+    } else {   // tts_modules.py:300-301: layer_norm(x) * !pad
+      a.ln_w = h->lnf_w;
+      a.ln_b = h->lnf_b;
+      a.out = out;
+      a.ln16 = out16;
+      a.mask16 = out16 != nullptr;
+    }
+    DSX_TRY(f2_run(l.ffn2, a, B, s));
+  }
+  return DSX_OK;
+}
+
+}  // namespace dsx
+
 extern "C" {
 
 int dsx_fs2dec_create(int device, const dsx_fs2dec_config* cfg, dsx_fs2dec** out) {
@@ -529,96 +636,18 @@ int dsx_fs2dec_forward(dsx_fs2dec* h, const float* x, dsx_strides xs, int B, int
   DSX_CHECK(x && out, DSX_E_INVALID, "x and out must not be NULL");
   DSX_CHECK(B > 0 && T > 0, DSX_E_INVALID, "B and T must be positive (got %d, %d)", B, T);
   DSX_CHECK(B <= 65535, DSX_E_INVALID, "B = %d utterances per call is above the 65535 the launch grid holds", B);
-  const dsx_fs2dec_config& c = h->cfg;
-  const int H = c.hidden, L = c.layers, heads = c.heads, D = H / heads;
-  const int mtiles = (T + kConvRows - 1) / kConvRows, Tp = mtiles * kConvRows;
+  const int H = h->cfg.hidden;
+  const int Tp = (T + kConvRows - 1) / kConvRows * kConvRows;
   DSX_CHECK(static_cast<long long>(B) * Tp * 4 * H < (1ll << 31), DSX_E_INVALID, "B * T = %lld frames is too large",
             static_cast<long long>(B) * T);
   DSX_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-
-  // workspace: fp32 X, fp16 A (LayerNorm outputs), O (attention), F (FFN hidden), Q, K, V^T, pad flags, positions
+  DSX_TRY(h->ws.reserve(fs2_workspace_bytes(h, B, T), s));
+  const Fs2Bufs w = fs2_carve(h, h->ws.ptr, B, T);
   const size_t frames = static_cast<size_t>(B) * T;
-  const size_t vt_b = static_cast<size_t>(B) * Tp * H * 2;
-  DSX_TRY(h->ws.reserve(align256(frames * H * 4) + 4 * align256(frames * H * 2) + align256(frames * 4 * H * 2) +
-                            align256(vt_b) + align256(frames) + align256(frames * 4),
-                        s));
-  Bump ws{static_cast<uint8_t*>(h->ws.ptr)};
-  float* X = ws.take<float>(frames * H * 4);
-  __half* A = ws.take<__half>(frames * H * 2);
-  __half* O = ws.take<__half>(frames * H * 2);
-  __half* Q = ws.take<__half>(frames * H * 2);
-  __half* K = ws.take<__half>(frames * H * 2);
-  __half* F = ws.take<__half>(frames * 4 * H * 2);
-  __half* VT = ws.take<__half>(vt_b);
-  uint8_t* PAD = ws.take<uint8_t>(frames);
-  int* POS = ws.take<int>(frames * 4);
-
-  const unsigned row_blocks = static_cast<unsigned>((frames * 32 + 255) / 256);
-  k_fs2_pack<<<row_blocks, 256, 0, s>>>(x, xs, B, T, H, X, PAD);
+  k_fs2_pack<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(x, xs, B, T, H, w.X, w.PAD);
   DSX_TRY(launch_check("k_fs2_pack"));
-  k_pos_scan<<<B, kScanThreads, 0, s>>>(X, T, H, POS);
-  DSX_TRY(launch_check("k_pos_scan"));
-  k_fs2_embed<<<row_blocks, 256, 0, s>>>(X, POS, PAD, h->alpha, static_cast<int>(frames), H, pos_neg_emb(H),
-                                         h->layers[0].ln1_w, h->layers[0].ln1_b, A);
-  DSX_TRY(launch_check("k_fs2_embed"));
-
-  Fs2ConvArgs base{};
-  base.T = T;
-  base.Tp = Tp;
-  base.H = H;
-  base.heads = heads;
-  base.D = D;
-  base.pad = PAD;
-  base.xres = X;
-  for (int i = 0; i < L; ++i) {
-    const dsx_fs2dec::Layer& l = h->layers[i];
-    // self-attention block (common_layers.py:569-580): x = (x + out_proj(MHA(LN1(x)))) * !pad
-    Fs2ConvArgs a = base;
-    a.x = A;
-    a.mode = F2_QKV;
-    a.qscale = static_cast<float>(sqrt(1.0 / D));   // math.sqrt(1 / head_dim) of F.multi_head_attention_forward
-    a.q = Q;
-    a.k = K;
-    a.vt = VT;
-    DSX_TRY(f2_run(l.qkv, a, B, s));
-    const dim3 agrid(mtiles, heads, B);
-    if (D == 64) {
-      k_fs2_attn<64><<<agrid, 128, attn_smem<64>(), s>>>(Q, K, VT, PAD, T, Tp, heads, O);
-    } else {
-      k_fs2_attn<128><<<agrid, 128, attn_smem<128>(), s>>>(Q, K, VT, PAD, T, Tp, heads, O);
-    }
-    DSX_TRY(launch_check("k_fs2_attn"));
-    a = base;
-    a.x = O;
-    a.mode = F2_RES;
-    a.ln_w = l.ln2_w;
-    a.ln_b = l.ln2_b;
-    a.ln16 = A;
-    DSX_TRY(f2_run(l.out, a, B, s));
-    // FFN block (:582-587, TransformerFFNLayer :503-522): x = (x + ffn_2(act(ffn_1(LN2(x)) * k^-0.5))) * !pad
-    a = base;
-    a.x = A;
-    a.mode = F2_FFN1;
-    a.ffn_scale = static_cast<float>(pow(static_cast<double>(c.kernel), -0.5));
-    a.relu = c.act;
-    a.o16 = F;
-    DSX_TRY(f2_run(l.ffn1, a, B, s));
-    a = base;
-    a.x = F;
-    a.mode = F2_RES;
-    if (i + 1 < L) {
-      a.ln_w = h->layers[i + 1].ln1_w;
-      a.ln_b = h->layers[i + 1].ln1_b;
-      a.ln16 = A;
-    } else {   // tts_modules.py:300-301: layer_norm(x) * !pad
-      a.ln_w = h->lnf_w;
-      a.ln_b = h->lnf_b;
-      a.out = out;
-    }
-    DSX_TRY(f2_run(l.ffn2, a, B, s));
-  }
-  return DSX_OK;
+  return fs2_stack_run(h, w, B, T, out, nullptr, s);
 }
 
 }  // extern "C"

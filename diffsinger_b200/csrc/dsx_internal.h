@@ -193,6 +193,8 @@ struct Workspace {
          cap_DTAB = 0, cap_EMB = 0, cap_TVALS = 0, cap_EPS = 0, cap_XTMP = 0, cap_XSTATE = 0;
 };
 
+struct FftDenoiser;   // dsx_fftdiff.cu
+
 }  // namespace dsx
 
 struct dsx_handle {
@@ -233,6 +235,7 @@ struct dsx_handle {
   size_t prof_used = 0;
   int64_t* trace_dev = nullptr;     // dsx_debug_trace: [2 * sm_count][DSX_TRACE_SLOTS] phase stamps of the step kernel
   bool trace_on = false;
+  dsx::FftDenoiser* fft = nullptr;  // dsx_load_fft: the denoiser is the FFT (m holds only M and H), else DiffNet
 };
 
 namespace dsx {
@@ -240,6 +243,8 @@ namespace dsx {
 // ---- dsx_simt.cu -------------------------------------------------------------------------
 int simt_pack_model(dsx_handle* h, const dsx_diffnet_params* p, cudaStream_t s);
 int launch_embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream_t s);
+// emb[row] = mlp(SinusoidalPosEmb(m.C)(t[row])) for `rows` rows (m: C and the mlp weights)
+int launch_embed_mlp(dsx_handle* h, const ModelDev& m, const int64_t* t_dev, int rows, float* emb, cudaStream_t s);
 int launch_pack_cond(dsx_handle* h, const float* cond, dsx_strides cs, const Geom& g, cudaStream_t s);
 int launch_inproj(dsx_handle* h, const float* x, dsx_strides xs, const Geom& g, int row0, int row_per_b,
                   cudaStream_t s);
@@ -298,5 +303,31 @@ int launch_tc_stack(dsx_handle* h, int nl, const Geom& g, int row0, int row_per_
 int dev_alloc(dsx_handle* h, void** p, size_t bytes, bool model_owned);
 int ensure_workspace(dsx_handle* h, const Geom& g, int rows, cudaStream_t s);
 int check_status(dsx_handle* h, cudaStream_t s, const char* what);
+
+// ---- dsx_fs2dec.cu: the FFTBlocks stack of a loaded decoder handle, shared by the FastSpeech2 decoder and the FFT
+// denoiser ----------------------------------------------------------------------------------------------------------
+struct Fs2Bufs {
+  float* X;          // [B][T][H] fp32 residual stream: the stack's input on entry
+  __half *A, *O, *Q, *K, *F, *VT;
+  uint8_t* PAD;      // [B][T] padding flags, set on entry
+  int* POS;
+};
+size_t fs2_workspace_bytes(const dsx_fs2dec* h, int B, int T);
+Fs2Bufs fs2_carve(const dsx_fs2dec* h, void* ws, int B, int T);   // ws: fs2_workspace_bytes(h, B, T) bytes
+// positions over channel 0, X = (X + alpha * table[pos]) * !pad, the L layers, then the final LayerNorm * !pad: to out
+// [B][T][H] fp32, or (out == NULL) to out16 as fp16.  2 + 5 L launches.
+int fs2_stack_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s);
+int fs2_layers(const dsx_fs2dec* h);
+
+// ---- dsx_fftdiff.cu: the FFT denoiser of the sampler handle ---------------------------------------------------------
+int fft_create(int device, const dsx_fft_config* c, const dsx_fft_params* p, cudaStream_t s, FftDenoiser** out);
+void fft_destroy(FftDenoiser* f);
+// per-(B, T) buffers and `rows` step-table rows; a moved cond-part buffer clears h->cond_ready
+int fft_workspace(dsx_handle* h, const Geom& g, int rows, cudaStream_t s);
+int fft_set_cond(dsx_handle* h, const float* cond, dsx_strides cs, const Geom& g, cudaStream_t s);
+int fft_embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream_t s);
+// eps (contiguous [B,1,M,T]) of x (any strides), utterance b at table row row0 + b * row_per_b
+int fft_eval(dsx_handle* h, const float* x, dsx_strides xs, const Geom& g, int row0, int row_per_b, float* eps,
+             cudaStream_t s);
 
 }  // namespace dsx

@@ -156,11 +156,16 @@ __global__ void k_embed_proj(ModelDev m, const float* __restrict__ emb, float* _
   }
 }
 
-int launch_embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream_t s) {
-  const size_t smem = static_cast<size_t>(5) * h->m.C * sizeof(float);
-  k_embed_table<<<rows, 512, smem, s>>>(h->m, t_dev, h->ws.EMB);
+int launch_embed_mlp(dsx_handle* h, const ModelDev& m, const int64_t* t_dev, int rows, float* emb, cudaStream_t s) {
+  const size_t smem = static_cast<size_t>(5) * m.C * sizeof(float);
+  k_embed_table<<<rows, 512, smem, s>>>(m, t_dev, emb);
   h->launches++;
   DSX_CUDA(cudaGetLastError());
+  return DSX_OK;
+}
+
+int launch_embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream_t s) {
+  DSX_TRY(launch_embed_mlp(h, h->m, t_dev, rows, h->ws.EMB, s));
   k_embed_proj<<<(h->m.L * h->m.C + 15) / 16, 512, 0, s>>>(h->m, h->ws.EMB, h->ws.DTAB, rows);
   h->launches++;
   DSX_CUDA(cudaGetLastError());

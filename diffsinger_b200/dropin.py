@@ -9,7 +9,9 @@ replaces, without editing any reference file,
 -- and the names bound from them in ``usr.*`` / ``tasks.*`` / ``inference.*`` modules already imported -- by subclasses
 whose ``forward(infer=True)`` runs the sm_90a sampler, and the ``'wavenet'`` entry of every ``DIFF_DECODERS`` registry by
 ``diffsinger_b200.DiffNet``.  Construction arguments, parameter / buffer names, ``p_losses`` and the returned ``ret`` dict
-are the reference's own, so the task files run unchanged.
+are the reference's own, so the task files run unchanged.  With ``diff_decoder_type: 'fft'`` the reference's own ``FFT``
+(usr/diff/candidate_decoder.py) stays the ``denoise_fn``: ``DsxSampler`` recognises it and runs its evaluations on dsx
+(``dsx_load_fft``), while training (``p_losses``) keeps calling the reference's module, so nothing is rebound for it.
 
     dropin.install_vocoder()
 

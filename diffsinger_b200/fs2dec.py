@@ -35,8 +35,9 @@ class MultiheadAttention(nn.Module):
 class TransformerFFNLayer(nn.Module):
     """common_layers.py:486-501: ffn_1 is a Conv1d ('SAME') or ConstantPad1d + Conv1d ('LEFT'), ffn_2 a Linear."""
 
-    def __init__(self, hidden_size, filter_size, padding='SAME', kernel_size=1):
+    def __init__(self, hidden_size, filter_size, padding='SAME', kernel_size=1, act='gelu'):
         super().__init__()
+        self.kernel_size, self.act = kernel_size, act
         if padding == 'SAME':
             self.ffn_1 = nn.Conv1d(hidden_size, filter_size, kernel_size, padding=kernel_size // 2)
         else:
@@ -50,20 +51,20 @@ class TransformerFFNLayer(nn.Module):
 class EncSALayer(nn.Module):
     """common_layers.py:542-562 with norm='ln' (LayerNorm eps 1e-5)."""
 
-    def __init__(self, c, num_heads, kernel_size, padding):
+    def __init__(self, c, num_heads, kernel_size, padding, act='gelu'):
         super().__init__()
         self.layer_norm1 = nn.LayerNorm(c)
         self.self_attn = MultiheadAttention(c, num_heads)
         self.layer_norm2 = nn.LayerNorm(c)
-        self.ffn = TransformerFFNLayer(c, 4 * c, kernel_size=kernel_size, padding=padding)
+        self.ffn = TransformerFFNLayer(c, 4 * c, kernel_size=kernel_size, padding=padding, act=act)
 
 
 class TransformerEncoderLayer(nn.Module):
     """tts_modules.py:16-31 (the layer is held as ``op``)."""
 
-    def __init__(self, hidden_size, kernel_size, num_heads, padding):
+    def __init__(self, hidden_size, kernel_size, num_heads, padding, act='gelu'):
         super().__init__()
-        self.op = EncSALayer(hidden_size, num_heads, kernel_size, padding)
+        self.op = EncSALayer(hidden_size, num_heads, kernel_size, padding, act)
 
 
 def _fs2dec_config(hidden_size, num_layers, kernel_size, num_heads, padding, act):
@@ -90,6 +91,20 @@ def _fs2dec_config(hidden_size, num_layers, kernel_size, num_heads, padding, act
     return cfg
 
 
+def fs2dec_params(num_layers, padding, t, arr):
+    """Fs2DecParams of the FFTBlocks stack under the reference's state-dict names (t, arr: see PackedModule._ensure)."""
+    ops = [f"layers.{i}.op" for i in range(num_layers)]
+    ffn1 = ".ffn.ffn_1." if padding == 'SAME' else ".ffn.ffn_1.1."
+    return _capi.Fs2DecParams(
+        ln1_w=arr([o + ".layer_norm1.weight" for o in ops]), ln1_b=arr([o + ".layer_norm1.bias" for o in ops]),
+        in_proj_w=arr([o + ".self_attn.in_proj_weight" for o in ops]),
+        out_proj_w=arr([o + ".self_attn.out_proj.weight" for o in ops]),
+        ln2_w=arr([o + ".layer_norm2.weight" for o in ops]), ln2_b=arr([o + ".layer_norm2.bias" for o in ops]),
+        ffn1_w=arr([o + ffn1 + "weight" for o in ops]), ffn1_b=arr([o + ffn1 + "bias" for o in ops]),
+        ffn2_w=arr([o + ".ffn.ffn_2.weight" for o in ops]), ffn2_b=arr([o + ".ffn.ffn_2.bias" for o in ops]),
+        ln_w=t("layer_norm.weight"), ln_b=t("layer_norm.bias"), pos_embed_alpha=t("pos_embed_alpha"))
+
+
 class FastspeechDecoder(PackedModule):
     def __init__(self, hidden_size=None, num_layers=None, kernel_size=None, num_heads=None, *, hparams=None):
         super().__init__()
@@ -106,7 +121,7 @@ class FastspeechDecoder(PackedModule):
         self.padding_idx = 0
         self.pos_embed_alpha = nn.Parameter(torch.Tensor([1]))
         self.embed_positions = SinusoidalPositionalEmbedding(self.hidden_size, self.padding_idx)
-        self.layers = nn.ModuleList([TransformerEncoderLayer(self.hidden_size, self.kernel_size, self.num_heads, padding)
+        self.layers = nn.ModuleList([TransformerEncoderLayer(self.hidden_size, self.kernel_size, self.num_heads, padding, act)
                                      for _ in range(self.num_layers)])
         self.layer_norm = nn.LayerNorm(self.hidden_size)
 
@@ -117,16 +132,7 @@ class FastspeechDecoder(PackedModule):
         return self._cfg
 
     def _params(self, sd, t, arr):
-        ops = [f"layers.{i}.op" for i in range(self.num_layers)]
-        ffn1 = ".ffn.ffn_1." if self.padding == 'SAME' else ".ffn.ffn_1.1."
-        return _capi.Fs2DecParams(
-            ln1_w=arr([o + ".layer_norm1.weight" for o in ops]), ln1_b=arr([o + ".layer_norm1.bias" for o in ops]),
-            in_proj_w=arr([o + ".self_attn.in_proj_weight" for o in ops]),
-            out_proj_w=arr([o + ".self_attn.out_proj.weight" for o in ops]),
-            ln2_w=arr([o + ".layer_norm2.weight" for o in ops]), ln2_b=arr([o + ".layer_norm2.bias" for o in ops]),
-            ffn1_w=arr([o + ffn1 + "weight" for o in ops]), ffn1_b=arr([o + ffn1 + "bias" for o in ops]),
-            ffn2_w=arr([o + ".ffn.ffn_2.weight" for o in ops]), ffn2_b=arr([o + ".ffn.ffn_2.bias" for o in ops]),
-            ln_w=t("layer_norm.weight"), ln_b=t("layer_norm.bias"), pos_embed_alpha=t("pos_embed_alpha"))
+        return fs2dec_params(self.num_layers, self.padding, t, arr)
 
     def forward(self, x, padding_mask=None, attn_mask=None, return_hiddens=False):
         """x: decoder_inp [B, T, hidden_size] (any strides).  A frame whose channels are all 0 is padding.

@@ -97,7 +97,9 @@ def default_precision():
 
 class DsxSampler:
     """One per (denoise_fn module, device).  `net` is any module with the reference DiffNet's parameter
-    names (usr/diff/net.py:91-104): the reference class itself or diffsinger_b200.DiffNet."""
+    names (usr/diff/net.py:91-104): the reference class itself or diffsinger_b200.DiffNet; or an FFT denoiser
+    (usr/diff/candidate_decoder.py:35-100, recognised by get_decode_inp.weight): the reference class or
+    diffsinger_b200.FFT, packed by fftdiff.load_fft (the precision applies to DiffNet only)."""
 
     def __init__(self, net, precision=None, dilation_cycle_length=None):
         self.net = net
@@ -169,6 +171,13 @@ class DsxSampler:
         sd = {k: v for k, v in self.net.state_dict().items()}
         key = (self.precision,) + tuple((k, v.data_ptr(), v._version, tuple(v.shape)) for k, v in sd.items())
         if key == self._wkey:
+            return h
+        if "get_decode_inp.weight" in sd:
+            from .fftdiff import load_fft
+            cfg = load_fft(h, self.net, sd, device)
+            self.M, self.C, self.H, self.L = cfg.mel_bins, cfg.residual_channels, cfg.dec.hidden, cfg.dec.layers
+            self._wkey = key
+            self._cond_key = self._cond_hold = None      # (re)loading frees the workspace
             return h
         L = len(self.net.residual_layers)
         f = lambda name: sd[name].detach().to(device=device, dtype=torch.float32).contiguous()

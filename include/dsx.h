@@ -119,7 +119,8 @@ int dsx_load_diffnet(dsx_handle* h, const dsx_diffnet_params* p, int M, int C, i
  * pointers to fp32[T] -- the module's buffers verbatim, never recomputed from hparams. */
 int dsx_set_schedule(dsx_handle* h, const float* const* bufs, int T);
 
-/* Replaces: DiffNet.forward(spec, diffusion_step, cond) (usr/diff/net.py:107-130).
+/* Replaces: DiffNet.forward(spec, diffusion_step, cond) (usr/diff/net.py:107-130), or FFT.forward after dsx_load_fft:
+ * one evaluation of the loaded denoiser, utterance b at diffusion step t[b].
  * x: [B,1,M,T] addressed through xs (b, c=mel bin, t); t: device int64[B];
  * cond: [B,H,T] through cs; eps out: contiguous [B,1,M,T]. */
 int dsx_diffnet_forward(dsx_handle* h, const float* x, dsx_strides xs, const int64_t* t,
@@ -434,6 +435,45 @@ int dsx_fs2dec_load(dsx_fs2dec* h, const dsx_fs2dec_params* p, void* stream);
  * padded tail included, gives the same bits as that utterance alone.  An utterance whose frames are all padding gives 0
  * (the reference's softmax over no key gives NaN there).  The workspace grows to the largest B * T seen. */
 int dsx_fs2dec_forward(dsx_fs2dec* h, const float* x, dsx_strides xs, int B, int T, float* out, void* stream);
+
+/* ---- FFT denoiser: the sampler handle's second denoiser ---------------------------------------------------------------
+ * Replaces: FFT (usr/diff/candidate_decoder.py:35-100, DIFF_DECODERS['fft'] of usr/diffsinger_task.py:23-27), the
+ * FastSpeech2 decoder stack run as the diffusion denoiser: eps = get_mel_out(FFTBlocks(get_decode_inp(
+ * [input_projection(x_t), cond, mlp(emb(t))]))).  input_projection is folded into get_decode_inp at load time (in double),
+ * so the entry GEMM has K = mel_bins; its operands, and those of the step-independent cond part, are hi+lo fp16 pairs
+ * (fp32-equivalent).  The step part of get_decode_inp is an fp32 table per diffusion step.  The FFTBlocks stack is the
+ * FastSpeech2 decoder's (fp16 operands, fp32 accumulation and residual stream); get_mel_out reads the final LayerNorm as an
+ * fp16 operand and writes eps in fp32. */
+typedef struct {
+  dsx_fs2dec_config dec;   /* hidden_size, dec_layers, dec_ffn_kernel_size, num_heads, ffn_padding, ffn_act     */
+  int residual_channels;   /* dim of input_projection and the step embedding: a multiple of 16 in [16, 1024]  */
+  int mel_bins;            /* audio_num_mel_bins: 80 (get_mel_out is Linear(hidden_size, 80))                  */
+} dsx_fft_config;
+
+/* Parameters, fp32 device pointers in the reference's state-dict layout (dim = residual_channels, H = hidden). */
+typedef struct {
+  dsx_fs2dec_params dec;   /* the FFTBlocks stack: layers.*, layer_norm.*, pos_embed_alpha                     */
+  const float* in_w;       /* input_projection.weight [dim, mel_bins, 1]                                      */
+  const float* in_b;       /* input_projection.bias   [dim]                                                   */
+  const float* mlp0_w;     /* mlp.0.weight [4 dim, dim]                                                       */
+  const float* mlp0_b;     /* mlp.0.bias   [4 dim]                                                            */
+  const float* mlp2_w;     /* mlp.2.weight [dim, 4 dim]                                                       */
+  const float* mlp2_b;     /* mlp.2.bias   [dim]                                                              */
+  const float* decode_inp_w; /* get_decode_inp.weight [H, dim + H + dim]: columns x | cond | step embedding   */
+  const float* decode_inp_b; /* get_decode_inp.bias   [H]                                                     */
+  const float* mel_out_w;  /* get_mel_out.weight [mel_bins, H]                                                */
+  const float* mel_out_b;  /* get_mel_out.bias   [mel_bins]                                                   */
+} dsx_fft_params;
+
+/* Replaces: FFT(hidden_size, dec_layers, dec_ffn_kernel_size, num_heads) + load_state_dict as the denoise_fn of
+ * GaussianDiffusion.  Validates like dsx_fs2dec_create plus residual_channels and mel_bins (DSX_E_INVALID,
+ * "unsupported ..."); on failure the handle keeps what it held.  Replaces the handle's denoiser (DiffNet or FFT), as
+ * dsx_load_diffnet replaces an FFT.  Afterwards dsx_diffnet_forward, dsx_set_cond, dsx_sample_ddpm, dsx_sample_plms,
+ * dsx_plms_update, dsx_infer and dsx_infer_host run the FFT denoiser with unchanged meaning; DSX_INFO_PRECISION reports
+ * DSX_PREC_FP16; the DiffNet-only options (STACK_*, FUSED_HEAD, SR_SETS, GATE_APPROX, PROFILE) are accepted and ignored;
+ * dsx_debug_read, dsx_debug_trace and dsx_debug_set_layer_limit return DSX_E_STATE.  A padding frame (all H channels of
+ * get_decode_inp's output exactly 0) gives eps = get_mel_out.bias. */
+int dsx_load_fft(dsx_handle* h, const dsx_fft_config* cfg, const dsx_fft_params* p, void* stream);
 
 #ifdef __cplusplus
 }
