@@ -26,8 +26,12 @@ SYMBOLS = (
     "dsx_hifigan_create", "dsx_hifigan_destroy", "dsx_hifigan_load", "dsx_hifigan_forward",
     "dsx_pe_create", "dsx_pe_destroy", "dsx_pe_load", "dsx_pe_forward",
     "dsx_fs2dec_create", "dsx_fs2dec_destroy", "dsx_fs2dec_load", "dsx_fs2dec_forward", "dsx_load_fft",
+    "dsx_fs2enc_create", "dsx_fs2enc_destroy", "dsx_fs2enc_load", "dsx_fs2enc_forward",
+    "dsx_durpred_create", "dsx_durpred_destroy", "dsx_durpred_load", "dsx_durpred_forward",
+    "dsx_length_totals", "dsx_length_regulate",
 )
-_VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy", "dsx_fs2dec_destroy")
+_VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy", "dsx_fs2dec_destroy",
+         "dsx_fs2enc_destroy", "dsx_durpred_destroy")
 
 
 class DsxError(RuntimeError):
@@ -98,6 +102,24 @@ class FftParams(ctypes.Structure):
                 ("mlp2_b", _fp), ("decode_inp_w", _fp), ("decode_inp_b", _fp), ("mel_out_w", _fp), ("mel_out_b", _fp)]
 
 
+class Fs2EncConfig(ctypes.Structure):
+    _fields_ = [("stack", Fs2DecConfig), ("vocab", ctypes.c_int), ("pos", ctypes.c_int)]
+
+
+class Fs2EncParams(ctypes.Structure):
+    _fields_ = [("stack", Fs2DecParams), ("embed_w", _fp)]
+
+
+class DurPredConfig(ctypes.Structure):
+    _fields_ = [("idim", ctypes.c_int), ("chans", ctypes.c_int), ("layers", ctypes.c_int), ("kernel", ctypes.c_int),
+                ("padding", ctypes.c_int), ("offset", ctypes.c_float)]
+
+
+class DurPredParams(ctypes.Structure):
+    _fields_ = [("conv_w", _fpp), ("conv_b", _fpp), ("ln_w", _fpp), ("ln_b", _fpp), ("linear_w", _fp),
+                ("linear_b", _fp)]
+
+
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"dsx CUDA library not found at {LIB_PATH}; build it with `python diffsinger_b200/build.py` "
@@ -141,6 +163,18 @@ lib.dsx_fs2dec_destroy.restype = None
 lib.dsx_fs2dec_load.argtypes = [_vp, ctypes.POINTER(Fs2DecParams), _vp]
 lib.dsx_fs2dec_forward.argtypes = [_vp, _vp, Strides, _i, _i, _vp, _vp]
 lib.dsx_load_fft.argtypes = [_vp, ctypes.POINTER(FftConfig), ctypes.POINTER(FftParams), _vp]
+lib.dsx_fs2enc_create.argtypes = [_i, ctypes.POINTER(Fs2EncConfig), ctypes.POINTER(_vp)]
+lib.dsx_fs2enc_destroy.argtypes = [_vp]
+lib.dsx_fs2enc_destroy.restype = None
+lib.dsx_fs2enc_load.argtypes = [_vp, ctypes.POINTER(Fs2EncParams), _vp]
+lib.dsx_fs2enc_forward.argtypes = [_vp, _vp, _i, _i, ctypes.POINTER(_vp), ctypes.POINTER(Strides), _i, _vp, _vp]
+lib.dsx_durpred_create.argtypes = [_i, ctypes.POINTER(DurPredConfig), ctypes.POINTER(_vp)]
+lib.dsx_durpred_destroy.argtypes = [_vp]
+lib.dsx_durpred_destroy.restype = None
+lib.dsx_durpred_load.argtypes = [_vp, ctypes.POINTER(DurPredParams), _vp]
+lib.dsx_durpred_forward.argtypes = [_vp, _vp, Strides, _vp, _i, _i, _vp, _vp, _vp]
+lib.dsx_length_totals.argtypes = [_vp, _vp, _i, _i, ctypes.c_float, _vp, _vp, _vp]
+lib.dsx_length_regulate.argtypes = [_vp, _vp, _i, _i, _i, _vp, _vp]
 for _n in SYMBOLS:
     if _n not in _VOID:
         getattr(lib, _n).restype = _i

@@ -15,7 +15,8 @@
 //                          the final LayerNorm * !pad -> the fp32 output
 // GEMMs use the implicit-GEMM core of dsx_conv.cuh (fp16 operands, fp32 accumulation).  The residual stream, LayerNorm
 // statistics and the softmax state are fp32.  Everything after k_fs2_pack is fs2_stack_run, which the FFT diffusion
-// denoiser (dsx_fftdiff.cu) runs on its own buffers.
+// denoiser (dsx_fftdiff.cu) runs on its own buffers; its layers (fs2_layers_run) are also the FastSpeech2 encoder's
+// (dsx_fs2enc.cu), after an entry of its own.
 //
 // Padded rows: a padding frame is 0 after each mask, but LN2(0) = beta2 is what the FFN conv's taps read from it, as in
 // the reference, so LN2 is written for every row < T; only rows at or past T read as the conv's zero padding.
@@ -359,7 +360,6 @@ __global__ void k_fs2_embed(float* X, const int* pos, const uint8_t* pad, const 
   const bool keep = !pad[warp];
   float* xr = X + static_cast<size_t>(warp) * H;
   float v[8];
-  float sum = 0.f;
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     if (i >= per) break;
@@ -367,28 +367,8 @@ __global__ void k_fs2_embed(float* X, const int* pos, const uint8_t* pad, const 
     const float y = xr[c] + alpha[0] * pos_table(ps, c, H, neg_emb);
     v[i] = keep ? y : 0.f;
     xr[c] = v[i];
-    sum += v[i];
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  const float mean = sum / static_cast<float>(H);
-  float sq = 0.f;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    if (i >= per) break;
-    const float d = v[i] - mean;
-    sq += d * d;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-  const float rstd = 1.f / sqrtf(sq / static_cast<float>(H) + kFs2LnEps);
-  __half* ar = A + static_cast<size_t>(warp) * H;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    if (i >= per) break;
-    const int c = lane + 32 * i;
-    ar[c] = __float2half_rn((v[i] - mean) * rstd * ln_w[c] + ln_b[c]);
-  }
+  warp_row_ln16(v, per, H, kFs2LnEps, ln_w, ln_b, A + static_cast<size_t>(warp) * H);
 }
 
 }  // namespace
@@ -497,9 +477,7 @@ Fs2Bufs fs2_carve(const dsx_fs2dec* h, void* base, int B, int T) {
 int fs2_layers(const dsx_fs2dec* h) { return h->cfg.layers; }
 
 int fs2_stack_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s) {
-  const dsx_fs2dec_config& c = h->cfg;
-  const int H = c.hidden, L = c.layers, heads = c.heads, D = H / heads;
-  const int mtiles = (T + kConvRows - 1) / kConvRows, Tp = mtiles * kConvRows;
+  const int H = h->cfg.hidden;
   const size_t frames = static_cast<size_t>(B) * T;
   const unsigned row_blocks = static_cast<unsigned>((frames * 32 + 255) / 256);
   k_pos_scan<<<B, kScanThreads, 0, s>>>(w.X, T, H, w.POS);
@@ -507,6 +485,18 @@ int fs2_stack_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* ou
   k_fs2_embed<<<row_blocks, 256, 0, s>>>(w.X, w.POS, w.PAD, h->alpha, static_cast<int>(frames), H, pos_neg_emb(H),
                                          h->layers[0].ln1_w, h->layers[0].ln1_b, w.A);
   DSX_TRY(launch_check("k_fs2_embed"));
+  return fs2_layers_run(h, w, B, T, out, out16, s);
+}
+
+void fs2_first_ln(const dsx_fs2dec* h, const float** w, const float** b) {
+  *w = h->layers[0].ln1_w;
+  *b = h->layers[0].ln1_b;
+}
+
+int fs2_layers_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s) {
+  const dsx_fs2dec_config& c = h->cfg;
+  const int H = c.hidden, L = c.layers, heads = c.heads, D = H / heads;
+  const int mtiles = (T + kConvRows - 1) / kConvRows, Tp = mtiles * kConvRows;
 
   Fs2ConvArgs base{};
   base.T = T;
@@ -598,6 +588,17 @@ void dsx_fs2dec_destroy(dsx_fs2dec* h) {
 
 int dsx_fs2dec_load(dsx_fs2dec* h, const dsx_fs2dec_params* p, void* stream) {
   DSX_CHECK(h && p, DSX_E_INVALID, "null handle or params");
+  DSX_CHECK(p->pos_embed_alpha, DSX_E_INVALID, "missing layer_norm or pos_embed_alpha");
+  return fs2_load(h, p, stream);
+}
+
+}  // extern "C"
+
+namespace dsx {
+
+// dsx_fs2dec_load without pos_embed_alpha, which the encoder's stack does not have (h->alpha stays NULL without it)
+int fs2_load(dsx_fs2dec* h, const dsx_fs2dec_params* p, void* stream) {
+  DSX_CHECK(h && p, DSX_E_INVALID, "null handle or params");
   DSX_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const dsx_fs2dec_config& c = h->cfg;
@@ -605,7 +606,7 @@ int dsx_fs2dec_load(dsx_fs2dec* h, const dsx_fs2dec_params* p, void* stream) {
   DSX_CHECK(p->ln1_w && p->ln1_b && p->in_proj_w && p->out_proj_w && p->ln2_w && p->ln2_b && p->ffn1_w && p->ffn1_b &&
                 p->ffn2_w && p->ffn2_b,
             DSX_E_INVALID, "missing per-layer arrays");
-  DSX_CHECK(p->ln_w && p->ln_b && p->pos_embed_alpha, DSX_E_INVALID, "missing layer_norm or pos_embed_alpha");
+  DSX_CHECK(p->ln_w && p->ln_b, DSX_E_INVALID, "missing layer_norm");
   DSX_CUDA(cudaStreamSynchronize(s));   // the old packs may still be read by queued work
   h->mem.free_all();
   h->loaded = false;
@@ -625,10 +626,15 @@ int dsx_fs2dec_load(dsx_fs2dec* h, const dsx_fs2dec_params* p, void* stream) {
   }
   DSX_TRY(f2_copy(h, &h->lnf_w, p->ln_w, H, "layer_norm.weight", L, s));
   DSX_TRY(f2_copy(h, &h->lnf_b, p->ln_b, H, "layer_norm.bias", L, s));
-  DSX_TRY(f2_copy(h, &h->alpha, p->pos_embed_alpha, 1, "pos_embed_alpha", L, s));
+  h->alpha = nullptr;
+  if (p->pos_embed_alpha) DSX_TRY(f2_copy(h, &h->alpha, p->pos_embed_alpha, 1, "pos_embed_alpha", L, s));
   h->loaded = true;
   return DSX_OK;
 }
+
+}  // namespace dsx
+
+extern "C" {
 
 int dsx_fs2dec_forward(dsx_fs2dec* h, const float* x, dsx_strides xs, int B, int T, float* out, void* stream) {
   DSX_CHECK(h, DSX_E_INVALID, "null handle");

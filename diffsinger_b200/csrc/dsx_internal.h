@@ -314,10 +314,16 @@ struct Fs2Bufs {
 };
 size_t fs2_workspace_bytes(const dsx_fs2dec* h, int B, int T);
 Fs2Bufs fs2_carve(const dsx_fs2dec* h, void* ws, int B, int T);   // ws: fs2_workspace_bytes(h, B, T) bytes
-// positions over channel 0, X = (X + alpha * table[pos]) * !pad, the L layers, then the final LayerNorm * !pad: to out
-// [B][T][H] fp32, or (out == NULL) to out16 as fp16.  2 + 5 L launches.
+// the decoder's entry -- positions over channel 0, X = (X + alpha * table[pos]) * !pad and LN1 of layer 0 -> A -- then
+// fs2_layers_run.  2 + 5 L launches.
 int fs2_stack_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s);
+// the L layers from X (masked), PAD and A = LN1 of layer 0 (fp16), then the final LayerNorm * !pad: to out [B][T][H] fp32,
+// or (out == NULL) to out16 as fp16.  5 L launches.
+int fs2_layers_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s);
 int fs2_layers(const dsx_fs2dec* h);
+void fs2_first_ln(const dsx_fs2dec* h, const float** w, const float** b);   // layer 0's layer_norm1 (device)
+// dsx_fs2dec_load with pos_embed_alpha optional (the encoder's FFTBlocks have none)
+int fs2_load(dsx_fs2dec* h, const dsx_fs2dec_params* p, void* stream);
 
 // ---- dsx_fftdiff.cu: the FFT denoiser of the sampler handle ---------------------------------------------------------
 int fft_create(int device, const dsx_fft_config* c, const dsx_fft_params* p, cudaStream_t s, FftDenoiser** out);

@@ -12,6 +12,7 @@
 //   PE_GN      bias -> fp32 pre-norm values, plus per-tile, per-16-channel-group (count, mean, M2) partials
 //   PE_LN      bias, ReLU, LayerNorm over the row (two-pass, reduced over the accumulator quad) -> fp16
 //   PE_HEAD    PE_LN, then Linear(P, 2) from registers -> pitch_pred, and f0 with the uv and padding rules
+//   PE_DUR     PE_LN, then the DurationPredictor's Linear(P, 1) from registers, * !mask -> xs, and out2dur -> int64 dur
 // GroupNorm statistics span a whole utterance, so k_pe_gn merges the tile partials in a fixed order (Chan's formula, no
 // atomics: deterministic) and applies x += relu(gn(y)).  The position embedding is dsx_posemb.cuh's: a scan per utterance
 // (k_pos_scan), then k_pos_add adds alpha * table[pos] with the table evaluated in fp32 on the fly.
@@ -33,7 +34,7 @@ constexpr int kPePrenetLayers = 3, kPePredLayers = 5, kPeEncKernel = 5, kPePrene
 constexpr int kPeMaxConvLayers = 16;
 constexpr float kBnEps = 1e-5f, kGnEps = 1e-5f, kLnEps = 1e-12f;
 
-enum { PE_PRENET = 0, PE_LINEAR = 1, PE_GN = 2, PE_LN = 3, PE_HEAD = 4 };
+enum { PE_PRENET = 0, PE_LINEAR = 1, PE_GN = 2, PE_LN = 3, PE_HEAD = 4, PE_DUR = 5 };
 enum { PE_MASK = 1, PE_OUT32 = 2, PE_OUT16 = 4 };
 
 // one conv or linear: its GEMM (one column tile) and the per-channel affine of its epilogue
@@ -59,6 +60,8 @@ struct PeConvArgs {
   float* f0;                   // [B][T] or null
   int pitch_norm, use_uv;
   float f0_mean, f0_std;
+  int64_t* dur;                // PE_DUR: [B][T] or null (xs goes to o32 [B][T])
+  float offset;
 };
 
 template <int NT>
@@ -106,7 +109,7 @@ __global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvA
   for (int e = 0; e < NH / 2; ++e) {
     const int col = c0 + acc_col(wtid, e);
     float v = col < n ? acc[e] + __ldg(p.g.b + col) : 0.f;
-    if (p.mode == PE_PRENET || p.mode == PE_LN || p.mode == PE_HEAD) v = fmaxf(v, 0.f);
+    if (p.mode == PE_PRENET || p.mode == PE_LN || p.mode == PE_HEAD || p.mode == PE_DUR) v = fmaxf(v, 0.f);
     acc[e] = v;
   }
 
@@ -152,7 +155,7 @@ __global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvA
     }
   }
 
-  if (p.mode == PE_LN || p.mode == PE_HEAD) {
+  if (p.mode == PE_LN || p.mode == PE_HEAD || p.mode == PE_DUR) {
     const float inv_n = 1.f / static_cast<float>(n);
     float s[2] = {0.f, 0.f};
 #pragma unroll
@@ -203,6 +206,29 @@ __global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvA
         if (p.pad[idx]) f = 0.f;
         p.f0[idx] = f;
       }
+    }
+    return;
+  }
+
+  if (p.mode == PE_DUR) {
+    // DurationPredictor (tts_modules.py:113-129): xs = Linear(LN(x) * !mask) * !mask, dur = clamp(round(exp(xs) - offset),
+    // 0) with round half to even.  A padding row is 0 in both.
+    float o[2] = {0.f, 0.f};
+#pragma unroll
+    for (int e = 0; e < NH / 2; ++e) {
+      const int col = c0 + acc_col(wtid, e);
+      if (col < n) o[(e >> 1) & 1] = fmaf(acc[e], __ldg(p.hw + col), o[(e >> 1) & 1]);
+    }
+    row_sum(o[0], o[1]);
+    if (wg != 0 || (wtid & 3) != 0) return;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int m = mrow[r];
+      if (m >= T) continue;
+      const size_t idx = rbase + m;
+      const float x = p.pad[idx] ? 0.f : o[r] + __ldg(p.hb);
+      p.o32[idx] = x;
+      if (p.dur) p.dur[idx] = __float2ll_rz(fmaxf(rintf(expf(x) - p.offset), 0.f));
     }
     return;
   }
@@ -559,6 +585,153 @@ int dsx_pe_forward(dsx_pe* h, const float* mel, dsx_strides ms, int B, int T, fl
       a.f0_std = c.f0_std;
     }
     DSX_TRY(pe_run(h->pred[i], a, B, s));
+    cur ^= 1;
+  }
+  return DSX_OK;
+}
+
+}  // extern "C"
+
+// ---- duration predictor ---------------------------------------------------------------------------------------------
+namespace dsx {
+namespace {
+
+constexpr int kDpMaxLayers = 16;
+
+// x logically [B, T, C] (any strides: b, c = channel, t) -> fp16 [B][T][C].  One warp per frame.
+__global__ void k_dp_pack(const float* x, dsx_strides xs, int B, int T, int C, __half* out) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= B * T) return;
+  const int b = warp / T, t = warp - b * T;
+  const float* src = x + b * xs.b + t * xs.t;
+  for (int c = lane; c < C; c += 32) out[static_cast<size_t>(warp) * C + c] = __float2half_rn(src[c * xs.c]);
+}
+
+}  // namespace
+}  // namespace dsx
+
+struct dsx_durpred {
+  int device = 0;
+  dsx_durpred_config cfg{};
+  bool loaded = false;
+  PePacked conv[dsx::kDpMaxLayers];
+  float* head = nullptr;       // linear.weight [P], bias [1]
+  DevAllocs mem;
+  GrowBuffer ws;
+};
+
+extern "C" {
+
+int dsx_durpred_create(int device, const dsx_durpred_config* c, dsx_durpred** out) {
+  DSX_CHECK(out, DSX_E_INVALID, "out is NULL");
+  *out = nullptr;
+  DSX_CHECK(c, DSX_E_INVALID, "config is NULL");
+  DSX_CHECK(c->idim >= 16 && c->idim <= 256 && c->idim % 16 == 0, DSX_E_INVALID,
+            "unsupported idim %d: a multiple of 16 in [16, 256]", c->idim);
+  DSX_CHECK(c->chans >= 16 && c->chans <= 256 && c->chans % 16 == 0, DSX_E_INVALID,
+            "unsupported n_chans %d: a multiple of 16 in [16, 256]", c->chans);
+  DSX_CHECK(c->layers >= 1 && c->layers <= kDpMaxLayers, DSX_E_INVALID, "unsupported n_layers %d: 1..%d", c->layers,
+            kDpMaxLayers);
+  DSX_CHECK(c->padding == 0 || c->padding == 1, DSX_E_INVALID, "unsupported padding %d: 0 (SAME) or 1 (LEFT)",
+            c->padding);
+  DSX_CHECK(c->kernel >= 1 && c->kernel <= 31 && (c->padding == 1 || c->kernel % 2 == 1), DSX_E_INVALID,
+            "unsupported kernel_size %d: in [1, 31], odd for SAME", c->kernel);
+  DSX_CHECK(isfinite(c->offset), DSX_E_INVALID, "unsupported offset: must be finite");
+  DSX_TRY(select_sm90_device(device, "duration predictor"));
+  DSX_TRY(conv_opt_in<256>([](auto k) { return k_pe_conv<decltype(k)::value>; }));
+  dsx_durpred* h = new dsx_durpred();
+  h->device = device;
+  h->cfg = *c;
+  *out = h;
+  return DSX_OK;
+}
+
+void dsx_durpred_destroy(dsx_durpred* h) {
+  if (!h) return;
+  cudaSetDevice(h->device);
+  cudaDeviceSynchronize();
+  h->mem.free_all();
+  h->ws.release();
+  delete h;
+}
+
+int dsx_durpred_load(dsx_durpred* h, const dsx_durpred_params* p, void* stream) {
+  DSX_CHECK(h && p, DSX_E_INVALID, "null handle or params");
+  DSX_CHECK(p->conv_w && p->conv_b && p->ln_w && p->ln_b && p->linear_w && p->linear_b, DSX_E_INVALID,
+            "missing conv, LayerNorm or linear arrays");
+  DSX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const dsx_durpred_config& c = h->cfg;
+  const int P = c.chans, k = c.kernel;
+  DSX_CUDA(cudaStreamSynchronize(s));   // the old packs may still be read by queued work
+  h->mem.free_all();
+  h->loaded = false;
+  const int tap0 = c.padding ? -(k - 1) : -(k - 1) / 2;   // ConstantPad1d LEFT (k - 1, 0) or SAME
+  char what[64];
+  for (int i = 0; i < c.layers; ++i) {
+    PePacked& pc = h->conv[i];
+    pc = PePacked{};
+    snprintf(what, sizeof what, "conv.%d.1", i);
+    DSX_CHECK(p->conv_w[i] && p->conv_b[i], DSX_E_INVALID, "missing %s", what);
+    pc.cin = i ? P : c.idim;
+    pc.n = P;
+    pc.taps = k;
+    pc.tap0 = tap0;
+    DSX_TRY(conv_pack(h->mem, pc, 256, PackArgs{p->conv_w[i], nullptr, p->conv_b[i], pc.cin, P, P, k, 1, 0}, s));
+    DSX_CHECK(p->ln_w[i] && p->ln_b[i], DSX_E_INVALID, "missing conv.%d.3", i);
+    DSX_TRY(h->mem.alloc(&pc.s, P * sizeof(float)));
+    DSX_TRY(h->mem.alloc(&pc.t, P * sizeof(float)));
+    DSX_CUDA(cudaMemcpyAsync(pc.s, p->ln_w[i], P * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    DSX_CUDA(cudaMemcpyAsync(pc.t, p->ln_b[i], P * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  }
+  DSX_TRY(h->mem.alloc(&h->head, (P + 1) * sizeof(float)));
+  DSX_CUDA(cudaMemcpyAsync(h->head, p->linear_w, P * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  DSX_CUDA(cudaMemcpyAsync(h->head + P, p->linear_b, sizeof(float), cudaMemcpyDeviceToDevice, s));
+  h->loaded = true;
+  return DSX_OK;
+}
+
+int dsx_durpred_forward(dsx_durpred* h, const float* x, dsx_strides xs_, const uint8_t* mask, int B, int T, float* xs,
+                        int64_t* dur, void* stream) {
+  DSX_CHECK(h, DSX_E_INVALID, "null handle");
+  DSX_CHECK(h->loaded, DSX_E_STATE, "dsx_durpred_load has not been called");
+  DSX_CHECK(x && mask && xs, DSX_E_INVALID, "x, mask and xs must not be NULL");
+  DSX_CHECK(B > 0 && T > 0, DSX_E_INVALID, "B and T must be positive (got %d, %d)", B, T);
+  DSX_CHECK(B <= 65535, DSX_E_INVALID, "B = %d utterances per call is above the 65535 the launch grid holds", B);
+  const dsx_durpred_config& c = h->cfg;
+  const int P = c.chans, C = std::max(c.idim, P);
+  DSX_CHECK(static_cast<long long>(B) * T * C < (1ll << 31), DSX_E_INVALID, "B * T = %lld tokens is too large",
+            static_cast<long long>(B) * T);
+  DSX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t frames = static_cast<size_t>(B) * T;
+  DSX_TRY(h->ws.reserve(2 * align256(frames * C * 2), s));
+  Bump ws{static_cast<uint8_t*>(h->ws.ptr)};
+  __half* A[2] = {ws.take<__half>(frames * C * 2), ws.take<__half>(frames * C * 2)};
+  k_dp_pack<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(x, xs_, B, T, c.idim, A[0]);
+  DSX_TRY(launch_check("k_dp_pack"));
+  // DurationPredictor._forward (tts_modules.py:113-129): n_layers x [conv, ReLU, LayerNorm, * !mask], then the head
+  int cur = 0;
+  for (int i = 0; i < c.layers; ++i) {
+    PeConvArgs a{};
+    a.T = T;
+    a.pad = mask;
+    a.x = A[cur];
+    a.scale = h->conv[i].s;
+    a.shift = h->conv[i].t;
+    if (i + 1 < c.layers) {
+      a.mode = PE_LN;
+      a.flags = PE_MASK | PE_OUT16;
+      a.o16 = A[cur ^ 1];
+    } else {
+      a.mode = PE_DUR;
+      a.hw = h->head;
+      a.hb = h->head + P;
+      a.o32 = xs;
+      a.dur = dur;
+      a.offset = c.offset;
+    }
+    DSX_TRY(pe_run(h->conv[i], a, B, s));
     cur ^= 1;
   }
   return DSX_OK;

@@ -32,6 +32,15 @@ rebinds ``FastspeechDecoder`` in ``modules.fastspeech.fs2`` and ``modules.diffsi
 ``FastSpeech2`` / ``FastSpeech2MIDI`` gets the dsx decoder; ``mel_out`` stays the reference's ``nn.Linear``.
 ``modules.fastspeech.tts_modules`` keeps the reference's class, so subclasses of it (usr/diff/candidate_decoder.py) are
 untouched.
+
+    dropin.install_fs2_encoder()      # before the model is built
+
+rebinds ``FastspeechEncoder``, ``FastspeechMIDIEncoder``, ``DurationPredictor`` and ``LengthRegulator`` in
+``modules.fastspeech.fs2`` and ``modules.diffsinger_midi.fs2`` (where the module defines or imports the name) to the
+classes of ``diffsinger_b200.fs2enc``.  ``FS_ENCODERS['fft']`` looks the encoder up when it is called and
+``FastSpeech2.__init__`` the other two, so the next ``FastSpeech2`` / ``FastSpeech2MIDI`` runs its encoder, duration
+predictor and length regulator on dsx; ``FastSpeech2.forward`` itself (the MIDI embeddings, the ``decoder_inp`` gather)
+stays the reference's.  ``modules.fastspeech.tts_modules`` keeps the reference's classes.
 """
 import importlib
 import sys
@@ -236,3 +245,32 @@ def uninstall_fs2_decoder():
         if mod is not None:
             mod.FastspeechDecoder = ref
         del _fs2[name]
+
+
+_fs2enc = {}
+_FS2ENC_NAMES = ("FastspeechEncoder", "FastspeechMIDIEncoder", "DurationPredictor", "LengthRegulator")
+
+
+def install_fs2_encoder():
+    from . import fs2enc
+    for name in _FS2_MODULES:
+        try:
+            mod = importlib.import_module(name)
+        except ModuleNotFoundError as e:
+            if e.name is None or not name.startswith(e.name):      # a missing dependency, not a missing module
+                raise
+            continue
+        for attr in _FS2ENC_NAMES:
+            if not hasattr(mod, attr):
+                continue
+            _fs2enc.setdefault((name, attr), getattr(mod, attr))
+            setattr(mod, attr, getattr(fs2enc, attr))
+    return fs2enc.FastspeechMIDIEncoder
+
+
+def uninstall_fs2_encoder():
+    for (name, attr), ref in list(_fs2enc.items()):
+        mod = sys.modules.get(name)
+        if mod is not None:
+            setattr(mod, attr, ref)
+        del _fs2enc[(name, attr)]

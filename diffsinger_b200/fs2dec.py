@@ -67,32 +67,33 @@ class TransformerEncoderLayer(nn.Module):
         self.op = EncSALayer(hidden_size, num_heads, kernel_size, padding, act)
 
 
-def _fs2dec_config(hidden_size, num_layers, kernel_size, num_heads, padding, act):
-    """-> Fs2DecConfig, or DsxError for what the kernels do not run."""
+def _fs2dec_config(hidden_size, num_layers, kernel_size, num_heads, padding, act, prefix="dec", what="decoder"):
+    """-> Fs2DecConfig, or DsxError for what the kernels do not run (prefix, what: the hparams' and the model's names)."""
     H, L, k, heads = int(hidden_size), int(num_layers), int(kernel_size), int(num_heads)
     problems = []
     if not (64 <= H <= 256 and H % 64 == 0):
         problems.append(f"hidden_size = {H} (a multiple of 64 in [64, 256])")
     if not 1 <= L <= 64:
-        problems.append(f"dec_layers = {L} (1..64)")
+        problems.append(f"{prefix}_layers = {L} (1..64)")
     if heads < 1 or H % heads or H // heads not in (64, 128):
         problems.append(f"num_heads = {heads} (hidden_size / num_heads must be 64 or 128)")
     if padding not in _PADDING:
         problems.append(f"ffn_padding = {padding!r} ('SAME' or 'LEFT')")
     if not 1 <= k <= 255 or (padding == 'SAME' and k % 2 == 0):
-        problems.append(f"dec_ffn_kernel_size = {k} (odd for 'SAME', <= 255)")
+        problems.append(f"{prefix}_ffn_kernel_size = {k} (odd for 'SAME', <= 255)")
     if act not in _ACT:
         problems.append(f"ffn_act = {act!r} ('gelu' or 'relu')")
     if problems:
-        raise DsxError("unsupported FastSpeech2 decoder configuration: " + "; ".join(problems))
+        raise DsxError(f"unsupported FastSpeech2 {what} configuration: " + "; ".join(problems))
     cfg = _capi.Fs2DecConfig()
     cfg.hidden, cfg.layers, cfg.kernel, cfg.heads = H, L, k, heads
     cfg.padding, cfg.act = _PADDING[padding], _ACT[act]
     return cfg
 
 
-def fs2dec_params(num_layers, padding, t, arr):
-    """Fs2DecParams of the FFTBlocks stack under the reference's state-dict names (t, arr: see PackedModule._ensure)."""
+def fs2dec_params(num_layers, padding, t, arr, alpha=True):
+    """Fs2DecParams of the FFTBlocks stack under the reference's state-dict names (t, arr: see PackedModule._ensure);
+    alpha=False: a stack without pos_embed_alpha (the encoder's)."""
     ops = [f"layers.{i}.op" for i in range(num_layers)]
     ffn1 = ".ffn.ffn_1." if padding == 'SAME' else ".ffn.ffn_1.1."
     return _capi.Fs2DecParams(
@@ -102,7 +103,7 @@ def fs2dec_params(num_layers, padding, t, arr):
         ln2_w=arr([o + ".layer_norm2.weight" for o in ops]), ln2_b=arr([o + ".layer_norm2.bias" for o in ops]),
         ffn1_w=arr([o + ffn1 + "weight" for o in ops]), ffn1_b=arr([o + ffn1 + "bias" for o in ops]),
         ffn2_w=arr([o + ".ffn.ffn_2.weight" for o in ops]), ffn2_b=arr([o + ".ffn.ffn_2.bias" for o in ops]),
-        ln_w=t("layer_norm.weight"), ln_b=t("layer_norm.bias"), pos_embed_alpha=t("pos_embed_alpha"))
+        ln_w=t("layer_norm.weight"), ln_b=t("layer_norm.bias"), pos_embed_alpha=t("pos_embed_alpha") if alpha else None)
 
 
 class FastspeechDecoder(PackedModule):

@@ -475,6 +475,100 @@ typedef struct {
  * get_decode_inp's output exactly 0) gives eps = get_mel_out.bias. */
 int dsx_load_fft(dsx_handle* h, const dsx_fft_config* cfg, const dsx_fft_params* p, void* stream);
 
+/* ---- FastSpeech2 encoder: phoneme tokens -> encoder_out --------------------------------------------------------------
+ * Replaces: FastspeechEncoder.forward(txt_tokens) (modules/fastspeech/tts_modules.py:310-347) and
+ * FastspeechMIDIEncoder.forward(txt_tokens, midi_embedding, midi_dur_embedding, slur_embedding)
+ * (modules/diffsinger_midi/fs2.py:11-36), in eval mode with use_pos_embed: the token embedding scaled by sqrt(H), the
+ * MIDI addends, the position term, then FFTBlocks without pos_embed_alpha (tts_modules.py:282-307) whose padding mask is
+ * txt_tokens == 0.  The layers are the FastSpeech2 decoder's (fp16 operands, fp32 accumulation, residual stream and
+ * output).  An encoder handle is independent of the other handles. */
+typedef struct dsx_fs2enc dsx_fs2enc;
+
+typedef struct {
+  dsx_fs2dec_config stack; /* hidden_size, enc_layers, enc_ffn_kernel_size, num_heads, ffn_padding, ffn_act: as the
+                              decoder's                                                                         */
+  int vocab;               /* rows of embed_tokens (len(dictionary)), >= 1                                      */
+  int pos;                 /* 0: SinusoidalPositionalEmbedding over the tokens (common_layers.py:88-143), added;
+                              1: RelPositionalEncoding (modules/commons/espnet_positional_embedding.py:91-113,
+                              rel_pos: true): x = x * sqrt(H) + pe[t]                                           */
+} dsx_fs2enc_config;
+
+typedef struct {
+  dsx_fs2dec_params stack; /* layers.*, layer_norm.*; pos_embed_alpha is not used (NULL)                        */
+  const float* embed_w;    /* embed_tokens.weight [vocab, H]                                                    */
+} dsx_fs2enc_params;
+
+/* Replaces: FastspeechEncoder / FastspeechMIDIEncoder(embed_tokens, hidden_size, num_layers, kernel_size, num_heads).
+ * Validates like dsx_fs2dec_create plus vocab and pos (DSX_E_INVALID, "unsupported ..."). */
+int dsx_fs2enc_create(int device, const dsx_fs2enc_config* cfg, dsx_fs2enc** out);
+void dsx_fs2enc_destroy(dsx_fs2enc* h);
+/* Replaces: load_state_dict of encoder.* (embed_tokens is the shared encoder_embed_tokens).  Call again after every
+ * change of the weights. */
+int dsx_fs2enc_load(dsx_fs2enc* h, const dsx_fs2enc_params* p, void* stream);
+
+/* Replaces: the encoder's forward.
+ *   tokens   int64 [B, T] contiguous; 0 is padding.  A token outside [0, vocab) reads as a zero embedding row (the caller
+ *            is expected to reject it first, as nn.Embedding does);
+ *   add[i]   NULL or fp32 logically [B, T, H] with element strides as[i] (b, c = channel, t): midi_embedding,
+ *            midi_dur_embedding, slur_embedding, added in that order after the scaled token embedding;
+ *   rel_len  pos 1: the length P of the RelPositionalEncoding table (5000, or the largest T the module has seen when
+ *            larger); row t of it holds position P - 1 - t.  Requires T <= P.  Ignored for pos 0;
+ *   out      encoder_out [B, T, H] contiguous fp32; padding rows are 0.
+ * Each utterance gives the same bits as that utterance alone at the same T; one whose tokens are all padding gives 0. */
+int dsx_fs2enc_forward(dsx_fs2enc* h, const int64_t* tokens, int B, int T, const float* const* add, const dsx_strides* as,
+                       int rel_len, float* out, void* stream);
+
+/* ---- Duration predictor ----------------------------------------------------------------------------------------------
+ * Replaces: DurationPredictor.forward / .inference (modules/fastspeech/tts_modules.py:59-151) with dur_loss 'mse', in eval
+ * mode: n_layers x [ConstantPad1d + Conv1d, ReLU, LayerNorm over channels (eps 1e-12), * !mask], Linear(n_chans, 1),
+ * * !mask, and out2dur.  The convolutions run on the pitch extractor's tensor-core conv kernel (fp16 operands, fp32
+ * accumulation); LayerNorm, the linear head and out2dur are fp32 in the last convolution's epilogue. */
+typedef struct dsx_durpred dsx_durpred;
+
+typedef struct {
+  int idim;              /* input channels: a multiple of 16 in [16, 256]                                       */
+  int chans;             /* n_chans (predictor_hidden, or hidden_size when that is <= 0): same range            */
+  int layers;            /* n_layers (dur_predictor_layers): 1..16                                              */
+  int kernel;            /* kernel_size (dur_predictor_kernel): 1..31, odd for SAME                             */
+  int padding;           /* 0 'SAME' ((k - 1) / 2 each side), 1 'LEFT' (k - 1 on the left)                      */
+  float offset;          /* out2dur's offset (1.0)                                                              */
+} dsx_durpred_config;
+
+typedef struct {
+  const float* const* conv_w;        /* conv.i.1.weight [chans, C_in, k], HOST array of n_layers device pointers  */
+  const float* const* conv_b;        /* conv.i.1.bias [chans]                                                     */
+  const float* const* ln_w;          /* conv.i.3.weight [chans]                                                   */
+  const float* const* ln_b;          /* conv.i.3.bias [chans]                                                     */
+  const float* linear_w;             /* linear.weight [1, chans]                                                  */
+  const float* linear_b;             /* linear.bias [1]                                                           */
+} dsx_durpred_params;
+
+int dsx_durpred_create(int device, const dsx_durpred_config* cfg, dsx_durpred** out);
+void dsx_durpred_destroy(dsx_durpred* h);
+int dsx_durpred_load(dsx_durpred* h, const dsx_durpred_params* p, void* stream);
+
+/* Replaces: DurationPredictor.forward(xs, x_masks) (-> xs) and .inference(xs, x_masks) (-> dur, xs).
+ *   x     fp32 logically [B, T, idim], element strides xs_ (b, c = channel, t);
+ *   mask  uint8 [B, T] contiguous, 1 = padding (the reference's src_padding);
+ *   xs    [B, T] contiguous fp32: the log-domain prediction, 0 on padding rows;
+ *   dur   [B, T] contiguous int64 or NULL: clamp(round_half_even(exp(xs) - offset), 0), 0 on padding rows. */
+int dsx_durpred_forward(dsx_durpred* h, const float* x, dsx_strides xs_, const uint8_t* mask, int B, int T, float* xs,
+                        int64_t* dur, void* stream);
+
+/* ---- Length regulator ------------------------------------------------------------------------------------------------
+ * Replaces: LengthRegulator.forward(dur, dur_padding, alpha) (modules/fastspeech/tts_modules.py:159-189) in two calls,
+ * because T_mel depends on the data, without its [B, T_txt, T_mel] temporaries.  Both run on the current device.
+ *
+ * dsx_length_totals: d = round_half_even(float(dur) * alpha) * !pad (pad: uint8 [B, T] or NULL), cum [B, T] int64 its
+ * inclusive prefix sum per utterance, totals [B + 1] int64: totals[b] = cum[b, T - 1], totals[B] = 1 when any d < 0
+ * (else 0).  One small copy of totals to the host gives T_mel = max totals[b] and the error flag.
+ * dsx_length_regulate: mel2ph [B, T_mel] int64: for frame f < totals[b], the 1-based index of the token whose
+ * [cum - d, cum) holds f; 0 from totals[b] on.  Bit-identical to the reference for non-negative d. */
+int dsx_length_totals(const int64_t* dur, const uint8_t* pad, int B, int T, float alpha, int64_t* cum, int64_t* totals,
+                      void* stream);
+int dsx_length_regulate(const int64_t* cum, const int64_t* totals, int B, int T, int T_mel, int64_t* mel2ph,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif
