@@ -11,6 +11,7 @@ PRECISIONS = {"fp32": PREC_FP32_SIMT, "fp32_simt": PREC_FP32_SIMT, "fp16": PREC_
               "fp16x3": PREC_FP16X3, "fp16s": PREC_FP16S}
 (INFO_PRECISION, INFO_KERNEL_LAUNCHES, INFO_WORKSPACE_BYTES, INFO_SM_COUNT, INFO_TC_CTA_GROUP, INFO_LAYER_KERNEL_NS,
  INFO_LAYER_KERNEL_LAUNCHES, INFO_STACK_MODE, INFO_CLUSTER_OCCUPANCY, INFO_STACK_KERNEL_LAUNCHES, INFO_STACK_ROWS) = range(11)
+TRACE_SLOTS = 256        # DSX_TRACE_SLOTS: int64 stamps per CTA row of dsx_debug_trace
 OPT_TC_CTA_GROUP, OPT_CP_PREFETCH, OPT_PROFILE, OPT_STACK_MODE, OPT_STACK_KERNEL, OPT_SR_SETS, OPT_BATCH_OFFSET, OPT_GATE_APPROX, OPT_STACK_ROWS, OPT_FUSED_HEAD = 0, 1, 2, 3, 4, 5, 6, 7, 8, 9
 SCHEDULE_BUFFERS = (
     "betas", "alphas_cumprod", "alphas_cumprod_prev", "sqrt_alphas_cumprod",

@@ -18,10 +18,14 @@
 //
 // Operands reach shared memory in the 128-byte-swizzled K-major layout wgmma reads (dsx_ptx.cuh) through a ring of R
 // stages: one stage = a 256-row x 64-k weight tile (32 KB, shared by the warpgroups), packed already swizzled and moved
-// by one bulk copy, + one 64 x 64 activation block per warpgroup, copied by cp.async (the taps shift frames and
-// zero-fill).  Each slot has a full barrier (the bulk copy's bytes and every thread's cp.async) and an empty barrier (one
-// arrival per warpgroup when its MMAs of the slot are done).  The ring runs on across GEMM phases: before an epilogue
-// starts, the first R stages of the next phase are issued, so the weight stream does not stop while the epilogues run.
+// by one bulk copy, + the A operands that are not resident: 64 x 64 activation blocks per warpgroup, copied by cp.async
+// (zero-filled outside [0, T)).  Each slot has a full barrier (the bulk copy's bytes and one arrival per thread, after
+// its cp.async if it copied a block) and an empty barrier (one arrival per warpgroup when its MMAs of the slot are done).
+// The ring runs on across GEMM phases: before an epilogue starts, the first R stages of the next phase are issued, so
+// the weight stream does not stop while the epilogues run.  With P <= 2 (R = 3) GEMM1's taps are not streamed: the
+// tile's conv input, frames t0 - 8 .. t0 + 64 NWG + 8, is copied once into a resident window, and tap j's A descriptor
+// starts (j - 1) d rows away from the warpgroup's rows.  Both chunks read it, so each element of y crosses L2 -> SM once
+// per layer instead of six times.  fp16x3 (R = 2) reads y's lo plane too and keeps streaming its taps.
 // Each warpgroup's rows go through the same instruction sequence whatever NWG is, so 64- and 128-frame CTAs give
 // bit-identical results.  While GEMM1 runs, the warpgroup prefetches the CP, x and skip rows its epilogues read into L2,
 // and the epilogues issue their global loads in batches ahead of their stores.
@@ -53,26 +57,45 @@ constexpr int kABytes = 64 * 128;          // one activation block: 64 rows x 64
 constexpr int kZBytes = 4 * kABytes;       // one plane (4 k-blocks) of a warpgroup's z / h / x_in operand
 constexpr int kEpiBatch = 8;               // accumulator pairs whose global loads a layer epilogue issues at once
 
+constexpr int kHalo = 8;                   // conv-input window rows beyond each end of a tile: the largest dilation
+                                           // (dilation_cycle_length <= 4 on this path, dsx_load_diffnet)
+
 // Shared memory of k_hp_step<NWG, R> from a 1024-aligned base (the dynamic allocation adds 1 KB for the alignment):
-//   R ring slots of STAGE bytes | full[R], empty[R] mbarriers (1 KB, keeps z aligned) | z hi plane, NWG x 32 KB | LO
-// R = 3 (P <= 2: fp16, fp16x2, fp16s): the residual layers never read z's lo plane; only the head does (HP = 3), and
-// during the head's H2 and input-projection GEMMs the ring carries weights only.  So lo k-block kb < 3 of warpgroup wg
-// lives in wg's activation block of slot kb, and LO holds k-block 3, NWG x 8 KB.
-// R = 2 (fp16x3, P = 3 inside the layers): LO is the whole lo plane, NWG x 32 KB.
-template <int NWG, int R>
+//   R ring slots of STAGE bytes | full[R], empty[R], window[4] mbarriers (1 KB, keeps what follows aligned) | ...
+// WIN (R = 3; P <= 2: fp16, fp16x2, fp16s): GEMM1 reads its three taps from one conv-input window per tile, so the ring
+// carries weight tiles only.  After the barriers:
+//   W, NWG x 40 KB: in the layers the window, 4 channel blocks of WROWS = 64 NWG + 2 kHalo rows (frames t0 - kHalo ..
+//     t0 + 64 NWG + kHalo of the tile), NWG x 8 + 2 KB each.  Once every warpgroup is done with GEMM1 chunk 1, its first
+//     NWG x 16 KB take z hi k-blocks 2-3 (the window is reloaded only after GEMM2).  In the head, z hi k-blocks 2-3 and
+//     then R activation slots of NWG x 8 KB for H1's A blocks; h's lo k-blocks 0..2 live in them (H2 and the input
+//     projection carry weights only).
+//   z hi k-blocks 0-1, NWG x 16 KB | LO: z lo k-block 3 (the layers never read z lo; the head does, HP = 3), NWG x 8 KB
+// !WIN (R = 2, fp16x3, P = 3 inside the layers; and the conditioner projection): a ring slot also holds one 64 x 64
+//   activation block per warpgroup, copied with the stage, and z is whole: hi plane NWG x 32 KB | LO plane NWG x 32 KB.
+template <int NWG, int R, bool WIN = (R == 3)>
 struct StepCfg {
   static_assert(R == 2 || R == 3, "ring depth");
   static constexpr int THREADS = NWG * 128;
-  static constexpr int STAGE = kWBytes + NWG * kABytes;
+  static constexpr int STAGE = kWBytes + (WIN ? 0 : NWG * kABytes);
   static constexpr int BARS = R * STAGE;
-  static constexpr int ZHI = BARS + 1024;
-  static constexpr int ZLO = ZHI + NWG * kZBytes;
+  static constexpr int W = BARS + 1024;
+  static constexpr int WROWS = 64 * NWG + 2 * kHalo;
+  static constexpr int WBLK = WROWS * 128;
+  static constexpr int ZHI23 = 2 * kABytes;                       // z hi k-blocks 2-3 of one warpgroup, in W
+  static constexpr int ASLOT = NWG * ZHI23;                       // the head's activation slots, in W
+  static constexpr int WSIZE = WIN ? std::max(4 * WBLK, ASLOT + R * NWG * kABytes) : 0;
+  static constexpr int ZHI = W + WSIZE;
+  static constexpr int ZHI_WG = WIN ? 2 * kABytes : kZBytes;      // z hi bytes per warpgroup at ZHI
+  static constexpr int ZLO = ZHI + NWG * ZHI_WG;
   static constexpr int SMEM = 1024 + ZLO + NWG * (R == 2 ? kZBytes : kABytes);
-  // NWG = 2: 1 + 3 x 48 + 1 + 64 + 16 KB (R = 3) or 1 + 2 x 48 + 1 + 128 KB (R = 2) = 226 KB, of 227 KB
+  static_assert(WBLK % 1024 == 0 && ASLOT % 1024 == 0, "window blocks and activation slots start 1024-aligned");
+  static_assert(!WIN || NWG * ZHI23 <= WSIZE, "z hi k-blocks 2-3 fit in W");
+  // NWG = 2: 1 + 3 x 32 + 1 + 80 (window 72) + 32 + 16 KB (R = 3) or 1 + 2 x 48 + 1 + 64 + 64 KB (R = 2) = 226 KB, of
+  // 227 KB.  NWG = 1, R = 3: 1 + 96 + 1 + 40 + 16 + 8 = 162 KB.
   static_assert(SMEM <= 232448, "shared memory budget (227 KB per block on sm_90)");
 };
-// the conditioner projection: the ring and its barriers only
-constexpr int kCondSmem = 1024 + StepCfg<2, 3>::BARS + 2 * 3 * 8;
+// the conditioner projection: the ring (with activation blocks) and its barriers only
+constexpr int kCondSmem = 1024 + StepCfg<2, 3, false>::BARS + 2 * 3 * 8;
 
 struct HpParams {
   const __half* w;           // residual-layer weights: wpack (hi / lo planes) or one stochastically rounded set
@@ -153,6 +176,19 @@ __device__ __forceinline__ void load_a(uint8_t* dst, const __half* src, int b, i
     cp16(d + sw128(r, c), src + (static_cast<size_t>(b) * Tp + (valid ? t : 0)) * kC + ch0 + c * 8, valid);
   }
 }
+// One channel block of a conv-input window: rows r < rows hold frame t_first + r of one utterance (utt: its [Tp][256]
+// frames), channels [ch0, ch0 + 64); frames outside [0, T) read as zero.  dst is 1024-aligned, so a wgmma descriptor
+// started at any row reads 64 consecutive frames.  Called by the NT threads of the CTA.
+template <int NT>
+__device__ __forceinline__ void load_wblock(uint8_t* dst, const __half* utt, int t_first, int ch0, int rows, int T, int tid) {
+  const uint32_t d = smem_u32(dst);
+#pragma unroll 1
+  for (int i = tid; i < rows * 8; i += NT) {
+    const int r = i >> 3, c = i & 7, t = t_first + r;
+    const bool valid = t >= 0 && t < T;
+    cp16(d + sw128(r, c), utt + static_cast<size_t>(valid ? t : 0) * kC + ch0 + c * 8, valid);
+  }
+}
 
 template <int N>
 __device__ __forceinline__ void fence_acc(float (&d)[N]) {
@@ -170,28 +206,36 @@ __device__ __forceinline__ uint8_t* smem_base() {
 }
 
 // The shared memory of one CTA, laid out as StepCfg says (the conditioner projection has no z): the operand ring, its
-// barriers, and this warpgroup's z operand.  Addresses are recomputed from the base where they are used, so only n
-// stays live: the stages consumed so far in the launch.  Every thread runs the same GEMM phases, so n is the same in
-// all of them; ring stage i uses slot i % R in barrier phase i / R.
-template <int NWG, int R>
+// barriers, and this warpgroup's z operand.  Addresses are recomputed from the base where they are used, so only n and
+// nw stay live: the stages consumed so far in the launch, and the conv-input windows.  Every thread runs the same GEMM
+// phases, so both are the same in all of them; ring stage i uses slot i % R in barrier phase i / R, window j completes
+// phase j of the window barriers.
+template <int NWG, int R, bool WIN = (R == 3)>
 struct Smem {
-  using Cfg = StepCfg<NWG, R>;
-  uint32_t n;
+  using Cfg = StepCfg<NWG, R, WIN>;
+  uint32_t n, nw;
   __device__ __forceinline__ uint8_t* slot(uint32_t i) const { return smem_base() + (i % R) * Cfg::STAGE; }
   __device__ __forceinline__ uint32_t full(uint32_t i) const { return smem_u32(smem_base() + Cfg::BARS) + (i % R) * 8; }
   __device__ __forceinline__ uint32_t empty(uint32_t i) const { return full(i) + R * 8; }
   __device__ __forceinline__ uint32_t parity(uint32_t i) const { return (i / R) & 1; }
-  // this warpgroup's activation block in slot j
-  __device__ __forceinline__ uint8_t* ablk(int j) const {
-    return smem_base() + j * Cfg::STAGE + kWBytes + (threadIdx.x >> 7) * kABytes;
+  // channel block c of the conv-input window (WIN) and its barrier
+  __device__ __forceinline__ uint8_t* wblk(int c) const { return smem_base() + Cfg::W + c * Cfg::WBLK; }
+  __device__ __forceinline__ uint32_t wbar(int c) const { return full(0) + 2 * R * 8 + c * 8; }
+  // warpgroup wg's activation block in slot j
+  __device__ __forceinline__ uint8_t* ablk(int j, int wg) const {
+    if (WIN) return smem_base() + Cfg::W + Cfg::ASLOT + j * NWG * kABytes + wg * kABytes;
+    return smem_base() + j * Cfg::STAGE + kWBytes + wg * kABytes;
   }
-  // k-block kb of z plane 0 (hi) or 1 (lo).  With R = 3 the lo plane may only be used while no activation block is in
-  // flight in the ring (the head's H2 and input projection, StepCfg).
+  // k-block kb of z plane 0 (hi) or 1 (lo).  With WIN, hi k-blocks 2-3 share W with the window, and the lo plane may
+  // only be used while no activation block is in flight in the ring (the head's H2 and input projection, StepCfg).
   __device__ __forceinline__ uint8_t* zblk(int plane, int kb) const {
     const int wg = threadIdx.x >> 7;
-    if (plane == 0) return smem_base() + Cfg::ZHI + wg * kZBytes + kb * kABytes;
-    if (R == 2) return smem_base() + Cfg::ZLO + wg * kZBytes + kb * kABytes;
-    return kb < R ? ablk(kb) : smem_base() + Cfg::ZLO + wg * kABytes;
+    if (plane == 0) {
+      if (WIN && kb >= 2) return smem_base() + Cfg::W + wg * Cfg::ZHI23 + (kb - 2) * kABytes;
+      return smem_base() + Cfg::ZHI + wg * Cfg::ZHI_WG + kb * kABytes;
+    }
+    if (!WIN) return smem_base() + Cfg::ZLO + wg * kZBytes + kb * kABytes;
+    return kb < R ? ablk(kb, wg) : smem_base() + Cfg::ZLO + wg * kABytes;
   }
   // (row r, channel k) of z plane `plane`
   __device__ __forceinline__ uint8_t* zat(int plane, int r, int k) const {
@@ -199,11 +243,14 @@ struct Smem {
   }
   __device__ __forceinline__ void init() {
     n = 0;
+    nw = 0;
     if (threadIdx.x == 0) {
       for (int j = 0; j < R; ++j) {
-        mbar_init(full(j), 1 + NWG * 128);     // the bulk copy's arrive.expect_tx + every thread's cp.async arrival
+        mbar_init(full(j), 1 + NWG * 128);     // the bulk copy's arrive.expect_tx + one arrival per thread
         mbar_init(empty(j), NWG);              // one release per warpgroup
       }
+      if (WIN)
+        for (int c = 0; c < 4; ++c) mbar_init(wbar(c), NWG * 128);   // every thread's cp.async arrival
       fence_mbar_init();
     }
     __syncthreads();
@@ -232,8 +279,9 @@ struct StageSrc {
   const __half* w0;   // packed weight tile, or its rows 0..127 when w1 is set
   const __half* w1;   // rows 128..255 from a second 128-row tile, or nullptr
   uint32_t wbytes;    // bytes of each weight copy
-  const __half* a;    // plane whose 64 x 64 block is copied into the slot; nullptr: the A operand is z
+  const __half* a;    // plane whose 64 x 64 block is copied into the slot; nullptr: the A operand is z or the window
   int b, at, ach;     // that block: utterance, first frame (may lie outside [0, T)), first channel
+  int wrow;           // >= 0: the A operand is window block ach / 64 from this row on (GEMM1 with WIN)
   int zplane, zkb;    // otherwise the plane and k-block of z
 };
 
@@ -261,7 +309,7 @@ __device__ __forceinline__ int phase_stages(const HpParams& p, const Phase& ph) 
   return kbs * phase_passes(p, ph.kind);
 }
 
-template <int NWG>
+template <int NWG, bool WIN>
 __device__ __forceinline__ StageSrc stage_src(const HpParams& p, const Phase& ph, int s) {
   const int frame0 = ph.u * 64 * NWG;
   const int P = phase_passes(p, ph.kind);
@@ -273,15 +321,22 @@ __device__ __forceinline__ StageSrc stage_src(const HpParams& p, const Phase& ph
   st.b = frame0 / p.Tp;
   st.at = frame0 % p.Tp + (threadIdx.x >> 7) * 64;
   st.ach = kb * 64;
+  st.wrow = -1;
   st.zplane = ap;
   st.zkb = kb;
   switch (ph.kind) {
-    case PH_G1:   // [y(t-d) | y(t) | y(t+d)]: k-block kb = tap * 4 + channel block
+    case PH_G1: {  // [y(t-d) | y(t) | y(t+d)]: k-block kb = tap * 4 + channel block
+      const int shift = ((kb >> 2) - 1) * (1 << (ph.l % p.cycle));
       st.w0 = w1_tile(p, ph.l, wp, ph.hq, kb);
-      st.a = p.Y + static_cast<size_t>(ph.l & 1) * 2 * p.plane + ap * p.plane;
-      st.at += ((kb >> 2) - 1) * (1 << (ph.l % p.cycle));
       st.ach = (kb & 3) * 64;
+      if (WIN) {   // P <= 2: every pass reads y's hi plane, resident in the window
+        st.wrow = kHalo + (threadIdx.x >> 7) * 64 + shift;
+      } else {
+        st.a = p.Y + static_cast<size_t>(ph.l & 1) * 2 * p.plane + ap * p.plane;
+        st.at += shift;
+      }
       break;
+    }
     case PH_G2:
       st.w0 = w2_tile(p, ph.l, wp, ph.hq, kb);
       break;
@@ -312,9 +367,11 @@ enum { kIssueW = 1, kIssueA = 2 };
 // Issues the parts of ring stage i: the weight tile (thread 0, once the slot's previous stage is released by every
 // warpgroup) and this warpgroup's activation block (every thread; its own MMAs of the slot's previous stage are done).
 // Every thread arrives on the full barrier with its A part, block or not, so the stage completes only when both parts
-// have landed.
-template <int NWG, int R>
-__device__ __forceinline__ void issue(const HpParams& p, const Smem<NWG, R>& sm, const StageSrc& st, uint32_t i, int parts) {
+// have landed.  With WIN a thread without a block arrives at once, so the stage does not wait for the window it may
+// have in flight.
+template <int NWG, int R, bool WIN>
+__device__ __forceinline__ void issue(const HpParams& p, const Smem<NWG, R, WIN>& sm, const StageSrc& st, uint32_t i,
+                                      int parts) {
   const uint32_t full = sm.full(i);
   uint8_t* slot = sm.slot(i);
   if ((parts & kIssueW) && threadIdx.x == 0) {
@@ -324,17 +381,33 @@ __device__ __forceinline__ void issue(const HpParams& p, const Smem<NWG, R>& sm,
     if (st.w1) bulk_g2s(smem_u32(slot) + st.wbytes, st.w1, st.wbytes, full);
   }
   if (parts & kIssueA) {
-    if (st.a) load_a(slot + kWBytes + (threadIdx.x >> 7) * kABytes, st.a, st.b, st.at, st.ach, p.T, p.Tp, threadIdx.x & 127);
-    cp_arrive_noinc(full);
+    if (st.a) load_a(sm.ablk(i % R, threadIdx.x >> 7), st.a, st.b, st.at, st.ach, p.T, p.Tp, threadIdx.x & 127);
+    if (WIN && !st.a) mbar_arrive(full);
+    else cp_arrive_noinc(full);
   }
 }
 
-// Issues parts of the first R stages of phase ph, the next one the ring will run (all its slots are released).
-template <int NWG, int R>
-__device__ __forceinline__ void fill(const HpParams& p, const Smem<NWG, R>& sm, const Phase& ph, int parts) {
+// The conv input of both GEMM1 chunks of tile u in layer l, into the window (StepCfg), copied by every thread of the
+// CTA.  Each channel block completes on its own barrier, so the first MMAs wait for block 0 only.
+template <int NWG, int R, bool WIN>
+__device__ __forceinline__ void load_window(const HpParams& p, const Smem<NWG, R, WIN>& sm, int l, int u) {
+  const int frame0 = u * 64 * NWG;
+  const __half* utt = p.Y + static_cast<size_t>(l & 1) * 2 * p.plane + static_cast<size_t>(frame0 / p.Tp) * p.Tp * kC;
+#pragma unroll 1
+  for (int c = 0; c < 4; ++c) {
+    load_wblock<NWG * 128>(sm.wblk(c), utt, frame0 % p.Tp - kHalo, c * 64, StepCfg<NWG, R, WIN>::WROWS, p.T, threadIdx.x);
+    cp_arrive_noinc(sm.wbar(c));
+  }
+}
+
+// Issues parts of the first R stages of phase ph, the next one the ring will run (all its slots are released).  With
+// WIN, the A part of GEMM1 chunk 0 is the tile's window; the caller makes sure no warpgroup still reads z from W.
+template <int NWG, int R, bool WIN>
+__device__ __forceinline__ void fill(const HpParams& p, const Smem<NWG, R, WIN>& sm, const Phase& ph, int parts) {
+  if (WIN && ph.kind == PH_G1 && ph.hq == 0 && (parts & kIssueA)) load_window(p, sm, ph.l, ph.u);
   const int n = min(R, phase_stages(p, ph));
 #pragma unroll 1
-  for (int j = 0; j < n; ++j) issue(p, sm, stage_src<NWG>(p, ph, j), sm.n + j, parts);
+  for (int j = 0; j < n; ++j) issue(p, sm, stage_src<NWG, WIN>(p, ph, j), sm.n + j, parts);
 }
 
 // c0 (weight rows 0..127) [and c1 (rows 128..255) when NH == 2] = sum over the stages s of phase ph of A_s . W_s^T.  The
@@ -342,9 +415,9 @@ __device__ __forceinline__ void fill(const HpParams& p, const Smem<NWG, R>& sm, 
 // wgmma group in flight behind the copies.  pre(s) runs after that (L2 prefetches of what the epilogues read, paced so
 // that they queue behind the operand copies).  Every thread of the CTA runs it; it ends with the accumulators complete
 // and every slot released by this warpgroup.
-template <int NH, int NWG, int R, class Pre = NoPrefetch>
-__device__ __forceinline__ void gemm(float (&c0)[64], float (&c1)[64], Smem<NWG, R>& sm, const HpParams& p, const Phase& ph,
-                                     Pre pre = Pre()) {
+template <int NH, int NWG, int R, bool WIN, class Pre = NoPrefetch>
+__device__ __forceinline__ void gemm(float (&c0)[64], float (&c1)[64], Smem<NWG, R, WIN>& sm, const HpParams& p,
+                                     const Phase& ph, Pre pre = Pre()) {
   const int nst = phase_stages(p, ph);
   const int wg = threadIdx.x >> 7;
   // the epilogue before this phase wrote z with st.shared: visible to the warpgroup's wgmmas from here
@@ -355,11 +428,16 @@ __device__ __forceinline__ void gemm(float (&c0)[64], float (&c1)[64], Smem<NWG,
 #pragma unroll 1
   for (int s = 0; s < nst; ++s) {
     const uint32_t i = sm.n + s;
-    const StageSrc st = stage_src<NWG>(p, ph, s);
+    const StageSrc st = stage_src<NWG, WIN>(p, ph, s);
     mbar_wait(sm.full(i), sm.parity(i));
-    fence_proxy_async_smem();   // the cp.async writes of the activation block -> the async proxy of wgmma
+    if (WIN && st.wrow >= 0) mbar_wait(sm.wbar(st.ach >> 6), sm.nw & 1);
+    fence_proxy_async_smem();   // the cp.async writes of the activation block or window -> the async proxy of wgmma
     uint8_t* slot = sm.slot(i);
-    const uint64_t a = wg_desc(smem_u32(st.a ? slot + kWBytes + wg * kABytes : sm.zblk(st.zplane, st.zkb)));
+    // (without WIN, ablk is slot + kWBytes + wg * kABytes; spelled out from slot, the R = 2 form spills less)
+    const uint8_t* aop = WIN && st.wrow >= 0 ? sm.wblk(st.ach >> 6) + st.wrow * 128
+                         : st.a ? (WIN ? sm.ablk(i % R, wg) : slot + kWBytes + wg * kABytes)
+                                : sm.zblk(st.zplane, st.zkb);
+    const uint64_t a = wg_desc(smem_u32(aop));
     const uint64_t w = wg_desc(smem_u32(slot));
     wg_fence();
 #pragma unroll
@@ -372,7 +450,7 @@ __device__ __forceinline__ void gemm(float (&c0)[64], float (&c1)[64], Smem<NWG,
     if (s > 0) {
       wg_wait1();
       if ((threadIdx.x & 127) == 0) mbar_arrive(sm.empty(i - 1));
-      if (s - 1 + R < nst) issue(p, sm, stage_src<NWG>(p, ph, s - 1 + R), i - 1 + R, kIssueW | kIssueA);
+      if (s - 1 + R < nst) issue(p, sm, stage_src<NWG, WIN>(p, ph, s - 1 + R), i - 1 + R, kIssueW | kIssueA);
     }
     pre(s);
   }
@@ -386,8 +464,8 @@ __device__ __forceinline__ void gemm(float (&c0)[64], float (&c1)[64], Smem<NWG,
 // ------------------------------------------------------------------------------------------
 // one residual layer of one tile
 // ------------------------------------------------------------------------------------------
-template <int NWG, int R>
-__device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem<NWG, R>& sm) {
+template <int NWG, int R, bool WIN>
+__device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem<NWG, R, WIN>& sm) {
   const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
   const int frame0 = u * 64 * NWG;
   const int b = frame0 / p.Tp, t0 = frame0 % p.Tp + wg * 64;
@@ -410,6 +488,12 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem
     gemm<2>(c0, c1, sm, p, Phase{PH_G1, l, u, h}, pre);
     // chunk 1's weights and taps do not depend on this epilogue; GEMM2's weights do not depend on either
     fill(p, sm, h == 0 ? Phase{PH_G1, l, u, 1} : Phase{PH_G2, l, u, 0}, kIssueW | kIssueA);
+    if (WIN && h == 1) {
+      // the window is spent; z hi k-blocks 2-3, which this epilogue writes, overlap it, and the other warpgroup's
+      // rows of it may still be read
+      sm.nw++;
+      __syncthreads();
+    }
     stamp(p, layer_slot(p, l, 2 * h));
     const float* cp = p.CP + (static_cast<size_t>(l) * NF + fbase) * 512 + h * 256;
     // the loads of kEpiBatch accumulator pairs are issued together, ahead of the stores that use them
@@ -452,8 +536,12 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem
   for (int q = 0; q < 2; ++q) {
     gemm<2>(c0, c1, sm, p, Phase{PH_G2, l, u, q});
     if (q == 0) fill(p, sm, Phase{PH_G2, l, u, 1}, kIssueW | kIssueA);
-    else if (u + static_cast<int>(gridDim.x) < p.units) fill(p, sm, Phase{PH_G1, l, u + static_cast<int>(gridDim.x), 0}, kIssueW | kIssueA);
-    else fill(p, sm, after_layer(p, l), kIssueW);   // its activation blocks are issued after the grid barrier
+    else if (u + static_cast<int>(gridDim.x) < p.units) {
+      if (WIN) __syncthreads();   // the next tile's window overlaps the z k-blocks the other warpgroup may still read
+      fill(p, sm, Phase{PH_G1, l, u + static_cast<int>(gridDim.x), 0}, kIssueW | kIssueA);
+    } else {
+      fill(p, sm, after_layer(p, l), kIssueW);   // its activation blocks or window are issued after the grid barrier
+    }
     stamp(p, layer_slot(p, l, 4 + 2 * q));
     // This thread's accumulators cover rows row0 and row0 + 8 and columns colb + 8 i + {0, 1} of each 128-column half
     // (acc_row / acc_col), so every address below is a per-thread base plus a compile-time offset; with the offsets
@@ -539,7 +627,7 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, Smem<NWG, R>
 
   if (do_head) {
     // H1: h = relu(s16 . W_s^T + b_s) -> fp16 hi / lo operand.  H2 carries weights only, so h's lo plane may take the
-    // ring's activation blocks (StepCfg).
+    // activation slots (StepCfg).
     gemm<2>(c0, c1, sm, p, Phase{PH_H1, 0, u, 0});
     fill(p, sm, Phase{PH_H2, 0, u, 0}, kIssueW | kIssueA);
     stamp(p, head_slot(p, 0));
@@ -677,7 +765,7 @@ __global__ void __launch_bounds__(NWG * 128, 1) k_hp_step(const __grid_constant_
 // CP[l][frame][h * 256 + n] = cond . W1cond^T (hi / lo operands, 3 passes) + dilated_conv.bias + conditioner_projection.bias,
 // for job (tile of 128 frames, layer) = (blockIdx.x, blockIdx.y)
 __global__ void __launch_bounds__(256, 1) k_hp_condproj(const __grid_constant__ HpParams p) {
-  Smem<2, 3> sm;   // the ring only: no z operand
+  Smem<2, 3, false> sm;   // the ring only, activation blocks included: no z operand, no window
   sm.init();
   const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
   const int u = blockIdx.x, l = blockIdx.y;
@@ -1039,9 +1127,50 @@ int launch_tc_stack(dsx_handle* h, int nl, const Geom& g, int row0, int row_per_
 struct SelfParams {
   const __half* a;   // [T][256] fp16, one utterance
   const __half* w;   // [256 rows][64], plain (BULK = false) or packed as the kernels' weights (sw128_elem)
-  float* out;        // [64][256]
+  float* out;        // [64][256] ([128][256] for the window)
   int t0, T;
+  int off;           // window: row offset of the A operand from row kHalo + 64 wg (a tap's frame shift)
 };
+
+// GEMM1's conv-input window as k_hp_step<2, 3> holds it: channel block 1 of the window of the 128-frame tile at t0,
+// copied by all 256 threads onto an mbarrier that the packed weight tile's bulk copy also completes.  Warpgroup wg
+// multiplies the 64 rows from window row kHalo + 64 wg + off, a descriptor start that is not 1024-aligned.
+__global__ void __launch_bounds__(256, 1) k_selftest_window(const __grid_constant__ SelfParams p) {
+  uint8_t* base = smem_base();
+  uint8_t* win = base + kWBytes;
+  const uint32_t full = smem_u32(win + StepCfg<2, 3>::WBLK);
+  const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127;
+  float c0[64], c1[64];
+  if (tid == 0) {
+    mbar_init(full, 1 + 256);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(full, kWBytes);
+    bulk_g2s(smem_u32(base), p.w, kWBytes, full);
+  }
+  load_wblock<256>(win, p.a, p.t0 - kHalo, 64, StepCfg<2, 3>::WROWS, p.T, tid);
+  cp_arrive_noinc(full);
+  mbar_wait(full, 0);
+  fence_proxy_async_smem();
+  const uint64_t a = wg_desc(smem_u32(win + (kHalo + wg * 64 + p.off) * 128)), w = wg_desc(smem_u32(base));
+  wg_fence();
+#pragma unroll
+  for (int k4 = 0; k4 < 4; ++k4) {
+    wgmma_n128(c0, a + 2 * k4, w + 2 * k4, k4 > 0);
+    wgmma_n128(c1, a + 2 * k4, w + (16384 >> 4) + 2 * k4, k4 > 0);
+  }
+  wg_commit();
+  wg_wait0();
+  fence_acc(c0);
+  fence_acc(c1);
+  for (int e = 0; e < 64; ++e) {
+    const int r = wg * 64 + acc_row(wtid, e), n = acc_col(wtid, e);
+    p.out[r * 256 + n] = c0[e];
+    p.out[r * 256 + 128 + n] = c1[e];
+  }
+}
 
 // BULK = false: cp.async of the plain tile into the swizzled layout; true: one bulk copy of the packed tile, completing
 // on an mbarrier together with the activation block's cp.async, as in the kernels' ring
@@ -1109,7 +1238,7 @@ static int run_selftest(std::string& report) {
   DSX_CUDA(cudaMalloc(&da, ha.size() * 2));
   DSX_CUDA(cudaMalloc(&dw, hw.size() * 2));
   DSX_CUDA(cudaMalloc(&dwp, hwp.size() * 2));
-  DSX_CUDA(cudaMalloc(&dout, 64 * 256 * 4));
+  DSX_CUDA(cudaMalloc(&dout, 128 * 256 * 4));
   DSX_CUDA(cudaMemcpy(da, ha.data(), ha.size() * 2, cudaMemcpyHostToDevice));
   DSX_CUDA(cudaMemcpy(dw, hw.data(), hw.size() * 2, cudaMemcpyHostToDevice));
   DSX_CUDA(cudaMemcpy(dwp, hwp.data(), hwp.size() * 2, cudaMemcpyHostToDevice));
@@ -1146,6 +1275,40 @@ static int run_selftest(std::string& report) {
       report += line;
       if (bad) failures++;
     }
+  // the window: tile at 0 of a 130-frame utterance (zero rows before frame 0 and from frame 130 on) and tile at 128 of
+  // the 150-frame one (real rows before the tile, zero rows after the utterance); taps at +-d for every dilation
+  const int wsmem = 1024 + kWBytes + StepCfg<2, 3>::WBLK + 8;
+  DSX_CUDA(cudaFuncSetAttribute(k_selftest_window, cudaFuncAttributeMaxDynamicSharedMemorySize, wsmem));
+  const int wins[2][2] = {{0, 130}, {128, T}};
+  const int offs[] = {-8, -4, -2, -1, 0, 1, 2, 4, 8};
+  for (const auto& wt : wins) {
+    int bad = 0;
+    double maxerr = 0;
+    for (int off : offs) {
+      SelfParams prm{da, dwp, dout, wt[0], wt[1], off};
+      DSX_CUDA(cudaMemset(dout, 0xff, 128 * 256 * 4));
+      k_selftest_window<<<1, 256, wsmem>>>(prm);
+      DSX_CUDA(cudaGetLastError());
+      DSX_CUDA(cudaDeviceSynchronize());
+      std::vector<float> out(128 * 256);
+      DSX_CUDA(cudaMemcpy(out.data(), dout, out.size() * 4, cudaMemcpyDeviceToHost));
+      for (int m = 0; m < 128; ++m)
+        for (int n = 0; n < 256; ++n) {
+          double ref = 0;
+          const int t = wt[0] + m + off;
+          if (t >= 0 && t < wt[1])
+            for (int k = 0; k < 64; ++k) ref += static_cast<double>(aval(t, 64 + k)) * wval(n, k);
+          const double e = fabs(ref - out[static_cast<size_t>(m) * 256 + n]);
+          if (!(e <= 1e-4)) bad++;
+          if (e > maxerr || e != e) maxerr = e;
+        }
+    }
+    char line[160];
+    snprintf(line, sizeof(line), "wgmma_m64n128k16 window t0=%d T=%d rows 8+-{0,1,2,4,8}, 2 warpgroups: bad=%d/294912 maxerr=%.3g\n",
+             wt[0], wt[1], bad, maxerr);
+    report += line;
+    if (bad) failures++;
+  }
   cudaFree(da);
   cudaFree(dw);
   cudaFree(dwp);

@@ -372,6 +372,17 @@ class DsxSampler:
     def set_layer_limit(self, n):
         check(lib.dsx_debug_set_layer_limit(self._h, n), "dsx_debug_set_layer_limit")
 
+    def debug_trace(self, enable):
+        """Phase timeline of the step kernel (dsx_debug_trace; slot layout in include/dsx.h).  debug_trace(True) clears the
+        trace and records every later step-kernel launch into it; debug_trace(False) stops recording and returns the
+        last launch's stamps as int64 [2 * SM count, DSX_TRACE_SLOTS] (%globaltimer ns per CTA row, 0 = not reached)."""
+        if enable:
+            check(lib.dsx_debug_trace(self._h, 1, None), "dsx_debug_trace")
+            return None
+        out = torch.zeros((2 * self.info(_capi.INFO_SM_COUNT), _capi.TRACE_SLOTS), dtype=torch.int64)
+        check(lib.dsx_debug_trace(self._h, 0, _ptr(out)), "dsx_debug_trace")
+        return out
+
 
 def selftest(device=0, which=-1):
     buf = ctypes.create_string_buffer(16384)
