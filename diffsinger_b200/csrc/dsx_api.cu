@@ -35,7 +35,7 @@ int dev_alloc(dsx_handle* h, void** p, size_t bytes, bool model_owned) {
 }
 
 static void free_ws(Workspace& w) {
-  void* ptrs[] = {w.X, w.SKIP, w.CONDF, w.G1, w.Zf, w.Y, w.CONDH, w.CP, w.S16, w.DTAB, w.EMB, w.TVALS, w.EPS, w.XTMP, w.XSTATE};
+  void* ptrs[] = {w.X, w.SKIP, w.CONDF, w.G1, w.Zf, w.Y, w.CONDH, w.CP, w.S16, w.FLAGS, w.DTAB, w.EMB, w.TVALS, w.EPS, w.XTMP, w.XSTATE};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   w = Workspace();
@@ -73,6 +73,7 @@ int ensure_workspace(dsx_handle* h, const Geom& g, int rows, cudaStream_t s) {
       NEED(Y, nf * m.C * 2 * 4);
       NEED(CONDH, nf * m.H * 2 * 2);
       NEED(S16, nf * m.C * 2 * 2);
+      NEED(FLAGS, nf / 64 * 2 * sizeof(unsigned));   // two per tile at the smallest tile height, 64 frames
       NEED(CP, static_cast<size_t>(m.L) * nf * 2 * m.C * 4);
       if (cond_before[0] != w.CONDH || cond_before[1] != w.CP) h->cond_ready = false;
     } else {

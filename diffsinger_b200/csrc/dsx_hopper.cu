@@ -3,8 +3,8 @@
 //   k_hp_step<NWG>   residual layers [l0, l1) of one DiffNet evaluation (usr/diff/net.py:58-78) and, optionally, what
 //                    follows them in a diffusion step: skip / output projections, the DDPM or PNDM update and the next
 //                    evaluation's input projection (net.py:115-130, shallow_diffusion_tts.py:134-199).  Persistent and
-//                    cooperative: every CTA walks over the frame tiles of a layer, a grid-wide barrier separates layers
-//                    (layer l+1 of a tile reads the conv input of its neighbour tiles).
+//                    cooperative: every CTA walks over the frame tiles of a layer, and a tile starts layer l+1 once its
+//                    neighbour tiles, whose conv input it reads, have published layer l (wait_layer).
 //   k_hp_condproj    conditioner projection of every layer, once per call (it does not depend on the diffusion step).
 //
 // Per residual layer and tile of 64 frames (one warpgroup; a CTA has NWG warpgroups = 64 * NWG frames):
@@ -32,7 +32,6 @@
 //
 // Precision (MMA passes P per k-block): P = 1 fp16 operands; P = 2 adds a W_lo pass (weights as hi+lo fp16 pairs);
 // P = 3 accumulates A_hi*W_hi + A_hi*W_lo + A_lo*W_hi (~2^-22 relative).  The conditioner projection is always 3-pass.
-#include <cooperative_groups.h>
 #include <stdio.h>
 #include <string.h>
 
@@ -45,11 +44,9 @@
 #include "dsx_ptx.cuh"
 #include "dsx_rng.cuh"
 
-namespace cg = cooperative_groups;
-
 namespace dsx {
 
-constexpr int kC = 256;                    // residual / conditioner channels supported by this path
+constexpr int kC = 256;                   // residual / conditioner channels supported by this path
 constexpr int kRowsPerLayer = 80 * 256;    // wpack rows (of 64 fp16) per layer: 64 W1 tiles + 16 W2 tiles of 256 rows
 constexpr int kSrRowsPerLayer = 32 * 256;  // rows per layer of one stochastically rounded weight set: 24 W1 + 8 W2 tiles
 constexpr int kWBytes = 256 * 128;         // one weight tile: 256 rows x 64 fp16
@@ -137,6 +134,8 @@ struct HpParams {
   int M;
   long long* trace;          // dsx_debug_trace buffer [trace_ctas][DSX_TRACE_SLOTS], or nullptr
   int trace_ctas;
+  unsigned* flags;           // [2][units] per-tile progress in this launch, zeroed before it: layers done | layers whose
+                             // GEMM1 and gates are done (paired tiles only)
 };
 
 // phase stamp of dsx_debug_trace (layout in dsx.h); one uniform branch when tracing is off
@@ -149,6 +148,54 @@ __device__ __forceinline__ void stamp(const HpParams& p, int slot) {
 }
 __device__ __forceinline__ int layer_slot(const HpParams& p, int l, int k) { return 1 + 9 * (l - p.l0) + k; }
 __device__ __forceinline__ int head_slot(const HpParams& p, int k) { return 1 + 9 * (p.l1 - p.l0) + k; }
+
+// ------------------------------------------------------------------------------------------
+// ordering between tiles
+// ------------------------------------------------------------------------------------------
+// Layer l of a tile reads y of layer l - 1 from its own frames and at most kHalo frames into its neighbour tiles of the
+// same utterance; x, skip, CP and S16 of a tile are read by that tile only, and windows zero-fill frames outside [0, T),
+// so tiles of different utterances never read each other.  So instead of a grid-wide barrier between layers, every
+// tile publishes p.flags[u] = layers done (after its residual epilogue wrote y) and a tile waits only for its
+// neighbours.  Waiting for the neighbours to finish layer l - 1 also means they have read Y buffer (l + 1) & 1 for the
+// last time before the tile overwrites it in layer l.
+//
+// Deadlock freedom: every CTA is resident (cooperative launch) and visits (layer, tile) in layer-major order, and a
+// wait at layer l is only ever for layer l - 1 or, between paired tiles, for an earlier point of layer l.  The CTA that
+// owns the awaited point is either past it or itself waiting at a strictly earlier point, and the earliest waiting
+// point of all waits for nothing that is not already done.
+//
+// Pairing: when every tile has its own CTA, tile j of utterance 2k + 1 starts layer l only after tile j of utterance
+// 2k has finished GEMM1 and the gates of layer l (p.flags[units + u]).  The two groups then run half a layer apart, so
+// one group's L2-bound GEMMs overlap the other's HBM-bound epilogues.  This is scheduling only: the tiles share no data.
+template <int NWG>
+__device__ __forceinline__ int partner_tile(const HpParams& p, int u) {
+  if (p.units > static_cast<int>(gridDim.x) || p.B < 2) return -1;
+  const int tpu = p.Tp / (64 * NWG), b = u / tpu;
+  if (b & 1) return u - tpu;
+  return b + 1 < p.B ? u + tpu : -1;
+}
+
+// thread 0: spins until the neighbours of tile u in its utterance have published n layers
+template <int NWG>
+__device__ __forceinline__ void wait_neighbours(const HpParams& p, int u, unsigned n) {
+  const int tpu = p.Tp / (64 * NWG);
+  if (u % tpu != 0) wait_geq(p.flags + u - 1, n);
+  if ((u + 1) % tpu != 0) wait_geq(p.flags + u + 1, n);
+}
+
+// Holds the CTA until tile u may start layer l.  Thread 0's acquire loads, followed by the __syncthreads, order the
+// neighbours' y writes before every thread's later reads of them: the window and the streamed taps are non-bulk
+// cp.async, which reads through the generic proxy.  (A bulk copy of the window would need a proxy fence after this.)
+template <int NWG>
+__device__ __forceinline__ void wait_layer(const HpParams& p, int l, int u) {
+  if (threadIdx.x == 0) {
+    const unsigned n = l - p.l0;
+    if (n > 0) wait_neighbours<NWG>(p, u, n);
+    const int pu = partner_tile<NWG>(p, u);
+    if (pu >= 0 && pu < u) wait_geq(p.flags + p.units + pu, n + 1);
+  }
+  __syncthreads();
+}
 
 // ------------------------------------------------------------------------------------------
 // operand loads and the GEMM loop
@@ -526,6 +573,8 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem
       }
     }
     stamp(p, layer_slot(p, l, 2 * h + 1));
+    // an even-utterance tile lets its partner start layer l (wait_layer)
+    if (h == 1 && tid == 0 && partner_tile<NWG>(p, u) > u) st_release_gpu(p.flags + p.units + u, l - p.l0 + 1);
   }
 
   // ---- GEMM2 + residual / skip epilogues ----
@@ -537,10 +586,14 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem
     gemm<2>(c0, c1, sm, p, Phase{PH_G2, l, u, q});
     if (q == 0) fill(p, sm, Phase{PH_G2, l, u, 1}, kIssueW | kIssueA);
     else if (u + static_cast<int>(gridDim.x) < p.units) {
-      if (WIN) __syncthreads();   // the next tile's window overlaps the z k-blocks the other warpgroup may still read
-      fill(p, sm, Phase{PH_G1, l, u + static_cast<int>(gridDim.x), 0}, kIssueW | kIssueA);
+      const Phase next{PH_G1, l, u + static_cast<int>(gridDim.x), 0};
+      fill(p, sm, next, kIssueW);
+      // the wait ends in a __syncthreads, which also keeps the next tile's window off the z k-blocks the other
+      // warpgroup may still read
+      wait_layer<NWG>(p, l, next.u);
+      fill(p, sm, next, kIssueA);
     } else {
-      fill(p, sm, after_layer(p, l), kIssueW);   // its activation blocks or window are issued after the grid barrier
+      fill(p, sm, after_layer(p, l), kIssueW);   // its activation blocks or window are issued after the next wait
     }
     stamp(p, layer_slot(p, l, 4 + 2 * q));
     // This thread's accumulators cover rows row0 and row0 + 8 and columns colb + 8 i + {0, 1} of each 128-column half
@@ -607,6 +660,11 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem
       }
     }
     stamp(p, layer_slot(p, l, 5 + 2 * q));
+    if (q == 0) {
+      // y of layer l is written: publish it to the neighbours
+      __syncthreads();
+      if (tid == 0) st_release_gpu(p.flags + u, l - p.l0 + 1);
+    }
   }
 }
 
@@ -718,6 +776,11 @@ __device__ __forceinline__ void head_tile(const HpParams& p, int u, Smem<NWG, R>
   gemm<2>(c0, c1, sm, p, Phase{PH_IN, 0, u, 0});
   fill(p, sm, head_phase(p, u + gridDim.x), kIssueW | kIssueA);
   stamp(p, head_slot(p, 4));
+  if (p.l1 > p.l0) {
+    // Y buffer 0, written below, is the conv input of layer L - 1 when L is odd: the neighbours must be done with it
+    if (tid == 0) wait_neighbours<NWG>(p, u, p.l1 - p.l0);
+    __syncthreads();
+  }
   const float* d0 = p.d0 + static_cast<size_t>(b) * p.d0_row_stride;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
@@ -747,19 +810,22 @@ __global__ void __launch_bounds__(NWG * 128, 1) k_hp_step(const __grid_constant_
   Smem<NWG, R> sm;
   sm.init();
   stamp(p, 0);
-  fill(p, sm, p.l0 < p.l1 ? Phase{PH_G1, p.l0, static_cast<int>(blockIdx.x), 0} : head_phase(p, blockIdx.x),
-       kIssueW | kIssueA);
+  const int u0 = blockIdx.x;
+  fill(p, sm, p.l0 < p.l1 ? Phase{PH_G1, p.l0, u0, 0} : head_phase(p, u0), kIssueW);
   for (int l = p.l0; l < p.l1; ++l) {
-    for (int u = blockIdx.x; u < p.units; u += gridDim.x) layer_tile<NWG, R>(p, l, u, sm);
-    if (l + 1 < p.l1 || p.head_flags) {
-      // every thread gets here with its ring copies issued and none of its barrier waits pending
-      cg::this_grid().sync();
-      stamp(p, layer_slot(p, l, 8));
-      fill(p, sm, after_layer(p, l), kIssueA);
-    }
+    // every thread gets here with its ring copies issued and none of its barrier waits pending
+    wait_layer<NWG>(p, l, u0);
+    if (l > p.l0) stamp(p, layer_slot(p, l - 1, 8));
+    fill(p, sm, Phase{PH_G1, l, u0, 0}, kIssueA);
+    for (int u = u0; u < p.units; u += gridDim.x) layer_tile<NWG, R>(p, l, u, sm);
   }
-  if (p.head_flags)
-    for (int u = blockIdx.x; u < p.units; u += gridDim.x) head_tile<NWG, R>(p, u, sm);
+  if (p.head_flags) {
+    // the head reads the tile's own S16 rows, written by other threads of the CTA
+    __syncthreads();
+    if (p.l0 < p.l1) stamp(p, layer_slot(p, p.l1 - 1, 8));
+    fill(p, sm, head_phase(p, u0), kIssueA);
+    for (int u = u0; u < p.units; u += gridDim.x) head_tile<NWG, R>(p, u, sm);
+  }
 }
 
 // CP[l][frame][h * 256 + n] = cond . W1cond^T (hi / lo operands, 3 passes) + dilated_conv.bias + conditioner_projection.bias,
@@ -989,6 +1055,7 @@ static HpParams base_params(dsx_handle* h, const Geom& g, int rows) {
   prm.bin = m.in_b;
   prm.trace = h->trace_on ? reinterpret_cast<long long*>(h->trace_dev) : nullptr;
   prm.trace_ctas = 2 * h->sm_count;
+  prm.flags = h->ws.FLAGS;
   return prm;
 }
 
@@ -1017,7 +1084,10 @@ static int launch_step(dsx_handle* h, const HpParams& prm, cudaStream_t s) {
   cfg.blockDim = dim3(StepCfg<NWG, R>::THREADS);
   cfg.dynamicSmemBytes = StepCfg<NWG, R>::SMEM;
   cfg.stream = s;
-  // cooperative: the layers of one launch are separated by grid-wide barriers, so every CTA must be resident
+  // The progress flags count from zero in every launch that runs layers.  A memset on the stream, rather than an epoch
+  // kept by the host, stays right under graph replay and when the batch geometry changes between calls.
+  if (prm.l1 > prm.l0) DSX_CUDA(cudaMemsetAsync(prm.flags, 0, 2 * static_cast<size_t>(prm.units) * sizeof(unsigned), s));
+  // cooperative: tiles spin-wait on the progress flags of other CTAs (wait_layer), so every CTA must be resident
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeCooperative;
   attr[0].val.cooperative = 1;

@@ -181,6 +181,7 @@ struct Workspace {
   __half* CONDH = nullptr;  // [2 planes][B][Tp][H]
   float* CP = nullptr;      // [L][B][Tp][512] conditioner projection + bias of every layer (tensor-core path)
   __half* S16 = nullptr;    // [2 planes][B][Tp][C] skip_sum / sqrt(L), operand of the head GEMM
+  unsigned* FLAGS = nullptr; // [2][B * Tp / 64] per-tile progress flags of the step kernel (tensor-core path)
   float* DTAB = nullptr;    // [rows][L][C]
   float* EMB = nullptr;     // [rows][C] scratch (mlp output)
   int64_t* TVALS = nullptr; // [rows]
@@ -190,7 +191,7 @@ struct Workspace {
   size_t bytes = 0;
   // byte capacities (grow-only)
   size_t cap_X = 0, cap_SKIP = 0, cap_CONDF = 0, cap_G1 = 0, cap_Zf = 0, cap_Y = 0, cap_CONDH = 0, cap_CP = 0, cap_S16 = 0,
-         cap_DTAB = 0, cap_EMB = 0, cap_TVALS = 0, cap_EPS = 0, cap_XTMP = 0, cap_XSTATE = 0;
+         cap_FLAGS = 0, cap_DTAB = 0, cap_EMB = 0, cap_TVALS = 0, cap_EPS = 0, cap_XTMP = 0, cap_XSTATE = 0;
 };
 
 struct FftDenoiser;   // dsx_fftdiff.cu

@@ -146,6 +146,23 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                : "memory");
 }
 
+// ---- progress flags between CTAs ----------------------------------------------------------------
+// release: the writes this thread has made or observed (through a __syncthreads before it) become visible at gpu scope
+// to any thread whose acquire load reads the value
+__device__ __forceinline__ void st_release_gpu(unsigned* p, unsigned v) {
+  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
+  unsigned v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+// spins until *p >= n
+__device__ __forceinline__ void wait_geq(const unsigned* p, unsigned n) {
+  while (ld_acquire_gpu(p) < n) {
+  }
+}
+
 // ---- global memory hints ------------------------------------------------------------------------
 // bytes (a multiple of 16) at a 16-byte aligned global address -> L2, asynchronously; nothing waits for it
 __device__ __forceinline__ void prefetch_l2(const void* src, uint32_t bytes) {

@@ -199,8 +199,9 @@ enum {
                                epilogue operands (conditioner projection, x, skip) into L2 */
   DSX_OPT_PROFILE = 2,      /* 1: bracket the residual-layer kernel(s) of every evaluation with CUDA events; 2: bracket the
                                head / update kernel of every DDPM step instead; 0: off.  Setting it resets the sums */
-  DSX_OPT_STACK_MODE = 3,   /* 1 (default): all residual layers of an evaluation in ONE persistent cooperative launch (grid-wide
-                               barrier between layers); 0: one launch per layer */
+  DSX_OPT_STACK_MODE = 3,   /* 1 (default): all residual layers of an evaluation in ONE persistent cooperative launch (a tile
+                               starts a layer when its neighbour tiles have finished the one before); 0: one launch per
+                               layer */
   DSX_OPT_STACK_KERNEL = 4, /* 1 (default): for FP16 / FP16X2 / FP16S the layers and the head of a step share ONE launch, with
                                64-frame CTAs for small batches and FP16S's stochastically rounded weight sets; 0: the layers use
                                the hi/lo weight planes at 128 frames per CTA (FP16S then runs the FP16X2 scheme) */
@@ -228,8 +229,9 @@ int dsx_debug_read(dsx_handle* h, int which, float* out, int B, int T, void* str
  *   slot 0                                launch entry
  *   slot 1 + 9 i + k, i = layer - l0      k = 0 / 2: GEMM1 chunk 0 / 1 end, 1 / 3: gate epilogue 0 / 1 end,
  *                                         4 / 6: GEMM2 residual / skip half end, 5 / 7: residual / skip epilogue end,
- *                                         8: exit of the grid barrier after the layer (0 when no barrier
- *                                         follows: the last layer of a launch without a head)
+ *                                         8: end of the wait before the next layer (for the neighbour tiles and,
+ *                                         between paired utterances, the partner tile) or before the head (0
+ *                                         when nothing follows: the last layer of a launch without a head)
  *   slot 1 + 9 n + k, n = layers launched head: k = 0 H1 GEMM end, 1 H1 epilogue end, 2 H2 GEMM end, 3 mel update end,
  *                                         4 input projection GEMM end, 5 input projection epilogue end
  * Slots past DSX_TRACE_SLOTS are not recorded (at most 27 layers per launch). */

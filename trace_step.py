@@ -7,7 +7,12 @@ Runs a bench.py config and records the step kernel's phase stamps (dsx_debug_tra
 last launch of each of N timed steps: with the fused head, one launch is one whole diffusion step.  Prints the mean µs
 of each layer phase over the CTAs, layers and steps, and of the head phases, with the card's name, power limit and the
 median SM clock during the traced steps.  A CTA that walks over several tiles of a layer (config 4) stamps its last
-tile only, so there GEMM1 chunk 0 also holds its earlier tiles; the layer total stays right.
+tile only, so there GEMM1 chunk 0 also holds its earlier tiles; the layer total stays right.  The last layer phase is the
+wait for the neighbour tiles (and, for paired utterances, the partner) that ends where the next layer starts.
+
+When the kernel runs the even and the odd utterances half a layer apart (every tile has its own CTA and B >= 2), the
+phase split is also printed for each of the two groups, with the mean time by which an odd-utterance tile starts a
+layer after its even partner.
 """
 import argparse
 import json
@@ -22,13 +27,36 @@ import numpy as np
 import torch
 
 LAYER_PHASES = ("GEMM1 chunk 0", "gate epilogue 0", "GEMM1 chunk 1", "gate epilogue 1", "GEMM2 residual half",
-                "residual epilogue", "GEMM2 skip half", "skip epilogue", "grid barrier")
+                "residual epilogue", "GEMM2 skip half", "skip epilogue", "wait before next layer")
 HEAD_PHASES = ("H1 GEMM", "H1 epilogue", "H2 GEMM", "mel update", "input projection GEMM", "input projection epilogue")
 
 
-def phase_split(tr, layers):
-    """tr: int64 [CTAs, slots] stamps of one launch over `layers` layers and the head.  -> (layer [n_phases] µs summed over
-    the CTAs and layers, number of (CTA, layer) samples, head [6] µs summed over the CTAs, CTAs)"""
+def utterance_groups(B, T, rows, ctas):
+    """Trace rows (CTAs) of the even and of the odd utterances when the step kernel runs them half a layer apart (every
+    tile has its own CTA and B >= 2: tile j of utterance 2k + 1 is paired with tile j of utterance 2k), else None.
+    -> (even rows, odd rows, [(even, odd) partner rows])"""
+    tpu = -(-T // 128) * 128 // rows
+    if B < 2 or B * tpu > ctas:
+        return None
+    u = np.arange(B * tpu)
+    b = u // tpu
+    pairs = [(int(i), int(i + tpu)) for i in u[(b % 2 == 0) & (b + 1 < B)]]
+    return u[b % 2 == 0], u[b % 2 == 1], pairs
+
+
+def start_offset(tr, layers, pairs):
+    """mean µs by which a paired odd-utterance tile starts layers 1 .. layers - 1 after its even partner (slot 8 of the
+    layer before: the end of the wait that starts the layer)"""
+    d = [tr[o, 9 * i] - tr[e, 9 * i] for e, o in pairs for i in range(1, layers) if tr[o, 9 * i] and tr[e, 9 * i]]
+    return float(np.mean(d)) * 1e-3 if d else None
+
+
+def phase_split(tr, layers, ctas=None):
+    """tr: int64 [CTAs, slots] stamps of one launch over `layers` layers and the head; ctas: the rows to use (all when
+    None).  -> (layer [n_phases] µs summed over the CTAs and layers, number of (CTA, layer) samples, head [6] µs summed
+    over the CTAs, CTAs)"""
+    if ctas is not None:
+        tr = tr[ctas]
     tr = tr[tr[:, 0] != 0].astype(np.float64)
     lay = np.zeros(len(LAYER_PHASES))
     n = 0
@@ -38,7 +66,7 @@ def phase_split(tr, layers):
         s = tr[:, base:base + 9]
         if i == layers - 1 and not s[:, 8].any():
             s = s.copy()
-            s[:, 8] = s[:, 7]                     # no grid barrier after the last layer of a launch without a head
+            s[:, 8] = s[:, 7]                     # no wait after the last layer of a launch without a head
         d = np.diff(np.concatenate([prev[:, None], s], axis=1), axis=1)
         lay += d.sum(axis=0)
         n += len(tr)
@@ -92,13 +120,22 @@ def main():
     torch.cuda.synchronize()
     cs = bench.ClockSampler(0)
     cs.start()
+    layers = bench.hp_for(cfg)["residual_layers"]
     lay, n, head, nh = np.zeros(len(LAYER_PHASES)), 0, np.zeros(len(HEAD_PHASES)), 0
+    glay, gn, offs = [np.zeros(len(LAYER_PHASES)), np.zeros(len(LAYER_PHASES))], [0, 0], []
+    groups = None
     for i in range(args.steps):
         arm.s.debug_trace(True)
         arm.step(args.warmup + i)
         tr = arm.s.debug_trace(False).numpy()
-        l_sum, l_n, h_sum, h_n = phase_split(tr, bench.hp_for(cfg)["residual_layers"])
+        l_sum, l_n, h_sum, h_n = phase_split(tr, layers)
         lay, n, head, nh = lay + l_sum, n + l_n, head + h_sum, nh + h_n
+        groups = utterance_groups(cfg["B"], cfg["T"], arm.s.info(_capi.INFO_STACK_ROWS), int((tr[:, 0] != 0).sum()))
+        if groups:
+            for g in range(2):
+                l_sum, l_n, _, _ = phase_split(tr, layers, groups[g])
+                glay[g], gn[g] = glay[g] + l_sum, gn[g] + l_n
+            offs.append(start_offset(tr.astype(np.float64), layers, groups[2]))
     cs.mark_end()
     clk = cs.finish()
     rows = arm.s.info(_capi.INFO_STACK_ROWS)
@@ -110,6 +147,14 @@ def main():
            "samples": {"cta_layers": n, "steps": args.steps},
            "layer_us": dict(zip(LAYER_PHASES, lay_us.round(2).tolist())), "layer_total_us": round(float(lay_us.sum()), 2),
            "head_us": dict(zip(HEAD_PHASES, head_us.round(2).tolist()))}
+    if groups:
+        res["groups"] = {}
+        for g, name in enumerate(("even utterances", "odd utterances")):
+            us = glay[g] / max(gn[g], 1)
+            res["groups"][name] = {"layer_us": dict(zip(LAYER_PHASES, us.round(2).tolist())),
+                                   "layer_total_us": round(float(us.sum()), 2)}
+        offs = [o for o in offs if o is not None]
+        res["odd_start_offset_us"] = round(float(np.mean(offs)), 2) if offs else None
     if args.json:
         print(json.dumps(res))
         return
@@ -124,6 +169,14 @@ def main():
     for k, v in res["head_us"].items():
         if v:
             print(f"  head: {k:<22s} {v:8.2f} us")
+    if groups:
+        names = list(res["groups"])
+        print(f"per group ({names[0]} | {names[1]}); an odd-utterance tile starts a layer "
+              f"{res['odd_start_offset_us']} us after its partner on average")
+        for k in LAYER_PHASES:
+            print(f"  {k:<28s} {res['groups'][names[0]]['layer_us'][k]:8.2f} {res['groups'][names[1]]['layer_us'][k]:8.2f} us")
+        print(f"  {'layer':<28s} {res['groups'][names[0]]['layer_total_us']:8.2f} "
+              f"{res['groups'][names[1]]['layer_total_us']:8.2f} us")
 
 
 if __name__ == "__main__":
