@@ -116,65 +116,71 @@ int check_status(dsx_handle* h, cudaStream_t s, const char* what) {
   return DSX_OK;
 }
 
-// Residual layers [0, nl) of one evaluation; `head` (may be null): what follows them in the step.  Returns through
-// *head_done whether the head ran inside the stack launch (the caller then skips launch_tc_head).
-static int run_layers(dsx_handle* h, const Geom& g, int row0, int row_per_b, int nl, cudaStream_t s, const HeadArgs* head = nullptr,
-                      bool* head_done = nullptr) {
-  if (head_done) *head_done = false;
-  const bool tc = h->precision != DSX_PREC_FP32_SIMT;
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  if (h->profile == 1) {
-    while (h->prof_events.size() < h->prof_used + 2) {
-      cudaEvent_t e;
-      DSX_CUDA(cudaEventCreate(&e));
-      h->prof_events.push_back(e);
-    }
-    e0 = h->prof_events[h->prof_used];
-    e1 = h->prof_events[h->prof_used + 1];
-    h->prof_used += 2;
-    DSX_CUDA(cudaEventRecord(e0, s));
+// `run` between two CUDA events on s when `on` (DSX_OPT_PROFILE), summed by DSX_INFO_LAYER_KERNEL_NS
+template <typename F>
+static int profiled(dsx_handle* h, bool on, cudaStream_t s, F&& run) {
+  if (!on) return run();
+  while (h->prof_events.size() < h->prof_used + 2) {
+    cudaEvent_t e;
+    DSX_CUDA(cudaEventCreate(&e));
+    h->prof_events.push_back(e);
   }
-  if (tc) {
-    // weight set of DSX_PREC_FP16S: evaluation (= table row) j of a loop uses set j % R
-    if (tc_stack_usable(h, g)) {
-      const bool fuse = head && head->flags && h->fused_head && nl == h->m.L && h->profile != 2;
-      DSX_TRY(launch_tc_stack(h, nl, g, row0, row_per_b, row0, s, fuse ? head : nullptr));
-      if (fuse && head_done) *head_done = true;
-    } else {
-      DSX_TRY(launch_tc_layers(h, 0, nl, g, row0, row_per_b, s));
-    }
-  } else {
-    for (int l = 0; l < nl; ++l) DSX_TRY(launch_simt_layer(h, l, g, row0, row_per_b, s));
-  }
-  if (h->profile == 1) DSX_CUDA(cudaEventRecord(e1, s));
+  const size_t i = h->prof_used;
+  h->prof_used += 2;
+  DSX_CUDA(cudaEventRecord(h->prof_events[i], s));
+  DSX_TRY(run());
+  DSX_CUDA(cudaEventRecord(h->prof_events[i + 1], s));
   return DSX_OK;
 }
 
-// One DiffNet evaluation: x (any strides) -> eps (contiguous [B,1,M,T]).
-static int run_eval(dsx_handle* h, const float* x, dsx_strides xs, const Geom& g, int row0, int row_per_b, float* eps,
-                    cudaStream_t s) {
-  if (h->fft) return fft_eval(h, x, xs, g, row0, row_per_b, eps, s);
-  const bool tc = h->precision != DSX_PREC_FP32_SIMT;
-  const int nl = (h->layer_limit >= 0) ? std::min(h->layer_limit, h->m.L) : h->m.L;
-  const DdpmCoef none{};
-  if (tc)
-    DSX_TRY(launch_tc_head(h, g, TC_INPROJ, const_cast<float*>(x), xs, nullptr, nullptr, 0, 0, none, row0, row_per_b, s));
-  else
-    DSX_TRY(launch_inproj(h, x, xs, g, row0, row_per_b, s));
-  HeadArgs ha;
-  ha.flags = TC_HEAD | TC_WRITE_EPS;
-  ha.x = const_cast<float*>(x);          // (read only with these flags)
-  ha.xs = xs;
-  ha.eps = eps;
-  bool head_done = false;
-  DSX_TRY(run_layers(h, g, row0, row_per_b, nl, s, (tc && nl == h->m.L) ? &ha : nullptr, &head_done));
-  if (nl == h->m.L && !head_done) {
-    if (tc)
-      DSX_TRY(launch_tc_head(h, g, TC_HEAD | TC_WRITE_EPS, nullptr, xs, eps, nullptr, 0, 0, none, row0, row_per_b, s));
-    else
-      DSX_TRY(launch_head(h, g, eps, s));
+// the tensor-core DiffNet kernels (fused heads, updates and input projections); the SIMT DiffNet and the FFT denoiser
+// evaluate to eps and run the fp32 update kernels
+static bool tc_diffnet(const dsx_handle* h) { return !h->fft && h->precision != DSX_PREC_FP32_SIMT; }
+
+// One evaluation of the loaded denoiser on x_in (strides ha.xs) at FiLM table row (row0, row_per_b), then what `ha`
+// asks for: eps (TC_WRITE_EPS), the DDPM (TC_UPDATE) or PLMS (TC_PLMS) update of ha.x, and on the tensor-core path the
+// input projection of the next evaluation (TC_INPROJ).  The tensor-core layers read x_in through the projection the
+// previous head made; `project` makes it here instead (a loop's first evaluation, a forward).  Fewer than L layers
+// (dsx_debug_set_layer_limit) run no head and nothing after it.
+static int evaluate(dsx_handle* h, const Geom& g, const float* x_in, int row0, int row_per_b, int nl, bool project,
+                    const HeadArgs& ha, cudaStream_t s) {
+  const bool head = nl == h->m.L;
+  if (tc_diffnet(h)) {
+    if (project) {
+      HeadArgs in;
+      in.flags = TC_INPROJ;
+      in.x = const_cast<float*>(x_in);   // read only with this flag
+      in.xs = ha.xs;
+      in.next_row0 = row0;
+      in.row_per_b = row_per_b;
+      DSX_TRY(launch_tc_step(h, g, 0, 0, row0, row_per_b, &in, s));
+    }
+    const bool fuse = head && tc_fuse_head(h);
+    DSX_TRY(profiled(h, h->profile == 1, s, [&] { return launch_tc_step(h, g, 0, nl, row0, row_per_b, fuse ? &ha : nullptr, s); }));
+    if (head && !fuse) DSX_TRY(profiled(h, h->profile == 2, s, [&] { return launch_tc_step(h, g, 0, 0, row0, row_per_b, &ha, s); }));
+    return DSX_OK;
   }
-  return DSX_OK;
+  // SIMT and FFT: eps to where the flags keep it, else to slot 4 of the EPS ring, then the fp32 update kernel
+  const size_t mel = static_cast<size_t>(g.B) * h->m.M * g.T;
+  const PlmsFuse* p = ha.plms;
+  float* eps = (ha.flags & TC_WRITE_EPS) ? ha.eps : (p && p->eps_store) ? p->eps_store : h->ws.EPS + 4 * mel;
+  if (h->fft) {
+    DSX_TRY(fft_eval(h, x_in, ha.xs, g, row0, row_per_b, eps, s));
+  } else {
+    DSX_TRY(launch_inproj(h, x_in, ha.xs, g, row0, row_per_b, s));
+    DSX_TRY(profiled(h, h->profile == 1, s, [&]() -> int {
+      for (int l = 0; l < nl; ++l) DSX_TRY(launch_simt_layer(h, l, g, row0, row_per_b, s));
+      return DSX_OK;
+    }));
+    if (!head) return DSX_OK;
+    DSX_TRY(launch_head(h, g, eps, s));
+  }
+  if (ha.flags & TC_UPDATE) return launch_ddpm_update(h, ha.x, eps, ha.noise, ha.seed, ha.offset, ha.c, mel, g.T, s);
+  if (!(ha.flags & TC_PLMS)) return DSX_OK;
+  float* x_out = p->x_out ? p->x_out : ha.x;
+  if (p->eps_store) return launch_plms_update(h, x_out, ha.x, eps, p->h1, p->h2, p->h3, p->c, mel, s);
+  // the warm-up's combine: this eps is the second of (eps_t + eps') / 2
+  return launch_plms_update(h, x_out, ha.x, p->h1, eps, nullptr, nullptr, p->c, mel, s);
 }
 
 // Workspace + tensor maps for (B, T) and, when `cond` is given, the conditioner pack and its hoisted projection (the
@@ -210,10 +216,6 @@ static int embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream
   return h->fft ? fft_embed_table(h, t_dev, rows, s) : launch_embed_table(h, t_dev, rows, s);
 }
 
-// the tensor-core DiffNet kernels (fused heads, updates and input projections); the FFT denoiser runs run_eval + the
-// fp32 update kernels
-static bool tc_diffnet(const dsx_handle* h) { return !h->fft && h->precision != DSX_PREC_FP32_SIMT; }
-
 static dsx_strides contiguous_mel(int M, int T) {
   dsx_strides xs;
   xs.b = static_cast<int64_t>(M) * T;
@@ -231,57 +233,45 @@ static int sample_ddpm_impl(dsx_handle* h, float* x, const Geom& g, int t_start,
   DSX_CUDA(cudaStreamSynchronize(s));   // tv is a stack-owned staging buffer
   DSX_TRY(embed_table(h, h->ws.TVALS, n_steps, s));
   const dsx_strides xs = contiguous_mel(h->m.M, g.T);
-  const bool tc = tc_diffnet(h);
-  if (tc) DSX_TRY(launch_tc_head(h, g, TC_INPROJ, x, xs, nullptr, nullptr, 0, 0, DdpmCoef{}, 0, 0, s));
   for (int j = 0; j < n_steps; ++j) {
     const int t = t_start - 1 - j;
-    if (!tc) DSX_TRY(run_eval(h, x, xs, g, j, 0, h->ws.EPS, s));
-    DdpmCoef c;
-    c.A = h->sched[DSX_SCH_SQRT_RECIP_ALPHAS_CUMPROD][t];
-    c.Bc = h->sched[DSX_SCH_SQRT_RECIPM1_ALPHAS_CUMPROD][t];
-    c.c1 = h->sched[DSX_SCH_POSTERIOR_MEAN_COEF1][t];
-    c.c2 = h->sched[DSX_SCH_POSTERIOR_MEAN_COEF2][t];
-    c.sigma = (t == 0) ? 0.f : expf(0.5f * h->sched[DSX_SCH_POSTERIOR_LOG_VARIANCE_CLIPPED][t]);
-    const float* nz = noise ? noise + static_cast<size_t>(j) * mel : nullptr;
-    if (tc) {
-      // 20 fused residual-layer kernels, then ONE kernel: head GEMMs + p_sample update + next step's input projection
-      const int flags = TC_HEAD | TC_UPDATE | (j + 1 < n_steps ? TC_INPROJ : 0);
-      HeadArgs ha;
-      ha.flags = flags; ha.x = x; ha.xs = xs; ha.noise = nz; ha.seed = seed; ha.offset = static_cast<uint64_t>(j); ha.c = c;
-      ha.next_row0 = j + 1; ha.row_per_b = 0;
-      bool head_done = false;
-      DSX_TRY(run_layers(h, g, j, 0, h->m.L, s, &ha, &head_done));
-      if (head_done) continue;               // ONE launch did the whole diffusion step
-      cudaEvent_t e0 = nullptr, e1 = nullptr;
-      if (h->profile == 2) {                       // DSX_OPT_PROFILE = 2: bracket the head kernel instead of the layer stack
-        while (h->prof_events.size() < h->prof_used + 2) {
-          cudaEvent_t e;
-          DSX_CUDA(cudaEventCreate(&e));
-          h->prof_events.push_back(e);
-        }
-        e0 = h->prof_events[h->prof_used];
-        e1 = h->prof_events[h->prof_used + 1];
-        h->prof_used += 2;
-        DSX_CUDA(cudaEventRecord(e0, s));
-      }
-      DSX_TRY(launch_tc_head(h, g, flags, x, xs, nullptr, nz, seed, static_cast<uint64_t>(j), c, j + 1, 0, s));
-      if (e1) DSX_CUDA(cudaEventRecord(e1, s));
-    } else {
-      DSX_TRY(launch_ddpm_update(h, x, h->ws.EPS, nz, seed, static_cast<uint64_t>(j), c, mel, g.T, s));
-    }
+    HeadArgs ha;
+    ha.flags = TC_HEAD | TC_UPDATE | (j + 1 < n_steps ? TC_INPROJ : 0);
+    ha.x = x;
+    ha.xs = xs;
+    ha.noise = noise ? noise + static_cast<size_t>(j) * mel : nullptr;
+    ha.seed = seed;
+    ha.offset = static_cast<uint64_t>(j);
+    ha.c.A = h->sched[DSX_SCH_SQRT_RECIP_ALPHAS_CUMPROD][t];
+    ha.c.Bc = h->sched[DSX_SCH_SQRT_RECIPM1_ALPHAS_CUMPROD][t];
+    ha.c.c1 = h->sched[DSX_SCH_POSTERIOR_MEAN_COEF1][t];
+    ha.c.c2 = h->sched[DSX_SCH_POSTERIOR_MEAN_COEF2][t];
+    ha.c.sigma = (t == 0) ? 0.f : expf(0.5f * h->sched[DSX_SCH_POSTERIOR_LOG_VARIANCE_CLIPPED][t]);
+    ha.next_row0 = j + 1;
+    DSX_TRY(evaluate(h, g, x, j, 0, h->m.L, j == 0, ha, s));
   }
   return DSX_OK;
 }
 
-// get_x_pred coefficients (usr/diff/shallow_diffusion_tts.py:174-185), fp32 op by op
-static void plms_coefs(const dsx_handle* h, int t, int interval, PlmsCoef& c) {
+// PLMS weights (w0, w1, w2, w3, denom) of eps_t and the earlier eps, by dsx_plms_update mode: 0 / 1 the warm-up's
+// first update and its combine, 2 / 3 / 4 with one / two / three earlier eps
+static const float kPlmsWeights[5][5] = {
+    {1.f, 0.f, 0.f, 0.f, 1.f}, {1.f, 1.f, 0.f, 0.f, 2.f}, {3.f, -1.f, 0.f, 0.f, 2.f},
+    {23.f, -16.f, 5.f, 0.f, 12.f}, {55.f, -59.f, 37.f, -9.f, 24.f}};
+
+// get_x_pred coefficients (usr/diff/shallow_diffusion_tts.py:174-185), fp32 op by op, and the weights of `mode`
+static PlmsCoef plms_coefs(const dsx_handle* h, int t, int interval, int mode) {
   const std::vector<float>& ac = h->sched[DSX_SCH_ALPHAS_CUMPROD];
   const float a_t = ac[t];
   const float a_prev = (t < interval) ? 1.0f : ac[std::max(t - interval, 0)];
   const float a_t_sq = sqrtf(a_t), a_prev_sq = sqrtf(a_prev);
+  PlmsCoef c;
   c.a_diff = a_prev - a_t;
   c.kx = 1.0f / (a_t_sq * (a_t_sq + a_prev_sq));
   c.ke = 1.0f / (a_t_sq * (sqrtf((1.0f - a_prev) * a_t) + sqrtf((1.0f - a_t) * a_prev)));
+  const float* w = kPlmsWeights[mode];
+  c.w0 = w[0]; c.w1 = w[1]; c.w2 = w[2]; c.w3 = w[3]; c.denom = w[4];
+  return c;
 }
 
 static int sample_plms_impl(dsx_handle* h, float* x, const Geom& g, int t_start, int interval, cudaStream_t s) {
@@ -299,86 +289,38 @@ static int sample_plms_impl(dsx_handle* h, float* x, const Geom& g, int t_start,
   DSX_CUDA(cudaStreamSynchronize(s));
   DSX_TRY(embed_table(h, h->ws.TVALS, n + 1, s));
   const dsx_strides xs = contiguous_mel(h->m.M, g.T);
-  float* E[5];
-  for (int i = 0; i < 5; ++i) E[i] = h->ws.EPS + static_cast<size_t>(i) * mel;
-  // history ring: hist[0] = most recent eps_t
-  float* hist[4] = {nullptr, nullptr, nullptr, nullptr};
-  int nh = 0, slot = 0;
-  const bool tc = tc_diffnet(h);
-  const DdpmCoef none{};
-  if (tc) {
-    // tcgen05 path: per evaluation the residual stack + ONE head kernel that also does the multistep combination, the
-    // get_x_pred update, the history store and the next evaluation's input projection (2 launches per PNDM step)
-    DSX_TRY(launch_tc_head(h, g, TC_INPROJ, x, xs, nullptr, nullptr, 0, 0, none, 0, 0, s));
-    for (int j = 0; j < n; ++j) {
-      const int t = steps[j];
-      float* e0 = E[slot];
-      PlmsFuse pf{};
-      plms_coefs(h, t, interval, pf.c);
-      const int next_flags = (j + 1 < n) ? TC_INPROJ : 0;
-      // residual stack of table row `row` followed by the head with `flags` / `pp` (fused into one launch where possible)
-      auto step = [&](int row, int flags, const PlmsFuse& pp, int next_row) -> int {
-        HeadArgs ha;
-        ha.flags = flags; ha.x = x; ha.xs = xs; ha.next_row0 = next_row; ha.row_per_b = 0; ha.plms = &pp;
-        bool head_done = false;
-        DSX_TRY(run_layers(h, g, row, 0, h->m.L, s, &ha, &head_done));
-        if (!head_done) DSX_TRY(launch_tc_head(h, g, flags, x, xs, nullptr, nullptr, 0, 0, none, next_row, 0, s, &pp));
-        return DSX_OK;
-      };
-      if (nh == 0) {
-        // x' = phi(x, eps_t, t) -> XTMP; eps'' = net(x', max(t - interval, 0)); eps* = (eps_t + eps'') / 2; x = phi(x, eps*, t)
-        PlmsFuse p1 = pf;
-        p1.c.w0 = 1.f; p1.c.denom = 1.f;
-        p1.eps_store = e0;
-        p1.x_out = h->ws.XTMP;
-        DSX_TRY(step(j, TC_HEAD | TC_PLMS | TC_INPROJ, p1, n));
-        pf.c.w0 = 1.f; pf.c.w1 = 1.f; pf.c.denom = 2.f;
-        pf.h1 = e0;
-        DSX_TRY(step(n, TC_HEAD | TC_PLMS | next_flags, pf, j + 1));
-      } else {
-        if (nh == 1) { pf.c.w0 = 3.f; pf.c.w1 = -1.f; pf.c.denom = 2.f; }
-        else if (nh == 2) { pf.c.w0 = 23.f; pf.c.w1 = -16.f; pf.c.w2 = 5.f; pf.c.denom = 12.f; }
-        else { pf.c.w0 = 55.f; pf.c.w1 = -59.f; pf.c.w2 = 37.f; pf.c.w3 = -9.f; pf.c.denom = 24.f; }
-        pf.h1 = hist[0];
-        pf.h2 = nh >= 2 ? hist[1] : nullptr;
-        pf.h3 = nh >= 3 ? hist[2] : nullptr;
-        pf.eps_store = e0;
-        DSX_TRY(step(j, TC_HEAD | TC_PLMS | next_flags, pf, j + 1));
-      }
-      hist[3] = hist[2]; hist[2] = hist[1]; hist[1] = hist[0]; hist[0] = e0;
-      nh = std::min(nh + 1, 4);
-      slot = (slot + 1) % 4;
-    }
-    return DSX_OK;
-  }
+  // eps_t of step j goes to slot j % 4 of the EPS ring; the three before it are the multistep history
+  auto ring = [&](int j) -> float* { return j >= 0 ? h->ws.EPS + static_cast<size_t>(j % 4) * mel : nullptr; };
   for (int j = 0; j < n; ++j) {
-    const int t = steps[j];
-    float* e0 = E[slot];
-    DSX_TRY(run_eval(h, x, xs, g, j, 0, e0, s));
-    PlmsCoef c{};
-    plms_coefs(h, t, interval, c);
-    if (nh == 0) {
-      // x' = phi(x, eps_t, t); eps' = net(x', max(t - interval, 0)); eps* = (eps_t + eps') / 2
-      PlmsCoef c1 = c;
-      c1.w0 = 1.f; c1.denom = 1.f;
-      DSX_TRY(launch_plms_update(h, h->ws.XTMP, x, e0, nullptr, nullptr, nullptr, c1, mel, s));
-      float* e1 = E[4];
-      DSX_TRY(run_eval(h, h->ws.XTMP, xs, g, n, 0, e1, s));
-      c.w0 = 1.f; c.w1 = 1.f; c.denom = 2.f;
-      DSX_TRY(launch_plms_update(h, x, x, e0, e1, nullptr, nullptr, c, mel, s));
-    } else if (nh == 1) {
-      c.w0 = 3.f; c.w1 = -1.f; c.denom = 2.f;
-      DSX_TRY(launch_plms_update(h, x, x, e0, hist[0], nullptr, nullptr, c, mel, s));
-    } else if (nh == 2) {
-      c.w0 = 23.f; c.w1 = -16.f; c.w2 = 5.f; c.denom = 12.f;
-      DSX_TRY(launch_plms_update(h, x, x, e0, hist[0], hist[1], nullptr, c, mel, s));
+    PlmsFuse pf{};
+    HeadArgs ha;
+    ha.flags = TC_HEAD | TC_PLMS | (j + 1 < n ? TC_INPROJ : 0);
+    ha.x = x;
+    ha.xs = xs;
+    ha.next_row0 = j + 1;
+    ha.plms = &pf;
+    if (j == 0) {
+      // warm-up: x' = phi(x, eps_t, t) -> XTMP; eps' = net(x', max(t - interval, 0)); x = phi(x, (eps_t + eps') / 2, t)
+      PlmsFuse first{};
+      first.c = plms_coefs(h, steps[0], interval, 0);
+      first.eps_store = ring(0);
+      first.x_out = h->ws.XTMP;
+      HeadArgs ha1 = ha;
+      ha1.flags = TC_HEAD | TC_PLMS | TC_INPROJ;
+      ha1.next_row0 = n;
+      ha1.plms = &first;
+      DSX_TRY(evaluate(h, g, x, 0, 0, h->m.L, true, ha1, s));
+      pf.c = plms_coefs(h, steps[0], interval, 1);
+      pf.h1 = ring(0);
+      DSX_TRY(evaluate(h, g, h->ws.XTMP, n, 0, h->m.L, false, ha, s));
     } else {
-      c.w0 = 55.f; c.w1 = -59.f; c.w2 = 37.f; c.w3 = -9.f; c.denom = 24.f;
-      DSX_TRY(launch_plms_update(h, x, x, e0, hist[0], hist[1], hist[2], c, mel, s));
+      pf.c = plms_coefs(h, steps[j], interval, std::min(j, 3) + 1);
+      pf.h1 = ring(j - 1);
+      pf.h2 = ring(j - 2);
+      pf.h3 = ring(j - 3);
+      pf.eps_store = ring(j);
+      DSX_TRY(evaluate(h, g, x, j, 0, h->m.L, false, ha, s));
     }
-    hist[3] = hist[2]; hist[2] = hist[1]; hist[1] = hist[0]; hist[0] = e0;
-    nh = std::min(nh + 1, 4);
-    slot = (slot + 1) % 4;
   }
   return DSX_OK;
 }
@@ -512,7 +454,13 @@ int dsx_diffnet_forward(dsx_handle* h, const float* x, dsx_strides xs, const int
   Geom g;
   DSX_TRY(prepare(h, cond, cs, B, T, B, g, s));
   DSX_TRY(embed_table(h, t, B, s));
-  DSX_TRY(run_eval(h, x, xs, g, 0, 1, eps, s));
+  HeadArgs ha;
+  ha.flags = TC_HEAD | TC_WRITE_EPS;
+  ha.x = const_cast<float*>(x);          // read only with these flags
+  ha.xs = xs;
+  ha.eps = eps;
+  const int nl = (h->layer_limit >= 0) ? std::min(h->layer_limit, h->m.L) : h->m.L;
+  DSX_TRY(evaluate(h, g, x, 0, 1, nl, true, ha, s));
   return check_status(h, s, "dsx_diffnet_forward");
 }
 
@@ -535,18 +483,9 @@ int dsx_plms_update(dsx_handle* h, float* x_out, const float* x_in, const float*
   static const int n_eps[5] = {1, 2, 2, 3, 4};
   for (int i = 0; i < n_eps[mode]; ++i) DSX_CHECK(eps[i], DSX_E_INVALID, "mode %d needs %d eps tensors", mode, n_eps[mode]);
   DSX_CUDA(cudaSetDevice(h->device));
-  PlmsCoef c{};
-  plms_coefs(h, t, interval, c);
-  switch (mode) {
-    case 0: c.w0 = 1.f; c.denom = 1.f; break;
-    case 1: c.w0 = 1.f; c.w1 = 1.f; c.denom = 2.f; break;
-    case 2: c.w0 = 3.f; c.w1 = -1.f; c.denom = 2.f; break;
-    case 3: c.w0 = 23.f; c.w1 = -16.f; c.w2 = 5.f; c.denom = 12.f; break;
-    default: c.w0 = 55.f; c.w1 = -59.f; c.w2 = 37.f; c.w3 = -9.f; c.denom = 24.f; break;
-  }
   const size_t mel = static_cast<size_t>(B) * h->m.M * T;
   return launch_plms_update(h, x_out, x_in, eps[0], n_eps[mode] > 1 ? eps[1] : nullptr, n_eps[mode] > 2 ? eps[2] : nullptr,
-                            n_eps[mode] > 3 ? eps[3] : nullptr, c, mel, s);
+                            n_eps[mode] > 3 ? eps[3] : nullptr, plms_coefs(h, t, interval, mode), mel, s);
 }
 
 int dsx_sample_ddpm(dsx_handle* h, float* x_inout, const float* cond, dsx_strides cs, int B, int T, int t_start,

@@ -1059,20 +1059,19 @@ static HpParams base_params(dsx_handle* h, const Geom& g, int rows) {
   return prm;
 }
 
-static void set_head(dsx_handle* h, HpParams& prm, int flags, float* x, dsx_strides xs, float* eps, const float* noise,
-                     uint64_t seed, uint64_t offset, DdpmCoef c, int next_row0, int row_per_b, const PlmsFuse* plms) {
-  prm.head_flags = flags;
-  prm.x = x;
-  prm.xs = xs;
-  prm.eps = eps;
-  prm.noise = noise;
-  prm.seed = seed;
-  prm.offset = offset;
+static void set_head(dsx_handle* h, HpParams& prm, const HeadArgs& a) {
+  prm.head_flags = a.flags;
+  prm.x = a.x;
+  prm.xs = a.xs;
+  prm.eps = a.eps;
+  prm.noise = a.noise;
+  prm.seed = a.seed;
+  prm.offset = a.offset;
   prm.b_off = h->batch_offset;
-  prm.c = c;
-  if (plms) prm.pl = *plms;
-  prm.d0 = h->ws.DTAB + static_cast<size_t>(next_row0) * h->m.L * kC;
-  prm.d0_row_stride = row_per_b * h->m.L * kC;
+  prm.c = a.c;
+  if (a.plms) prm.pl = *a.plms;
+  prm.d0 = h->ws.DTAB + static_cast<size_t>(a.next_row0) * h->m.L * kC;
+  prm.d0_row_stride = a.row_per_b * h->m.L * kC;
 }
 
 template <int NWG, int R>
@@ -1109,25 +1108,6 @@ static int launch_step(dsx_handle* h, const HpParams& prm, int rows, cudaStream_
 
 static int gate_mode(const dsx_handle* h, int P) { return h->gate_approx >= 0 ? h->gate_approx : (P == 3 ? 0 : 1); }
 
-// Layers [l0, l1) of one evaluation with the hi / lo weight planes: one launch (stack mode) or one launch per layer.
-int launch_tc_layers(dsx_handle* h, int l0, int l1, const Geom& g, int row0, int row_per_b, cudaStream_t s) {
-  HpParams prm = base_params(h, g, 128);
-  prm.w = h->m.wpack;
-  prm.P = (h->precision == DSX_PREC_FP16S) ? 2 : h->precision;   // DSX_PREC_FP16 = 1, FP16X2 = 2, FP16X3 = 3 == MMA passes
-  prm.fast_gate = gate_mode(h, prm.P);
-  prm.dtab = h->ws.DTAB + static_cast<size_t>(row0) * h->m.L * kC;
-  prm.d_row_stride = row_per_b * h->m.L * kC;
-  if (h->stack_mode && l1 - l0 > 1) {
-    prm.l0 = l0; prm.l1 = l1;
-    return launch_step(h, prm, 128, s);
-  }
-  for (int l = l0; l < l1; ++l) {
-    prm.l0 = l; prm.l1 = l + 1;
-    DSX_TRY(launch_step(h, prm, 128, s));
-  }
-  return DSX_OK;
-}
-
 // CP for the conditioner currently packed in ws.CONDH (called once per API call, after launch_pack_cond).
 int launch_tc_condproj(dsx_handle* h, const Geom& g, cudaStream_t s) {
   if (!h->attr_cond) {
@@ -1142,14 +1122,6 @@ int launch_tc_condproj(dsx_handle* h, const Geom& g, cudaStream_t s) {
   return DSX_OK;
 }
 
-int launch_tc_head(dsx_handle* h, const Geom& g, int flags, float* x_state, dsx_strides xs, float* eps_out,
-                   const float* noise, uint64_t seed, uint64_t offset, DdpmCoef c, int next_row0, int row_per_b,
-                   cudaStream_t s, const PlmsFuse* plms) {
-  HpParams prm = base_params(h, g, 128);
-  set_head(h, prm, flags, x_state, xs, eps_out, noise, seed, offset, c, next_row0, row_per_b, plms);
-  return launch_step(h, prm, 128, s);
-}
-
 // Frames per CTA for this call: 64 (one warpgroup per CTA, twice the CTAs) whenever the whole batch then has a CTA per
 // tile at once, i.e. for small batches that would otherwise leave most SMs idle; 128 otherwise.
 static int stack_rows(dsx_handle* h, const Geom& g) {
@@ -1158,36 +1130,49 @@ static int stack_rows(dsx_handle* h, const Geom& g) {
   return (cap64 > 0 && g.frames_padded() / 64 <= static_cast<size_t>(cap64)) ? 64 : 128;
 }
 
-// Does the one-launch-per-step form take this call?  (precisions with a single weight plane per pass set)
-bool tc_stack_usable(dsx_handle* h, const Geom&) {
-  if (h->stack_kernel == 0 || !h->stack_mode) return false;
-  return h->precision == DSX_PREC_FP16 || h->precision == DSX_PREC_FP16X2 || h->precision == DSX_PREC_FP16S;
+// The stack form: every layer of an evaluation in one launch at stack_rows, one weight plane per MMA pass (fp16s: the
+// stochastically rounded set of the table row).  It takes FP16 / FP16X2 / FP16S under DSX_OPT_STACK_KERNEL and
+// DSX_OPT_STACK_MODE; every other layer launch uses the hi / lo planes at 128 rows.
+static bool stack_form(const dsx_handle* h) {
+  return h->stack_kernel && h->stack_mode &&
+         (h->precision == DSX_PREC_FP16 || h->precision == DSX_PREC_FP16X2 || h->precision == DSX_PREC_FP16S);
 }
 
-// Layers [0, nl) of one evaluation (table row row0, weight set `wset` in fp16s), optionally followed by the head, in one
-// launch.
-int launch_tc_stack(dsx_handle* h, int nl, const Geom& g, int row0, int row_per_b, int wset, cudaStream_t s, const HeadArgs* head) {
+bool tc_fuse_head(const dsx_handle* h) { return stack_form(h) && h->fused_head && h->profile != 2; }
+
+int launch_tc_step(dsx_handle* h, const Geom& g, int l0, int l1, int row0, int row_per_b, const HeadArgs* head,
+                   cudaStream_t s) {
   const ModelDev& m = h->m;
-  if (nl <= 0) return DSX_OK;
-  const int rows = stack_rows(h, g);
-  h->stack_rows_used = rows;
+  const bool layers = l1 > l0, stack = layers && stack_form(h);
+  if (!layers && !head) return DSX_OK;
+  DSX_CHECK(!layers || !head || (stack && l0 == 0 && l1 == m.L), DSX_E_INVALID,
+            "the head shares a launch only with all layers in the stack form");
+  const int rows = stack ? stack_rows(h, g) : 128;
   HpParams prm = base_params(h, g, rows);
-  const bool sr = (h->precision == DSX_PREC_FP16S);
-  prm.w_sr = sr ? 1 : 0;
-  prm.w = sr ? m.wsr + static_cast<size_t>(wset % std::max(1, m.wsr_sets)) * m.L * kSrRowsPerLayer * 64 : m.wpack;
-  prm.P = (h->precision == DSX_PREC_FP16X2) ? 2 : 1;
+  if (head) set_head(h, prm, *head);
+  if (!layers) return launch_step(h, prm, rows, s);
+  if (stack) {
+    const bool sr = (h->precision == DSX_PREC_FP16S);
+    prm.w_sr = sr ? 1 : 0;
+    prm.w = sr ? m.wsr + static_cast<size_t>(row0 % std::max(1, m.wsr_sets)) * m.L * kSrRowsPerLayer * 64 : m.wpack;
+    prm.P = (h->precision == DSX_PREC_FP16X2) ? 2 : 1;
+  } else {
+    prm.w = m.wpack;
+    prm.P = (h->precision == DSX_PREC_FP16S) ? 2 : h->precision;   // DSX_PREC_FP16 = 1, FP16X2 = 2, FP16X3 = 3 == MMA passes
+  }
   prm.fast_gate = gate_mode(h, prm.P);
   prm.dtab = h->ws.DTAB + static_cast<size_t>(row0) * m.L * kC;
   prm.d_row_stride = row_per_b * m.L * kC;
-  prm.l0 = 0;
-  prm.l1 = nl;
-  if (head && head->flags) {
-    DSX_CHECK(nl == m.L, DSX_E_INVALID, "the fused head needs the whole stack");
-    set_head(h, prm, head->flags | TC_HEAD, head->x, head->xs, head->eps, head->noise, head->seed, head->offset, head->c,
-             head->next_row0, head->row_per_b, head->plms);
+  const int per_launch = h->stack_mode ? l1 - l0 : 1;   // DSX_OPT_STACK_MODE = 0: one launch per layer
+  for (int l = l0; l < l1; l += per_launch) {
+    prm.l0 = l;
+    prm.l1 = l + per_launch;
+    DSX_TRY(launch_step(h, prm, rows, s));
   }
-  DSX_TRY(launch_step(h, prm, rows, s));
-  h->stack_launches++;
+  if (stack) {
+    h->stack_launches++;
+    h->stack_rows_used = rows;
+  }
   return DSX_OK;
 }
 

@@ -204,7 +204,6 @@ struct dsx_handle {
   bool loaded = false;
   int precision = DSX_PREC_FP32_SIMT;
   int tc_group = 0;             // 2 when the tensor-core path (sm_90 wgmma kernels) is available on the device, else 0
-  int use_graph = 0;
   int layer_limit = -1;
   int64_t launches = 0;
   int64_t stack_launches = 0;   // one-launch-per-step launches of k_hp_step (layers + fused head)
@@ -266,7 +265,6 @@ int launch_epilogue(dsx_handle* h, const float* x, const int64_t* mel2ph, const 
 // ---- dsx_hopper.cu -----------------------------------------------------------------------
 int tc_pack_model(dsx_handle* h, cudaStream_t s);
 int launch_tc_condproj(dsx_handle* h, const Geom& g, cudaStream_t s);
-int launch_tc_layers(dsx_handle* h, int l0, int l1, const Geom& g, int row0, int row_per_b, cudaStream_t s);
 // Head / tail of DiffNet on tensor cores.  flags: 1 = head (skip -> eps), 2 = write eps, 4 = DDPM update of x,
 // 8 = input projection of x (after the update if any) for the evaluation that uses table row (next_row0, row_per_b).
 enum { TC_HEAD = 1, TC_WRITE_EPS = 2, TC_UPDATE = 4, TC_INPROJ = 8, TC_PLMS = 16 };
@@ -280,13 +278,9 @@ struct PlmsFuse {
   float* eps_store;  // this evaluation's eps -> history ring slot (or null)
   float* x_out;      // result; null: in place
 };
-int launch_tc_head(dsx_handle* h, const Geom& g, int flags, float* x_state, dsx_strides xs, float* eps_out,
-                   const float* noise, uint64_t seed, uint64_t offset, DdpmCoef c, int next_row0, int row_per_b,
-                   cudaStream_t s, const PlmsFuse* plms = nullptr);
 bool tc_supported(const dsx_handle* h);
 
-bool tc_stack_usable(dsx_handle* h, const Geom& g);
-// What follows the residual stack inside a diffusion step (launch_tc_head's job), optionally fused into the layers' launch
+// What follows the residual stack of an evaluation: eps, a sampler update and the next evaluation's input projection
 struct HeadArgs {
   int flags = 0;            // TC_* (0: no head)
   float* x = nullptr;       // mel state
@@ -298,8 +292,13 @@ struct HeadArgs {
   int next_row0 = 0, row_per_b = 0;   // FiLM table row of the NEXT evaluation (TC_INPROJ)
   const PlmsFuse* plms = nullptr;
 };
-int launch_tc_stack(dsx_handle* h, int nl, const Geom& g, int row0, int row_per_b, int wset, cudaStream_t s,
-                    const HeadArgs* head = nullptr);
+// Whether the head of an evaluation of all layers runs inside the layers' launch: the stack form with DSX_OPT_FUSED_HEAD,
+// except under DSX_OPT_PROFILE = 2, which times the head as a launch of its own.
+bool tc_fuse_head(const dsx_handle* h);
+// k_hp_step for layers [l0, l1) of the evaluation at FiLM table row (row0, row_per_b), followed in the same launch by
+// `head` (only with all layers where tc_fuse_head allows it); with no layers, `head` alone at 128 rows.
+int launch_tc_step(dsx_handle* h, const Geom& g, int l0, int l1, int row0, int row_per_b, const HeadArgs* head,
+                   cudaStream_t s);
 
 int dev_alloc(dsx_handle* h, void** p, size_t bytes, bool model_owned);
 int ensure_workspace(dsx_handle* h, const Geom& g, int rows, cudaStream_t s);

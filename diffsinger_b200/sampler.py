@@ -144,8 +144,6 @@ class DsxSampler:
     def set_option(self, what, value):
         check(lib.dsx_set_option(self._handle(self._device or torch.device("cuda", torch.cuda.current_device())),
                                  what, value), "dsx_set_option")
-        if what == _capi.OPT_TC_CTA_GROUP:
-            pass
 
     def info(self, what):
         out = ctypes.c_int64()

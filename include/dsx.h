@@ -197,8 +197,9 @@ enum {
   DSX_OPT_TC_CTA_GROUP = 0, /* accepts 2 only; kept for ABI compatibility, no effect */
   DSX_OPT_CP_PREFETCH = 1,  /* accepted and ignored (kept for ABI compatibility): the step kernel always prefetches the
                                epilogue operands (conditioner projection, x, skip) into L2 */
-  DSX_OPT_PROFILE = 2,      /* 1: bracket the residual-layer kernel(s) of every evaluation with CUDA events; 2: bracket the
-                               head / update kernel of every DDPM step instead; 0: off.  Setting it resets the sums */
+  DSX_OPT_PROFILE = 2,      /* 1: bracket the residual-layer kernel(s) of every evaluation with CUDA events; 2: run the
+                               tensor-core head of every evaluation (DDPM, PLMS, dsx_diffnet_forward) as a launch of its own
+                               and bracket that instead; 0: off.  Setting it resets the sums */
   DSX_OPT_STACK_MODE = 3,   /* 1 (default): all residual layers of an evaluation in ONE persistent cooperative launch (a tile
                                starts a layer when its neighbour tiles have finished the one before); 0: one launch per
                                layer */
