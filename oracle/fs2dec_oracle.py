@@ -51,7 +51,7 @@ def decoder(sd, x, hp, table=None):
     pad = padding_mask(x)
     nonpad_TB = 1 - pad.transpose(0, 1).to(x.dtype)[:, :, None]   # .float() in the reference; x.dtype keeps .half() fp16
     if table is None or table.shape[0] < 1 + T:                    # common_layers.py:127-135
-        table = sinusoidal_table(max(2000, 1 + T), H)
+        table = sinusoidal_table(max(2000, 1 + T), H, dtype=torch.float64 if x.dtype == torch.float64 else torch.float)
     table = table.to(x)
     pos = make_positions(x[..., 0])
     x = x + sd["pos_embed_alpha"] * table.index_select(0, pos.view(-1)).view(B, T, -1)

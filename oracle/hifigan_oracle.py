@@ -31,22 +31,32 @@ def get_padding(kernel_size, dilation=1):                      # hifigan.py:26-2
     return int((kernel_size * dilation - dilation) / 2)
 
 
-def resblock1(sd, pre, x, k, dil):
+def _round(fp16):
+    """fp16=True: a conv operand as the dsx kernels read it, rounded to fp16 (and back to the tensor's own dtype)"""
+    return (lambda t: t.half().to(t.dtype)) if fp16 else (lambda t: t)
+
+
+def resblock1(sd, pre, x, k, dil, fp16=False):
     """ResBlock1.forward, hifigan.py:54-62 (note `x = xt + x` is executed once per pair in the reference)."""
+    r = _round(fp16)
     for j, d in enumerate(dil):
         xt = F.leaky_relu(x, LRELU_SLOPE)
-        xt = F.conv1d(xt, conv_weight(sd, f"{pre}.convs1.{j}"), sd[f"{pre}.convs1.{j}.bias"], dilation=d, padding=get_padding(k, d))
+        xt = F.conv1d(r(xt), r(conv_weight(sd, f"{pre}.convs1.{j}")), sd[f"{pre}.convs1.{j}.bias"], dilation=d,
+                      padding=get_padding(k, d))
         xt = F.leaky_relu(xt, LRELU_SLOPE)
-        xt = F.conv1d(xt, conv_weight(sd, f"{pre}.convs2.{j}"), sd[f"{pre}.convs2.{j}.bias"], dilation=1, padding=get_padding(k, 1))
+        xt = F.conv1d(r(xt), r(conv_weight(sd, f"{pre}.convs2.{j}")), sd[f"{pre}.convs2.{j}.bias"], dilation=1,
+                      padding=get_padding(k, 1))
         x = xt + x
     return x
 
 
-def resblock2(sd, pre, x, k, dil):
+def resblock2(sd, pre, x, k, dil, fp16=False):
     """ResBlock2.forward, hifigan.py:85-90."""
+    r = _round(fp16)
     for j, d in enumerate(dil):
         xt = F.leaky_relu(x, LRELU_SLOPE)
-        xt = F.conv1d(xt, conv_weight(sd, f"{pre}.convs.{j}"), sd[f"{pre}.convs.{j}.bias"], dilation=d, padding=get_padding(k, d))
+        xt = F.conv1d(r(xt), r(conv_weight(sd, f"{pre}.convs.{j}")), sd[f"{pre}.convs.{j}.bias"], dilation=d,
+                      padding=get_padding(k, d))
         x = xt + x
     return x
 
@@ -85,8 +95,11 @@ def nsf_source(sd, f0_up, rate, harmonic_num=8, sine_amp=0.1):
     return sine_merge, noise, uv
 
 
-def generator(sd, h, mel, f0=None):
-    """HifiGanGenerator.forward (hifigan.py:149-171): mel [B, 80, T] (+ f0 [B, T] in Hz, 0 = unvoiced) -> wav [B, 1, T * prod(rates)]."""
+def generator(sd, h, mel, f0=None, fp16=False):
+    """HifiGanGenerator.forward (hifigan.py:149-171): mel [B, 80, T] (+ f0 [B, T] in Hz, 0 = unvoiced) -> wav [B, 1, T * prod(rates)].
+    fp16=True: the input and weight of conv_pre, of every ups and of every ResBlock conv rounded to fp16, as the dsx
+    kernels round them; the NSF source, the noise convs, conv_post and every sum stay in the input's dtype."""
+    r = _round(fp16)
     rates, ksz = h["upsample_rates"], h["upsample_kernel_sizes"]
     nk = len(h["resblock_kernel_sizes"])
     block = resblock1 if h["resblock"] == "1" else resblock2
@@ -96,10 +109,10 @@ def generator(sd, h, mel, f0=None):
         f0_up = F.interpolate(f0[:, None], scale_factor=float(up), mode="nearest").transpose(1, 2)     # torch.nn.Upsample, :115,152
         har, _, _ = nsf_source(sd, f0_up, h["audio_sample_rate"])
         har = har.transpose(1, 2)
-    x = F.conv1d(mel, conv_weight(sd, "conv_pre"), sd["conv_pre.bias"], padding=3)
+    x = F.conv1d(r(mel), r(conv_weight(sd, "conv_pre")), sd["conv_pre.bias"], padding=3)
     for i, (u, k) in enumerate(zip(rates, ksz)):
         x = F.leaky_relu(x, LRELU_SLOPE)
-        x = F.conv_transpose1d(x, conv_weight(sd, f"ups.{i}"), sd[f"ups.{i}.bias"], stride=u, padding=(k - u) // 2)
+        x = F.conv_transpose1d(r(x), r(conv_weight(sd, f"ups.{i}")), sd[f"ups.{i}.bias"], stride=u, padding=(k - u) // 2)
         if har is not None:
             if i + 1 < len(rates):
                 s = int(np.prod(rates[i + 1:]))
@@ -108,8 +121,8 @@ def generator(sd, h, mel, f0=None):
                 x = x + F.conv1d(har, sd[f"noise_convs.{i}.weight"], sd[f"noise_convs.{i}.bias"])
         xs = None
         for j, (rk, rd) in enumerate(zip(h["resblock_kernel_sizes"], h["resblock_dilation_sizes"])):
-            r = block(sd, f"resblocks.{i * nk + j}", x, rk, rd)
-            xs = r if xs is None else xs + r
+            y = block(sd, f"resblocks.{i * nk + j}", x, rk, rd, fp16)
+            xs = y if xs is None else xs + y
         x = xs / nk
     x = F.leaky_relu(x)                                   # (default slope 0.01, as the reference: hifigan.py:167)
     x = F.conv1d(x, conv_weight(sd, "conv_post"), sd["conv_post.bias"], padding=3)

@@ -1,7 +1,8 @@
 """GPU: the pitch extractor of libdsx.so against the reference's output (tests/golden/pitch_extractor.npz) and the CPU
 oracle (oracle/pe_oracle.py).
 
-The kernels run every conv and linear with fp16 operands and fp32 accumulation.  A CPU simulation of that rounding on
+The kernels run every conv and linear with fp16 operands and fp32 accumulation.  A CPU simulation of that rounding
+(pe_oracle.pitch_extractor(fp16=True); the norms, the position term and the Linear(P, 2) head stay fp32) on
 the committed fixture (H = 32, B = 2, T = 48) gives, against fp32, max 5.5e-3 / mean 1.3e-3 on channel 0 (log2 Hz) and
 max 3.5e-3 / mean 1.0e-3 on channel 1 (uv logit), with no uv flips; the reference's smallest |uv logit| there is 4.7e-3.
 At H = 256, B = 4, T = 400 the same simulation gave max 5.2e-3 / 4.4e-3 and mean 1.0e-3 / 9.6e-4.  The bounds below are

@@ -55,3 +55,31 @@ def test_oracle_is_bit_exact_against_the_live_reference():
         b = H.generator(sd, h, mel, f0)
     assert b.shape == g["wav_nsf"].shape
     assert np.abs(b.numpy() - g["wav_nsf"]).max() <= 1e-6 * np.abs(g["wav_nsf"]).max()
+
+
+def test_fp16_option_leaves_the_fp32_path_bit_identical():
+    g, sd, h, mel, f0 = _case()
+    with torch.no_grad():
+        torch.manual_seed(int(g["rng_seed"]))
+        a = H.generator(sd, h, mel, f0)
+        torch.manual_seed(int(g["rng_seed"]))
+        b = H.generator(sd, h, mel, f0, fp16=False)
+    assert torch.equal(a, b)
+
+
+def test_fp16_simulation_is_within_the_quoted_error():
+    """generator(fp16=True) on the fixtures: within the max 9e-5 / mean 2e-5 (on a 0.1 signal) that
+    test_gpu_hifigan.py quotes for the kernels' fp16 operands, and not bit-identical to fp32 (it does round)"""
+    for name, peak in (("hifigan_nsf.npz", 0.1), ("hifigan_nsf_b1t9.npz", None)):
+        g, sd, h, mel, f0 = _case(name)
+        with torch.no_grad():
+            torch.manual_seed(int(g["rng_seed"]))
+            wav = H.generator(sd, h, mel, f0, fp16=True).numpy()
+            outs = [(wav, g["wav_nsf"])]
+            if "wav_plain" in g.files:
+                outs.append((H.generator(sd, h, mel, fp16=True).numpy(), g["wav_plain"]))
+        for out, ref in outs:
+            scale = (peak or np.abs(ref).max()) / 0.1
+            d = np.abs(out - ref)
+            assert d.max() <= 9e-5 * scale and d.mean() <= 2e-5 * scale, (name, d.max(), d.mean())
+            assert d.max() > 0
