@@ -28,7 +28,8 @@
 // per layer instead of six times.  fp16x3 (R = 2) reads y's lo plane too and keeps streaming its taps.
 // Each warpgroup's rows go through the same instruction sequence whatever NWG is, so 64- and 128-frame CTAs give
 // bit-identical results.  While GEMM1 runs, the warpgroup prefetches the CP, x and skip rows its epilogues read into L2,
-// and the epilogues issue their global loads in batches ahead of their stores.
+// and the epilogues issue their global loads in batches ahead of their stores: every operand of a batch, including the
+// residual and skip epilogues' bias and FiLM pairs, is loaded before the batch's first store.
 //
 // Precision (MMA passes P per k-block): P = 1 fp16 operands; P = 2 adds a W_lo pass (weights as hi+lo fp16 pairs);
 // P = 3 accumulates A_hi*W_hi + A_hi*W_lo + A_lo*W_hi (~2^-22 relative).  The conditioner projection is always 3-pass.
@@ -609,11 +610,15 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem
     __half* yo = Yout + tb;
     __half* so = p.S16 + tb;
     const bool read_old = q == 0 || l > 0;
+    const bool read_d = q == 0 && !last;
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
 #pragma unroll
       for (int e0 = 0; e0 < 64; e0 += 2 * kEpiBatch) {
-        float2 old[kEpiBatch];
+        // the batch's x or skip pairs, and the bias and FiLM pairs of its kEpiBatch / 2 columns (shared by rows row0 and
+        // row0 + 8), all ahead of the stores: loaded in the element loop, each bias or FiLM pair would be a round trip
+        // that the element's stores wait for
+        float2 old[kEpiBatch], bbv[kEpiBatch / 2], dvv[kEpiBatch / 2];
 #pragma unroll
         for (int j = 0; j < kEpiBatch; ++j) {
           const int e = e0 + 2 * j, o = ((e & 2) ? 8 * kC : 0) + hh * 128 + (e >> 2) * 8;
@@ -621,18 +626,25 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem
           if (read_old && ((e & 2) ? ok8 : ok0)) old[j] = *reinterpret_cast<const float2*>(src + o);
         }
 #pragma unroll
+        for (int i = 0; i < kEpiBatch / 2; ++i) {
+          const int c = hh * 128 + ((e0 >> 2) + i) * 8;
+          bbv[i] = __ldg(reinterpret_cast<const float2*>(bias + c));
+          dvv[i] = make_float2(0.f, 0.f);
+          if (read_d) dvv[i] = __ldg(reinterpret_cast<const float2*>(dn + c));
+        }
+#pragma unroll
         for (int j = 0; j < kEpiBatch; ++j) {
           const int e = e0 + 2 * j, c = hh * 128 + (e >> 2) * 8, o = ((e & 2) ? 8 * kC : 0) + c;
           if (!((e & 2) ? ok8 : ok0)) continue;
           const float a0 = hh ? c1[e] : c0[e], a1 = hh ? c1[e + 1] : c0[e + 1];
-          const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + c));
+          const float2 bb = bbv[j >> 1];
           if (q == 0) {
             float2 xv = old[j];
             xv.x = (xv.x + (a0 + bb.x)) * 0.70710678118654752440f;
             xv.y = (xv.y + (a1 + bb.y)) * 0.70710678118654752440f;
             *reinterpret_cast<float2*>(dst + o) = xv;
             if (!last) {
-              const float2 dv = __ldg(reinterpret_cast<const float2*>(dn + c));
+              const float2 dv = dvv[j >> 1];
               const float ya = xv.x + dv.x, yb = xv.y + dv.y;
               const __half2 hy = __floats2half2_rn(ya, yb);
               *reinterpret_cast<__half2*>(yo + o) = hy;
