@@ -22,84 +22,47 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-int dev_alloc(dsx_handle* h, void** p, size_t bytes, bool model_owned) {
-  void* q = nullptr;
-  cudaError_t e = cudaMalloc(&q, bytes ? bytes : 1);
-  if (e != cudaSuccess) {
-    set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
-    return e == cudaErrorMemoryAllocation ? DSX_E_NOMEM : DSX_E_CUDA;
-  }
-  if (model_owned) h->owned.push_back(q);
-  *p = q;
-  return DSX_OK;
-}
-
-static void free_ws(Workspace& w) {
-  void* ptrs[] = {w.X, w.SKIP, w.CONDF, w.G1, w.Zf, w.Y, w.CONDH, w.CP, w.S16, w.FLAGS, w.DTAB, w.EMB, w.TVALS, w.EPS, w.XTMP, w.XSTATE};
-  for (void* p : ptrs)
-    if (p) cudaFree(p);
-  w = Workspace();
-}
-
-// Grow-only workspace: every buffer keeps its byte capacity; a call with a new (B, T) that fits re-uses the allocations
-// (only the geometry changes), so utterance lengths that change from call to call cost no
-// cudaFree / cudaMalloc (cudaFree synchronises the device).  New allocations are zeroed on the caller's stream.
+// Grow-only workspace: a call with a new (B, T) that fits re-uses the allocations (only the geometry changes), so
+// utterance lengths that change from call to call cost no cudaFree / cudaMalloc.  New allocations are zeroed on the
+// caller's stream: padding frames, SKIP and FLAGS depend on it.
 int ensure_workspace(dsx_handle* h, const Geom& g, int rows, cudaStream_t s) {
   Workspace& w = h->ws;
   const ModelDev& m = h->m;
   const bool tc = h->precision != DSX_PREC_FP32_SIMT;
   const size_t nf = g.frames_padded();
-  bool moved = false;
-  auto need = [&](void** p, size_t& cap, size_t bytes) -> int {
-    if (cap >= bytes && *p) return DSX_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    w.bytes -= cap;
-    cap = 0;
-    const size_t grow = bytes + bytes / 8;      // headroom: slightly longer utterances next time do not reallocate
-    DSX_TRY(dev_alloc(h, p, grow, false));
-    DSX_CUDA(cudaMemsetAsync(*p, 0, grow, s));
-    cap = grow;
-    w.bytes += grow;
-    moved = true;
-    return DSX_OK;
-  };
-#define NEED(field, bytes) DSX_TRY(need(reinterpret_cast<void**>(&w.field), w.cap_##field, (bytes)))
   if (!h->fft) {   // the FFT denoiser keeps its own per-evaluation buffers (fft_workspace)
-    NEED(X, nf * m.C * 4);
-    NEED(SKIP, nf * m.C * 4);
+    DSX_TRY(w.X.reserve_zeroed(nf * m.C * 4, s));
+    DSX_TRY(w.SKIP.reserve_zeroed(nf * m.C * 4, s));
     if (tc) {
       const void* cond_before[2] = {w.CONDH, w.CP};
-      NEED(Y, nf * m.C * 2 * 4);
-      NEED(CONDH, nf * m.H * 2 * 2);
-      NEED(S16, nf * m.C * 2 * 2);
-      NEED(FLAGS, nf / 64 * 2 * sizeof(unsigned));   // two per tile at the smallest tile height, 64 frames
-      NEED(CP, static_cast<size_t>(m.L) * nf * 2 * m.C * 4);
+      DSX_TRY(w.Y.reserve_zeroed(nf * m.C * 2 * 4, s));
+      DSX_TRY(w.CONDH.reserve_zeroed(nf * m.H * 2 * 2, s));
+      DSX_TRY(w.S16.reserve_zeroed(nf * m.C * 2 * 2, s));
+      DSX_TRY(w.FLAGS.reserve_zeroed(nf / 64 * 2 * sizeof(unsigned), s));   // two per tile at the smallest tile height, 64 frames
+      DSX_TRY(w.CP.reserve_zeroed(static_cast<size_t>(m.L) * nf * 2 * m.C * 4, s));
       if (cond_before[0] != w.CONDH || cond_before[1] != w.CP) h->cond_ready = false;
     } else {
       const void* cond_before = w.CONDF;
-      NEED(G1, nf * 2 * m.C * 4);
-      NEED(Zf, nf * m.C * 4);
-      NEED(CONDF, nf * m.H * 4);
+      DSX_TRY(w.G1.reserve_zeroed(nf * 2 * m.C * 4, s));
+      DSX_TRY(w.Zf.reserve_zeroed(nf * m.C * 4, s));
+      DSX_TRY(w.CONDF.reserve_zeroed(nf * m.H * 4, s));
       if (cond_before != w.CONDF) h->cond_ready = false;
     }
   }
   if (w.rows_cap < rows) {
     const int keep_rows = std::max(rows, w.rows_cap + w.rows_cap / 2);
     if (!h->fft) {
-      NEED(DTAB, static_cast<size_t>(keep_rows) * m.L * m.C * 4);
-      NEED(EMB, static_cast<size_t>(keep_rows) * m.C * 4);
+      DSX_TRY(w.DTAB.reserve_zeroed(static_cast<size_t>(keep_rows) * m.L * m.C * 4, s));
+      DSX_TRY(w.EMB.reserve_zeroed(static_cast<size_t>(keep_rows) * m.C * 4, s));
     }
-    NEED(TVALS, static_cast<size_t>(keep_rows) * 8);
+    DSX_TRY(w.TVALS.reserve_zeroed(static_cast<size_t>(keep_rows) * 8, s));
     w.rows_cap = keep_rows;
   }
   if (h->fft) DSX_TRY(fft_workspace(h, g, w.rows_cap, s));
   const size_t mel = static_cast<size_t>(g.B) * m.M * g.T;
-  NEED(EPS, 5 * mel * 4);
-  NEED(XTMP, mel * 4);
-  NEED(XSTATE, mel * 4);
-#undef NEED
-  if (moved) h->ws_epoch++;
+  DSX_TRY(w.EPS.reserve_zeroed(5 * mel * 4, s));
+  DSX_TRY(w.XTMP.reserve_zeroed(mel * 4, s));
+  DSX_TRY(w.XSTATE.reserve_zeroed(mel * 4, s));
   w.g = g;
   return DSX_OK;
 }
@@ -183,7 +146,7 @@ static int evaluate(dsx_handle* h, const Geom& g, const float* x_in, int row0, i
   return launch_plms_update(h, x_out, ha.x, p->h1, eps, nullptr, nullptr, p->c, mel, s);
 }
 
-// Workspace + tensor maps for (B, T) and, when `cond` is given, the conditioner pack and its hoisted projection (the
+// Workspace for (B, T) and, when `cond` is given, the conditioner pack and its hoisted projection (the
 // step-independent part of every residual layer).  cond == NULL re-uses what the last call with a conditioner left behind
 // (dsx_set_cond or any entry point): callers that drive the sampling loop themselves, one p_sample / DiffNet.forward per
 // call, pay the pack + projection once per utterance batch instead of once per step.
@@ -336,16 +299,8 @@ const char* dsx_last_error(void) { return g_err; }
 
 int dsx_create(int device, dsx_handle** out) {
   DSX_CHECK(out, DSX_E_INVALID, "out is NULL");
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) {
-    set_error("no CUDA device available (%s); dsx has no CPU fallback", cudaGetErrorString(e));
-    return DSX_E_CUDA;
-  }
-  DSX_CHECK(device >= 0 && device < ndev, DSX_E_INVALID, "device %d out of range (%d devices)", device, ndev);
-  DSX_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
-  DSX_CUDA(cudaGetDeviceProperties(&prop, device));
+  DSX_TRY(select_device(device, &prop));
   dsx_handle* h = new dsx_handle();
   h->device = device;
   h->sm_count = prop.multiProcessorCount;
@@ -364,8 +319,7 @@ int dsx_create(int device, dsx_handle** out) {
 }
 
 static void free_model(dsx_handle* h) {
-  for (void* p : h->owned) cudaFree(p);
-  h->owned.clear();
+  h->mem.free_all();
   h->loaded = false;
 }
 
@@ -374,11 +328,10 @@ void dsx_destroy(dsx_handle* h) {
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();
   free_model(h);
-  free_ws(h->ws);
+  h->ws.release();
   fft_destroy(h->fft);
   for (cudaEvent_t e : h->prof_events) cudaEventDestroy(e);
-  for (void* p : h->stage)
-    if (p) cudaFree(p);
+  for (GrowBuffer& b : h->stage) b.release();
   if (h->status_dev) cudaFree(h->status_dev);
   if (h->status_host) cudaFreeHost(h->status_host);
   if (h->trace_dev) cudaFree(h->trace_dev);
@@ -396,10 +349,9 @@ int dsx_load_diffnet(dsx_handle* h, const dsx_diffnet_params* p, int M, int C, i
   DSX_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   free_model(h);
-  free_ws(h->ws);
+  h->ws.release();
   fft_destroy(h->fft);
   h->fft = nullptr;
-  h->ws_epoch++;
   h->cond_ready = false;
   memset(&h->m, 0, sizeof(h->m));
   h->m.M = M; h->m.C = C; h->m.H = H; h->m.L = L; h->m.cycle = dilation_cycle;
@@ -424,10 +376,9 @@ int dsx_load_fft(dsx_handle* h, const dsx_fft_config* cfg, const dsx_fft_params*
   FftDenoiser* f = nullptr;
   DSX_TRY(fft_create(h->device, cfg, p, s, &f));   // validates and packs before the old denoiser is let go
   free_model(h);
-  free_ws(h->ws);
+  h->ws.release();
   fft_destroy(h->fft);
   h->fft = f;
-  h->ws_epoch++;
   h->cond_ready = false;
   memset(&h->m, 0, sizeof(h->m));
   h->m.M = cfg->mel_bins;
@@ -565,22 +516,15 @@ int dsx_infer_host(dsx_handle* h, const float* cond_host, dsx_strides cs, const 
             DSX_E_INVALID, "dsx_infer_host: cond_host must be a dense permutation of a contiguous [B,H,T] block (strides %lld %lld %lld)",
             static_cast<long long>(cs.b), static_cast<long long>(cs.c), static_cast<long long>(cs.t));
   int rc = DSX_OK;
-  auto up = [&](int slot, const void* src, size_t bytes) -> void* {
-    if (rc != DSX_OK || !src) return nullptr;
-    if (h->stage_cap[slot] < bytes) {
-      if (h->stage[slot]) cudaFree(h->stage[slot]);
-      h->stage[slot] = nullptr;
-      h->stage_cap[slot] = 0;
-      rc = dev_alloc(h, &h->stage[slot], bytes, false);
-      if (rc != DSX_OK) return nullptr;
-      h->stage_cap[slot] = bytes;
-    }
-    if (src != reinterpret_cast<const void*>(1) &&
-        cudaMemcpyAsync(h->stage[slot], src, bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+  auto up = [&](int slot, const void* src, size_t bytes, bool copy = true) -> void* {
+    if (rc != DSX_OK || (copy && !src)) return nullptr;
+    GrowBuffer& b = h->stage[slot];
+    rc = b.reserve(bytes, s);
+    if (rc == DSX_OK && copy && cudaMemcpyAsync(b.ptr, src, bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) {
       set_error("host->device copy failed");
       rc = DSX_E_CUDA;
     }
-    return h->stage[slot];
+    return b.ptr;
   };
   float* d_cond = static_cast<float*>(up(0, cond_host, cond_elems * 4));
   float* d_fs2 = static_cast<float*>(up(1, fs2_mel_host, mel * 4));
@@ -588,7 +532,7 @@ int dsx_infer_host(dsx_handle* h, const float* cond_host, dsx_strides cs, const 
   float* d_min = static_cast<float*>(up(3, spec_min_host, M * 4));
   float* d_max = static_cast<float*>(up(4, spec_max_host, M * 4));
   int64_t* d_m2p = static_cast<int64_t*>(up(5, mel2ph_host, static_cast<size_t>(B) * T * 8));
-  float* d_out = static_cast<float*>(up(6, reinterpret_cast<const void*>(1), mel * 4));   // output buffer only
+  float* d_out = static_cast<float*>(up(6, nullptr, mel * 4, false));   // output buffer: no upload
   if (rc == DSX_OK)
     rc = dsx_infer(h, d_cond, cs, d_fs2, nullptr, d_x, nullptr, seed, d_m2p, d_min, d_max, B, T, K_step, pndm_interval,
                    d_out, stream);
@@ -605,7 +549,7 @@ int dsx_get_info(dsx_handle* h, int what, int64_t* out) {
   switch (what) {
     case DSX_INFO_PRECISION: *out = h->precision; break;
     case DSX_INFO_KERNEL_LAUNCHES: *out = h->launches; break;
-    case DSX_INFO_WORKSPACE_BYTES: *out = static_cast<int64_t>(h->ws.bytes); break;
+    case DSX_INFO_WORKSPACE_BYTES: *out = static_cast<int64_t>(h->ws.bytes()); break;
     case DSX_INFO_SM_COUNT: *out = h->sm_count; break;
     case DSX_INFO_TC_CTA_GROUP: *out = h->tc_group; break;
     case DSX_INFO_LAYER_KERNEL_LAUNCHES: *out = static_cast<int64_t>(h->prof_used / 2); break;

@@ -329,9 +329,7 @@ int fft_embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream_t 
   DSX_TRY(launch_embed_mlp(h, f->emb, t_dev, rows, emb, s));
   const int warps = rows * H;
   k_fft_tproj<<<(warps + 7) / 8, 256, 0, s>>>(emb, f->wd, dim + H + dim, dim + H, dim, H, rows, ttab);
-  DSX_TRY(launch_check("k_fft_tproj"));
-  h->launches++;
-  return DSX_OK;
+  return counted_launch(h, "k_fft_tproj");
 }
 
 int fft_eval(dsx_handle* h, const float* x, dsx_strides xs, const Geom& g, int row0, int row_per_b, float* eps,

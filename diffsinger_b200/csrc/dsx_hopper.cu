@@ -994,18 +994,16 @@ int tc_pack_model(dsx_handle* h, cudaStream_t s) {
   __half* wpack;
   float* b1p;
   const size_t rows = static_cast<size_t>(h->m.L) * kRowsPerLayer;
-  DSX_TRY(dev_alloc(h, reinterpret_cast<void**>(&wpack), rows * 64 * sizeof(__half), true));
-  DSX_TRY(dev_alloc(h, reinterpret_cast<void**>(&b1p), static_cast<size_t>(h->m.L) * 512 * sizeof(float), true));
+  DSX_TRY(h->mem.alloc(&wpack, rows * 64 * sizeof(__half)));
+  DSX_TRY(h->mem.alloc(&b1p, static_cast<size_t>(h->m.L) * 512 * sizeof(float)));
   k_pack_wtc<<<dim3(kRowsPerLayer / 256, h->m.L), 256, 0, s>>>(h->m.w1f, h->m.w2f, h->m.b1f, wpack, b1p);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
+  DSX_TRY(counted_launch(h, "k_pack_wtc"));
   h->m.wpack = wpack;
   h->m.b1p = b1p;
   __half* whead;
-  DSX_TRY(dev_alloc(h, reinterpret_cast<void**>(&whead), static_cast<size_t>(32) * 128 * 64 * sizeof(__half), true));
+  DSX_TRY(h->mem.alloc(&whead, static_cast<size_t>(32) * 128 * 64 * sizeof(__half)));
   k_pack_whead<<<32, 128, 0, s>>>(h->m.skip_w, h->m.fin_w, h->m.in_w, whead, h->m.M);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
+  DSX_TRY(counted_launch(h, "k_pack_whead"));
   h->m.whead = whead;
   h->m.wsr = nullptr;
   h->m.wsr_sets = 0;
@@ -1013,10 +1011,9 @@ int tc_pack_model(dsx_handle* h, cudaStream_t s) {
     const int R = std::max(1, h->sr_sets);
     __half* wsr;
     const size_t srows = static_cast<size_t>(R) * h->m.L * kSrRowsPerLayer;
-    DSX_TRY(dev_alloc(h, reinterpret_cast<void**>(&wsr), srows * 64 * sizeof(__half), true));
+    DSX_TRY(h->mem.alloc(&wsr, srows * 64 * sizeof(__half)));
     k_pack_wsr<<<dim3(32, h->m.L, R), 256, 0, s>>>(h->m.w1f, h->m.w2f, wsr, h->m.L, h->sr_seed);
-    h->launches++;
-    DSX_CUDA(cudaGetLastError());
+    DSX_TRY(counted_launch(h, "k_pack_wsr"));
     h->m.wsr = wsr;
     h->m.wsr_sets = R;
   }
@@ -1105,8 +1102,7 @@ static int launch_step(dsx_handle* h, const HpParams& prm, cudaStream_t s) {
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   DSX_CUDA(cudaLaunchKernelEx(&cfg, k_hp_step<NWG, R>, prm));
-  h->launches++;
-  return DSX_OK;
+  return counted_launch(h, "k_hp_step");
 }
 
 // Layers that read z's lo plane (P = 3) keep it out of the ring and run a two-stage ring; every other launch runs three.
@@ -1129,9 +1125,7 @@ int launch_tc_condproj(dsx_handle* h, const Geom& g, cudaStream_t s) {
   HpParams prm = base_params(h, g, 128);
   prm.w = h->m.wpack;
   k_hp_condproj<<<dim3(static_cast<unsigned>(prm.units), static_cast<unsigned>(h->m.L)), 256, kCondSmem, s>>>(prm);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+  return counted_launch(h, "k_hp_condproj");
 }
 
 // Frames per CTA for this call: 64 (one warpgroup per CTA, twice the CTAs) whenever the whole batch then has a CTA per

@@ -1,6 +1,5 @@
 // Internal declarations shared by the dsx translation units (not part of the C ABI).
 #pragma once
-#include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -34,7 +33,7 @@ void set_error(const char* fmt, ...);
     if (_r != DSX_OK) return _r; \
   } while (0)
 
-// ---- handle plumbing of the vocoder and the pitch extractor --------------------------------------
+// ---- handle plumbing ------------------------------------------------------------------------------
 // the error of the last launch, if any, as DSX_E_CUDA naming the kernel
 inline int launch_check(const char* what) {
   cudaError_t e = cudaGetLastError();
@@ -87,11 +86,24 @@ struct GrowBuffer {
     cap = need + need / 8;
     return DSX_OK;
   }
+  // reserve that zero-fills a buffer it (re)allocated, on s
+  int reserve_zeroed(size_t need, cudaStream_t s) {
+    if (cap >= need) return DSX_OK;
+    DSX_TRY(reserve(need, s));
+    DSX_CUDA(cudaMemsetAsync(ptr, 0, cap, s));
+    return DSX_OK;
+  }
   void release() {
     if (ptr) cudaFree(ptr);
     ptr = nullptr;
     cap = 0;
   }
+};
+
+// a GrowBuffer that reads as a T*
+template <typename T>
+struct Buf : GrowBuffer {
+  operator T*() const { return static_cast<T*>(ptr); }
 };
 
 inline size_t align256(size_t bytes) { return (bytes + 255) & ~size_t(255); }
@@ -107,8 +119,8 @@ struct Bump {
   }
 };
 
-// makes `device` current after checking that it exists and is sm_90, the only target of the kernels of `what`
-inline int select_sm90_device(int device, const char* what) {
+// makes `device` current after checking that it exists; its properties to *prop
+inline int select_device(int device, cudaDeviceProp* prop) {
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev == 0) {
@@ -116,11 +128,17 @@ inline int select_sm90_device(int device, const char* what) {
     return DSX_E_CUDA;
   }
   DSX_CHECK(device >= 0 && device < ndev, DSX_E_INVALID, "device %d out of range (%d devices)", device, ndev);
+  DSX_CUDA(cudaGetDeviceProperties(prop, device));
+  DSX_CUDA(cudaSetDevice(device));
+  return DSX_OK;
+}
+
+// select_device for the kernels of `what`, whose only target is sm_90
+inline int select_sm90_device(int device, const char* what) {
   cudaDeviceProp prop;
-  DSX_CUDA(cudaGetDeviceProperties(&prop, device));
+  DSX_TRY(select_device(device, &prop));
   DSX_CHECK(prop.major == 9 && prop.minor == 0, DSX_E_CUDA, "the %s's kernels are built for sm_90a; device %d is sm_%d%d",
             what, device, prop.major, prop.minor);
-  DSX_CUDA(cudaSetDevice(device));
   return DSX_OK;
 }
 
@@ -169,29 +187,42 @@ struct ModelDev {
   int wsr_sets;        // R
 };
 
+// Grow-only buffers of the sampler, each its own allocation: growth of one leaves the others, and what they hold, in place
 struct Workspace {
-  Geom g;               // capacity geometry (B, Tp) currently allocated
+  Geom g;               // geometry (B, T) of the last call
   int rows_cap = 0;     // step-table rows
-  float* X = nullptr;       // [B][Tp][C] residual stream
-  float* SKIP = nullptr;    // [B][Tp][C]
-  float* CONDF = nullptr;   // [B][Tp][H] fp32 (SIMT path)
-  float* G1 = nullptr;      // [B][Tp][2C] SIMT GEMM output scratch
-  float* Zf = nullptr;      // [B][Tp][C]  SIMT gate output
-  __half* Y = nullptr;      // [2 buffers][2 planes][B][Tp][C]
-  __half* CONDH = nullptr;  // [2 planes][B][Tp][H]
-  float* CP = nullptr;      // [L][B][Tp][512] conditioner projection + bias of every layer (tensor-core path)
-  __half* S16 = nullptr;    // [2 planes][B][Tp][C] skip_sum / sqrt(L), operand of the head GEMM
-  unsigned* FLAGS = nullptr; // [2][B * Tp / 64] per-tile progress flags of the step kernel (tensor-core path)
-  float* DTAB = nullptr;    // [rows][L][C]
-  float* EMB = nullptr;     // [rows][C] scratch (mlp output)
-  int64_t* TVALS = nullptr; // [rows]
-  float* EPS = nullptr;     // [5][B][M][T] current + PLMS history ring
-  float* XTMP = nullptr;    // [B][M][T] PLMS warm-up state
-  float* XSTATE = nullptr;  // [B][M][T] mel state of dsx_infer
-  size_t bytes = 0;
-  // byte capacities (grow-only)
-  size_t cap_X = 0, cap_SKIP = 0, cap_CONDF = 0, cap_G1 = 0, cap_Zf = 0, cap_Y = 0, cap_CONDH = 0, cap_CP = 0, cap_S16 = 0,
-         cap_FLAGS = 0, cap_DTAB = 0, cap_EMB = 0, cap_TVALS = 0, cap_EPS = 0, cap_XTMP = 0, cap_XSTATE = 0;
+  Buf<float> X;         // [B][Tp][C] residual stream
+  Buf<float> SKIP;      // [B][Tp][C]
+  Buf<float> CONDF;     // [B][Tp][H] fp32 (SIMT path)
+  Buf<float> G1;        // [B][Tp][2C] SIMT GEMM output scratch
+  Buf<float> Zf;        // [B][Tp][C]  SIMT gate output
+  Buf<__half> Y;        // [2 buffers][2 planes][B][Tp][C]
+  Buf<__half> CONDH;    // [2 planes][B][Tp][H]
+  Buf<float> CP;        // [L][B][Tp][512] conditioner projection + bias of every layer (tensor-core path)
+  Buf<__half> S16;      // [2 planes][B][Tp][C] skip_sum / sqrt(L), operand of the head GEMM
+  Buf<unsigned> FLAGS;  // [2][B * Tp / 64] per-tile progress flags of the step kernel (tensor-core path)
+  Buf<float> DTAB;      // [rows][L][C]
+  Buf<float> EMB;       // [rows][C] scratch (mlp output)
+  Buf<int64_t> TVALS;   // [rows]
+  Buf<float> EPS;       // [5][B][M][T] current + PLMS history ring
+  Buf<float> XTMP;      // [B][M][T] PLMS warm-up state
+  Buf<float> XSTATE;    // [B][M][T] mel state of dsx_infer
+  // f(GrowBuffer&) on every buffer: the one list of them, behind bytes() and release()
+  template <typename F>
+  void each(F f) {
+    f(X); f(SKIP); f(CONDF); f(G1); f(Zf); f(Y); f(CONDH); f(CP); f(S16); f(FLAGS); f(DTAB); f(EMB); f(TVALS); f(EPS);
+    f(XTMP); f(XSTATE);
+  }
+  size_t bytes() {   // DSX_INFO_WORKSPACE_BYTES
+    size_t n = 0;
+    each([&](GrowBuffer& b) { n += b.cap; });
+    return n;
+  }
+  void release() {
+    each([](GrowBuffer& b) { b.release(); });
+    g = Geom();
+    rows_cap = 0;
+  }
 };
 
 struct FftDenoiser;   // dsx_fftdiff.cu
@@ -208,15 +239,14 @@ struct dsx_handle {
   int64_t launches = 0;
   int64_t stack_launches = 0;   // one-launch-per-step launches of k_hp_step (layers + fused head)
   dsx::ModelDev m{};
-  std::vector<void*> owned;   // device allocations of the model
+  dsx::DevAllocs mem;         // device allocations of the model
   int sched_T = 0;
   std::vector<float> sched[DSX_SCH_COUNT];
   dsx::Workspace ws;
   int* status_dev = nullptr;   // kernel watchdog / self-check word
   int* status_host = nullptr;  // pinned mirror
   int profile = 0;
-  void* stage[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // dsx_infer_host device staging
-  size_t stage_cap[7] = {0, 0, 0, 0, 0, 0, 0};
+  dsx::GrowBuffer stage[7];    // dsx_infer_host device staging
   int stack_kernel = 1;                // DSX_OPT_STACK_KERNEL: 1 = layers and head of a step in one launch where it applies
   int step_occ[3] = {};                // co-resident CTAs of k_hp_step<NWG, R> <1, 3> / <2, 3> / <2, 2> on the device (0 unknown, -1 none)
   int fused_head = 1;                  // DSX_OPT_FUSED_HEAD: the head / sampler update / next input projection run inside the stack launch
@@ -224,7 +254,6 @@ struct dsx_handle {
   int stack_rows_used = 0;             // rows per CTA of the last stack launch
   int sr_sets = 64;                    // DSX_OPT_SR_SETS: weight sets of DSX_PREC_FP16S (takes effect at the next dsx_load_diffnet)
   unsigned long long sr_seed = 0x5DEECE66Dull;
-  unsigned long long ws_epoch = 0;     // bumped whenever a workspace buffer moves (tensor maps are rebuilt)
   bool cond_ready = false;             // CONDH / CP (or CONDF) hold the conditioner of dsx_set_cond for geometry cond_geom
   dsx::Geom cond_geom;
   int gate_approx = -1;                // DSX_OPT_GATE_APPROX: -1 = default (tanh.approx gate), 0 / 1 forced
@@ -239,6 +268,12 @@ struct dsx_handle {
 };
 
 namespace dsx {
+
+// launch_check of a launch (or the last of n) that DSX_INFO_KERNEL_LAUNCHES counts
+inline int counted_launch(dsx_handle* h, const char* what, int n = 1) {
+  h->launches += n;
+  return launch_check(what);
+}
 
 // ---- dsx_simt.cu -------------------------------------------------------------------------
 int simt_pack_model(dsx_handle* h, const dsx_diffnet_params* p, cudaStream_t s);
@@ -300,7 +335,6 @@ bool tc_fuse_head(const dsx_handle* h);
 int launch_tc_step(dsx_handle* h, const Geom& g, int l0, int l1, int row0, int row_per_b, const HeadArgs* head,
                    cudaStream_t s);
 
-int dev_alloc(dsx_handle* h, void** p, size_t bytes, bool model_owned);
 int ensure_workspace(dsx_handle* h, const Geom& g, int rows, cudaStream_t s);
 int check_status(dsx_handle* h, cudaStream_t s, const char* what);
 

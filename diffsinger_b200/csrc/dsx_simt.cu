@@ -42,52 +42,40 @@ int simt_pack_model(dsx_handle* h, const dsx_diffnet_params* p, cudaStream_t s) 
   ModelDev& m = h->m;
   const int C = m.C, H = m.H, M = m.M, L = m.L;
   const size_t K1 = 3 * static_cast<size_t>(C) + H;
-  float *in_w, *in_b, *mlp0_w, *mlp0_b, *mlp2_w, *mlp2_b, *dif_w, *dif_b, *w1f, *b1f, *w2f, *b2f, *skip_w, *skip_b,
-      *fin_w, *fin_b;
-#define ALLOC(ptr, n) DSX_TRY(dev_alloc(h, reinterpret_cast<void**>(&ptr), (n) * sizeof(float), true))
-#define COPY(dst, src, n) DSX_CUDA(cudaMemcpyAsync(dst, src, (n) * sizeof(float), cudaMemcpyDeviceToDevice, s))
-  ALLOC(in_w, static_cast<size_t>(C) * M);
-  ALLOC(in_b, C);
-  ALLOC(mlp0_w, static_cast<size_t>(4) * C * C);
-  ALLOC(mlp0_b, 4 * C);
-  ALLOC(mlp2_w, static_cast<size_t>(4) * C * C);
-  ALLOC(mlp2_b, C);
-  ALLOC(dif_w, static_cast<size_t>(L) * C * C);
-  ALLOC(dif_b, static_cast<size_t>(L) * C);
-  ALLOC(w1f, static_cast<size_t>(L) * 2 * C * K1);
-  ALLOC(b1f, static_cast<size_t>(L) * 2 * C);
-  ALLOC(w2f, static_cast<size_t>(L) * 2 * C * C);
-  ALLOC(b2f, static_cast<size_t>(L) * 2 * C);
-  ALLOC(skip_w, static_cast<size_t>(C) * C);
-  ALLOC(skip_b, C);
-  ALLOC(fin_w, static_cast<size_t>(M) * C);
-  ALLOC(fin_b, M);
-  COPY(in_w, p->in_w, static_cast<size_t>(C) * M);
-  COPY(in_b, p->in_b, C);
-  COPY(mlp0_w, p->mlp0_w, static_cast<size_t>(4) * C * C);
-  COPY(mlp0_b, p->mlp0_b, 4 * C);
-  COPY(mlp2_w, p->mlp2_w, static_cast<size_t>(4) * C * C);
-  COPY(mlp2_b, p->mlp2_b, C);
-  COPY(skip_w, p->skip_w, static_cast<size_t>(C) * C);
-  COPY(skip_b, p->skip_b, C);
-  COPY(fin_w, p->fin_w, static_cast<size_t>(M) * C);
-  COPY(fin_b, p->fin_b, M);
+  // field = a new array of `count` blocks of n floats, block i a copy of src[i]
+  auto put = [&](const float*& field, const float* const* src, int count, size_t n) -> int {
+    float* d;
+    DSX_TRY(h->mem.alloc(&d, count * n * sizeof(float)));
+    for (int i = 0; i < count; ++i)
+      DSX_CUDA(cudaMemcpyAsync(d + i * n, src[i], n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    field = d;
+    return DSX_OK;
+  };
+  DSX_TRY(put(m.in_w, &p->in_w, 1, static_cast<size_t>(C) * M));
+  DSX_TRY(put(m.in_b, &p->in_b, 1, C));
+  DSX_TRY(put(m.mlp0_w, &p->mlp0_w, 1, static_cast<size_t>(4) * C * C));
+  DSX_TRY(put(m.mlp0_b, &p->mlp0_b, 1, 4 * C));
+  DSX_TRY(put(m.mlp2_w, &p->mlp2_w, 1, static_cast<size_t>(4) * C * C));
+  DSX_TRY(put(m.mlp2_b, &p->mlp2_b, 1, C));
+  DSX_TRY(put(m.dif_w, p->dif_w, L, static_cast<size_t>(C) * C));
+  DSX_TRY(put(m.dif_b, p->dif_b, L, C));
+  DSX_TRY(put(m.w2f, p->out_w, L, static_cast<size_t>(2) * C * C));
+  DSX_TRY(put(m.b2f, p->out_b, L, 2 * C));
+  DSX_TRY(put(m.skip_w, &p->skip_w, 1, static_cast<size_t>(C) * C));
+  DSX_TRY(put(m.skip_b, &p->skip_b, 1, C));
+  DSX_TRY(put(m.fin_w, &p->fin_w, 1, static_cast<size_t>(M) * C));
+  DSX_TRY(put(m.fin_b, &p->fin_b, 1, M));
+  float *w1f, *b1f;
+  DSX_TRY(h->mem.alloc(&w1f, static_cast<size_t>(L) * 2 * C * K1 * sizeof(float)));
+  DSX_TRY(h->mem.alloc(&b1f, static_cast<size_t>(L) * 2 * C * sizeof(float)));
   for (int l = 0; l < L; ++l) {
-    COPY(dif_w + static_cast<size_t>(l) * C * C, p->dif_w[l], static_cast<size_t>(C) * C);
-    COPY(dif_b + static_cast<size_t>(l) * C, p->dif_b[l], C);
-    COPY(w2f + static_cast<size_t>(l) * 2 * C * C, p->out_w[l], static_cast<size_t>(2) * C * C);
-    COPY(b2f + static_cast<size_t>(l) * 2 * C, p->out_b[l], 2 * C);
     k_pack_w1f<<<2 * C, 256, 0, s>>>(p->dil_w[l], p->cond_w[l], p->dil_b[l], p->cond_b[l],
                                      w1f + static_cast<size_t>(l) * 2 * C * K1, b1f + static_cast<size_t>(l) * 2 * C,
                                      C, H);
-    h->launches++;
+    DSX_TRY(counted_launch(h, "k_pack_w1f"));
   }
-  DSX_CUDA(cudaGetLastError());
-#undef ALLOC
-#undef COPY
-  m.in_w = in_w; m.in_b = in_b; m.mlp0_w = mlp0_w; m.mlp0_b = mlp0_b; m.mlp2_w = mlp2_w; m.mlp2_b = mlp2_b;
-  m.dif_w = dif_w; m.dif_b = dif_b; m.w1f = w1f; m.b1f = b1f; m.w2f = w2f; m.b2f = b2f;
-  m.skip_w = skip_w; m.skip_b = skip_b; m.fin_w = fin_w; m.fin_b = fin_b;
+  m.w1f = w1f;
+  m.b1f = b1f;
   return DSX_OK;
 }
 
@@ -159,17 +147,13 @@ __global__ void k_embed_proj(ModelDev m, const float* __restrict__ emb, float* _
 int launch_embed_mlp(dsx_handle* h, const ModelDev& m, const int64_t* t_dev, int rows, float* emb, cudaStream_t s) {
   const size_t smem = static_cast<size_t>(5) * m.C * sizeof(float);
   k_embed_table<<<rows, 512, smem, s>>>(m, t_dev, emb);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+  return counted_launch(h, "k_embed_table");
 }
 
 int launch_embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream_t s) {
   DSX_TRY(launch_embed_mlp(h, h->m, t_dev, rows, h->ws.EMB, s));
   k_embed_proj<<<(h->m.L * h->m.C + 15) / 16, 512, 0, s>>>(h->m, h->ws.EMB, h->ws.DTAB, rows);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+  return counted_launch(h, "k_embed_proj");
 }
 
 // ------------------------------------------------------------------------------------------
@@ -208,11 +192,11 @@ __global__ void k_pack_cond(const float* __restrict__ cond, dsx_strides cs, int 
 int launch_pack_cond(dsx_handle* h, const float* cond, dsx_strides cs, const Geom& g, cudaStream_t s) {
   dim3 grid((g.Tp + 31) / 32, (h->m.H + 31) / 32, g.B), block(32, 8);
   const bool tc = h->precision != DSX_PREC_FP32_SIMT;
-  k_pack_cond<<<grid, block, 0, s>>>(cond, cs, g.B, g.T, g.Tp, h->m.H, tc ? nullptr : h->ws.CONDF,
-                                     tc ? h->ws.CONDH : nullptr, g.frames_padded() * h->m.H);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+  float* const condf = h->ws.CONDF;
+  __half* const condh = h->ws.CONDH;
+  k_pack_cond<<<grid, block, 0, s>>>(cond, cs, g.B, g.T, g.Tp, h->m.H, tc ? nullptr : condf, tc ? condh : nullptr,
+                                     g.frames_padded() * h->m.H);
+  return counted_launch(h, "k_pack_cond");
 }
 
 // ------------------------------------------------------------------------------------------
@@ -264,12 +248,12 @@ int launch_inproj(dsx_handle* h, const float* x, dsx_strides xs, const Geom& g, 
                   cudaStream_t s) {
   dim3 grid((g.T + kInFrames - 1) / kInFrames, g.B);
   const bool tc = h->precision != DSX_PREC_FP32_SIMT;
+  __half* const y = h->ws.Y;
+  const float* const dtab = h->ws.DTAB;
   k_inproj<<<grid, 256, kInFrames * h->m.M * sizeof(float), s>>>(
-      h->m, x, xs, g.T, g.Tp, h->ws.X, tc ? h->ws.Y : nullptr, g.frames_padded() * h->m.C,
-      tc ? h->ws.DTAB : nullptr, row0, row_per_b);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+      h->m, x, xs, g.T, g.Tp, h->ws.X, tc ? y : nullptr, g.frames_padded() * h->m.C, tc ? dtab : nullptr, row0,
+      row_per_b);
+  return counted_launch(h, "k_inproj");
 }
 
 // ------------------------------------------------------------------------------------------
@@ -387,9 +371,7 @@ int launch_simt_layer(dsx_handle* h, int layer, const Geom& g, int row0, int row
   k_simt_gemm<0><<<grid1, 256, 0, s>>>(a2, m.w2f + static_cast<size_t>(layer) * 2 * C * C, C, 2 * C, h->ws.G1, 2 * C);
   k_resid<<<eb, 256, 0, s>>>(h->ws.G1, m.b2f + static_cast<size_t>(layer) * 2 * C, h->ws.X, h->ws.SKIP, C, ne,
                              layer == 0);
-  h->launches += 4;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+  return counted_launch(h, "fp32 residual layer (k_simt_gemm, k_gate, k_simt_gemm, k_resid)", 4);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -433,9 +415,7 @@ int launch_head(dsx_handle* h, const Geom& g, float* eps, cudaStream_t s) {
   k_simt_gemm<0><<<grid2, 256, 0, s>>>(a2, m.fin_w, C, M, h->ws.G1, 2 * C);
   dim3 grid3((g.T + 31) / 32, (M + 31) / 32, g.B), block3(32, 8);
   k_eps_out<<<grid3, block3, 0, s>>>(h->ws.G1, m.fin_b, eps, M, g.T, g.Tp, 2 * C);
-  h->launches += 4;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+  return counted_launch(h, "fp32 head (k_simt_gemm, k_bias_relu, k_simt_gemm, k_eps_out)", 4);
 }
 
 // p_sample after the network (shallow_diffusion_tts.py:134-166), same fp32 operation order
@@ -464,9 +444,7 @@ __global__ void k_ddpm_update(float* __restrict__ x, const float* __restrict__ e
 int launch_ddpm_update(dsx_handle* h, float* x, const float* eps, const float* noise, uint64_t seed, uint64_t offset,
                        DdpmCoef c, size_t n, int T, cudaStream_t s) {
   k_ddpm_update<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(x, eps, noise, seed, offset, c, n, h->m.M, T, h->batch_offset);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+  return counted_launch(h, "k_ddpm_update");
 }
 
 // PLMS (shallow_diffusion_tts.py:174-199): eps' = (w0*e0 + w1*e1 + w2*e2 + w3*e3) / denom with the
@@ -489,9 +467,7 @@ __global__ void k_plms_update(float* __restrict__ xo, const float* __restrict__ 
 int launch_plms_update(dsx_handle* h, float* x_out, const float* x_in, const float* e0, const float* e1,
                        const float* e2, const float* e3, PlmsCoef c, size_t n, cudaStream_t s) {
   k_plms_update<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(x_out, x_in, e0, e1, e2, e3, c, n);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+  return counted_launch(h, "k_plms_update");
 }
 
 // prologue of the infer branch (shallow_diffusion_tts.py:249-255): norm_spec (:278-279), transpose to
@@ -527,9 +503,7 @@ int launch_prologue(dsx_handle* h, float* x, const float* fs2_mel, const float* 
                     cudaStream_t s) {
   dim3 grid((T + 31) / 32, (M + 31) / 32, B), block(32, 8);
   k_prologue<<<grid, block, 0, s>>>(x, fs2_mel, start_noise, seed, spec_min, spec_max, sa, s1a, T, M, h->batch_offset);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+  return counted_launch(h, "k_prologue");
 }
 
 // epilogue (:271-275): x[:,0].transpose(1,2) -> denorm_spec (:281-282) -> * (mel2ph > 0)
@@ -558,9 +532,7 @@ int launch_epilogue(dsx_handle* h, const float* x, const int64_t* mel2ph, const 
                     const float* spec_max, float* mel_out, int B, int T, int M, cudaStream_t s) {
   dim3 grid((T + 31) / 32, (M + 31) / 32, B), block(32, 8);
   k_epilogue<<<grid, block, 0, s>>>(x, mel2ph, spec_min, spec_max, mel_out, T, M);
-  h->launches++;
-  DSX_CUDA(cudaGetLastError());
-  return DSX_OK;
+  return counted_launch(h, "k_epilogue");
 }
 
 }  // namespace dsx

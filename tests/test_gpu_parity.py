@@ -433,6 +433,27 @@ def test_shard_equivalence_and_determinism(dsx):
     s.close()
 
 
+@pytest.mark.parametrize("prec", ["fp32", "fp16s"])
+def test_handle_survives_workspace_growth(dsx, prec):
+    """The workspace is grow-only: a larger (B, T) and more steps free and reallocate every buffer (zero-filled), and the
+    small call that follows, in the grown buffers, returns what it returned in the first ones, bit for bit."""
+    from diffsinger_b200 import _capi
+    S = O.make_schedule(O.linear_beta_schedule(100, 0.06))
+    s, dev = make_sampler(dsx, 1, prec, S)
+
+    def run(B, T, K):
+        cond, xT = rs_normal(3, (B, 256, T)).to(dev), rs_normal(4, (B, 1, 80, T)).to(dev)
+        return s.sample_ddpm(xT, cond, 100, K, seed=7), s.info(_capi.INFO_WORKSPACE_BYTES)
+
+    small, w_small = run(1, 100, 3)
+    large, w_large = run(3, 400, 8)
+    again, w_again = run(1, 100, 3)
+    assert torch.isfinite(large).all()
+    assert torch.equal(small, again)
+    assert w_large > w_small and w_again == w_large
+    s.close()
+
+
 def test_seed_mode_shard_equivalence(dsx):
     """In-kernel Philox noise is indexed by the GLOBAL utterance number (DSX_OPT_BATCH_OFFSET, set by
     parallel.sharded_infer): with one seed, two half-batch shards reproduce the unsharded batch bit for bit and the
