@@ -30,9 +30,10 @@ SYMBOLS = (
     "dsx_fs2enc_create", "dsx_fs2enc_destroy", "dsx_fs2enc_load", "dsx_fs2enc_forward",
     "dsx_durpred_create", "dsx_durpred_destroy", "dsx_durpred_load", "dsx_durpred_forward",
     "dsx_length_totals", "dsx_length_regulate",
+    "dsx_train_create", "dsx_train_destroy", "dsx_train_tape_bytes", "dsx_train_workspace_bytes", "dsx_train_forward", "dsx_train_backward",
 )
 _VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy", "dsx_fs2dec_destroy",
-         "dsx_fs2enc_destroy", "dsx_durpred_destroy")
+         "dsx_fs2enc_destroy", "dsx_durpred_destroy", "dsx_train_destroy")
 
 
 class DsxError(RuntimeError):
@@ -121,6 +122,11 @@ class DurPredParams(ctypes.Structure):
                 ("linear_b", _fp)]
 
 
+class TrainConfig(ctypes.Structure):
+    _fields_ = [("M", ctypes.c_int), ("C", ctypes.c_int), ("H", ctypes.c_int), ("L", ctypes.c_int),
+                ("dilation_cycle", ctypes.c_int)]
+
+
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"dsx CUDA library not found at {LIB_PATH}; build it with `python diffsinger_b200/build.py` "
@@ -176,6 +182,15 @@ lib.dsx_durpred_load.argtypes = [_vp, ctypes.POINTER(DurPredParams), _vp]
 lib.dsx_durpred_forward.argtypes = [_vp, _vp, Strides, _vp, _i, _i, _vp, _vp, _vp]
 lib.dsx_length_totals.argtypes = [_vp, _vp, _i, _i, ctypes.c_float, _vp, _vp, _vp]
 lib.dsx_length_regulate.argtypes = [_vp, _vp, _i, _i, _i, _vp, _vp]
+lib.dsx_train_create.argtypes = [_i, ctypes.POINTER(TrainConfig), ctypes.POINTER(_vp)]
+lib.dsx_train_destroy.argtypes = [_vp]
+lib.dsx_train_destroy.restype = None
+lib.dsx_train_tape_bytes.argtypes = [_vp, _i, _i, ctypes.POINTER(ctypes.c_size_t)]
+lib.dsx_train_workspace_bytes.argtypes = [_vp, _i, _i, ctypes.POINTER(ctypes.c_size_t)]
+lib.dsx_train_forward.argtypes = [_vp, ctypes.POINTER(DiffNetParams), _vp, Strides, _vp, _vp, Strides, _i, _i, _vp,
+                                  ctypes.c_size_t, _vp, ctypes.c_size_t, _vp, _vp]
+lib.dsx_train_backward.argtypes = [_vp, ctypes.POINTER(DiffNetParams), _vp, _vp, ctypes.POINTER(DiffNetParams), _vp,
+                                   _i, _i, _vp, ctypes.c_size_t, _vp]
 for _n in SYMBOLS:
     if _n not in _VOID:
         getattr(lib, _n).restype = _i

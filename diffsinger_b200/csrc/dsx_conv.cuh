@@ -75,11 +75,12 @@ int conv_opt_in(K kernel_of) {
   return DSX_OK;
 }
 
-// acc (this warpgroup's NT / WG columns) = A . B over all g.kc chunks.  A is the 64 rows from m0 of utterance b of x
-// [B][lx][g.cin]; B is column tile `tile` of g.w.  smem: conv_smem<NT>() bytes, 1024-byte aligned.
+// acc (this warpgroup's NT / WG columns) = A . B over all g.kc chunks, or acc += A . B with `accumulate` (a second
+// operand pair summed into the same accumulators).  A is the 64 rows from m0 of utterance b of x [B][lx][g.cin]; B is
+// column tile `tile` of g.w.  smem: conv_smem<NT>() bytes, 1024-byte aligned.
 template <int NT, int WG>
 __device__ __forceinline__ void conv_k_loop(const ConvGemm& g, const __half* x, int lx, int valid_rows, int b, int m0,
-                                            int tile, uint8_t* smem, float (&acc)[NT / WG / 2]) {
+                                            int tile, uint8_t* smem, float (&acc)[NT / WG / 2], bool accumulate = false) {
   constexpr int NH = NT / WG, NTHR = 128 * WG, kA = kConvRows * 128, kStage = kA + NT * 128;
   const int tid = threadIdx.x, wg = WG > 1 ? tid >> 7 : 0;   // a constant 0 keeps the wgmma descriptors uniform
   auto load = [&](int s, uint8_t* buf) {
@@ -99,8 +100,10 @@ __device__ __forceinline__ void conv_k_loop(const ConvGemm& g, const __half* x, 
     }
   };
 
+  if (!accumulate) {
 #pragma unroll
-  for (int e = 0; e < NH / 2; ++e) acc[e] = 0.f;
+    for (int e = 0; e < NH / 2; ++e) acc[e] = 0.f;
+  }
   load(0, smem);
   cp_commit();
 #pragma unroll 1

@@ -280,6 +280,8 @@ int simt_pack_model(dsx_handle* h, const dsx_diffnet_params* p, cudaStream_t s);
 int launch_embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream_t s);
 // emb[row] = mlp(SinusoidalPosEmb(m.C)(t[row])) for `rows` rows (m: C and the mlp weights)
 int launch_embed_mlp(dsx_handle* h, const ModelDev& m, const int64_t* t_dev, int rows, float* emb, cudaStream_t s);
+// the same, also saving each row's sinusoid, mlp.0 output and its Mish to save [rows][9 C] (the training step's tape)
+int launch_embed_saved(const ModelDev& m, const int64_t* t_dev, int rows, float* emb, float* save, cudaStream_t s);
 int launch_pack_cond(dsx_handle* h, const float* cond, dsx_strides cs, const Geom& g, cudaStream_t s);
 int launch_inproj(dsx_handle* h, const float* x, dsx_strides xs, const Geom& g, int row0, int row_per_b,
                   cudaStream_t s);

@@ -85,7 +85,10 @@ int simt_pack_model(dsx_handle* h, const dsx_diffnet_params* p, cudaStream_t s) 
 // cos as separate fp32 ops); here each transcendental is evaluated in double and rounded once,
 // which is within 1 ulp of any conforming fp32 libm.
 // ------------------------------------------------------------------------------------------
-__global__ void k_embed_table(ModelDev m, const int64_t* __restrict__ tvals, float* __restrict__ emb_out) {
+// save (or null): [row][9 C] the sinusoid (C), mlp.0's output (4 C) and the Mish of it (4 C), for the training step's
+// backward
+__global__ void k_embed_table(ModelDev m, const int64_t* __restrict__ tvals, float* __restrict__ emb_out,
+                              float* __restrict__ save) {
   extern __shared__ float sm[];
   const int C = m.C;
   float* e0 = sm;           // [C]  sinusoid
@@ -117,7 +120,13 @@ __global__ void k_embed_table(ModelDev m, const int64_t* __restrict__ tvals, flo
     // Mish: x * tanh(softplus(x)); softplus with torch's threshold (20) semantics
     float sp = acc > 20.f ? acc : log1pf(expf(acc));
     if (lane == 0) h1[j] = acc * tanhf(sp);
+    if (save && lane == 0) {
+      save[static_cast<size_t>(row) * 9 * C + C + j] = acc;
+      save[static_cast<size_t>(row) * 9 * C + 5 * C + j] = h1[j];
+    }
   }
+  if (save)
+    for (int i = threadIdx.x; i < C; i += blockDim.x) save[static_cast<size_t>(row) * 9 * C + i] = e0[i];
   __syncthreads();
   for (int j = warp; j < C; j += nwarps) {
     float acc = dot(m.mlp2_w + static_cast<size_t>(j) * 4 * C, h1, 4 * C) + m.mlp2_b[j];
@@ -146,8 +155,14 @@ __global__ void k_embed_proj(ModelDev m, const float* __restrict__ emb, float* _
 
 int launch_embed_mlp(dsx_handle* h, const ModelDev& m, const int64_t* t_dev, int rows, float* emb, cudaStream_t s) {
   const size_t smem = static_cast<size_t>(5) * m.C * sizeof(float);
-  k_embed_table<<<rows, 512, smem, s>>>(m, t_dev, emb);
+  k_embed_table<<<rows, 512, smem, s>>>(m, t_dev, emb, nullptr);
   return counted_launch(h, "k_embed_table");
+}
+
+int launch_embed_saved(const ModelDev& m, const int64_t* t_dev, int rows, float* emb, float* save, cudaStream_t s) {
+  const size_t smem = static_cast<size_t>(5) * m.C * sizeof(float);
+  k_embed_table<<<rows, 512, smem, s>>>(m, t_dev, emb, save);
+  return launch_check("k_embed_table");
 }
 
 int launch_embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream_t s) {

@@ -6,8 +6,9 @@
 Same state-dict keys (``denoise_fn.residual_layers.{l}.dilated_conv.weight`` ...), so reference
 checkpoints load with ``strict=True``.  Under ``torch.no_grad`` / ``infer=True`` every evaluation goes
 to the sm_90a kernels through the C ABI and fails loudly on CPU tensors.  The training branch
-(``p_losses`` under autograd) is outside this round's scope (section 8f rank 4): it keeps the module
-graph in plain PyTorch ops so existing training code still runs, and is never used for inference.
+(``p_losses`` under autograd) keeps the module graph in plain PyTorch ops unless ``DiffNet`` is built with the
+``dsx_train`` opt-in (hparams key or ``train=`` keyword): then its forward and backward run on the sm_90a training
+step of ``diffsinger_b200.train``.
 """
 import math
 from collections import deque
@@ -84,7 +85,7 @@ class DiffNet(nn.Module):
     """Drop-in for usr.diff.net.DiffNet: ``DiffNet(in_dims=80)`` reads ``hidden_size``,
     ``residual_layers``, ``residual_channels``, ``dilation_cycle_length`` from hparams (net.py:84-89)."""
 
-    def __init__(self, in_dims=80, hparams=None, precision=None):
+    def __init__(self, in_dims=80, hparams=None, precision=None, train=None):
         super().__init__()
         hp = _get_hparams(hparams)
         self.params = params = dict(
@@ -102,6 +103,15 @@ class DiffNet(nn.Module):
         nn.init.zeros_(self.output_projection.weight)
         self._dsx = None
         self._dsx_precision = precision or hp.get("dsx_precision")
+        self._dsx_train = bool(train if train is not None else hp.get("dsx_train", False))
+        self._dsx_trainer = None
+
+    def _dsx_train_step(self):
+        if self._dsx_trainer is None:
+            from .train import TrainStep
+            object.__setattr__(self, "_dsx_trainer", TrainStep(len(self.residual_layers),
+                                                               self.params["dilation_cycle_length"]))
+        return self._dsx_trainer
 
     @property
     def dsx(self):
@@ -114,7 +124,11 @@ class DiffNet(nn.Module):
 
         Training mode (``self.training``: p_losses under autograd) or an input that itself requires grad keeps the module
         graph in plain PyTorch ops; everything else -- ``model.eval()``, with or without ``torch.no_grad()`` -- is inference
-        and goes to libdsx (no silent PyTorch path: CPU tensors / a missing library raise)."""
+        and goes to libdsx (no silent PyTorch path: CPU tensors / a missing library raise).  With the ``dsx_train``
+        opt-in, training mode under autograd runs libdsx's training step instead (DsxError for what it does not run)."""
+        if self._dsx_train and self.training and torch.is_grad_enabled():
+            from .train import diffnet_train_forward
+            return diffnet_train_forward(self, spec, diffusion_step, cond)
         if self.training or (torch.is_grad_enabled() and spec.requires_grad):
             return self._forward_autograd(spec, diffusion_step, cond)
         return self.dsx.diffnet_forward(spec, diffusion_step, cond)
@@ -123,6 +137,7 @@ class DiffNet(nn.Module):
         # the lazily created sampler holds a ctypes handle: copies (EMA deepcopy, torch.save of the module) rebuild theirs
         state = self.__dict__.copy()
         state["_dsx"] = None
+        state["_dsx_trainer"] = None
         return state
 
     def _forward_autograd(self, spec, diffusion_step, cond):

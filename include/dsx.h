@@ -18,6 +18,7 @@
 #ifndef DSX_H_
 #define DSX_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -571,6 +572,54 @@ int dsx_length_totals(const int64_t* dur, const uint8_t* pad, int B, int T, floa
                       void* stream);
 int dsx_length_regulate(const int64_t* cum, const int64_t* totals, int B, int T, int T_mel, int64_t* mel2ph,
                         void* stream);
+
+/* ---- DiffNet training step: forward with a saved tape, and backward --------------------------------------------------
+ * Replaces: DiffNet.forward (usr/diff/net.py:107-130) under autograd, as GaussianDiffusion.p_losses
+ * (usr/diff/shallow_diffusion_tts.py:213-231) calls it in training, and its backward: the gradient of every DiffNet
+ * parameter and of cond (not of spec).  q_sample, the loss and the optimizer stay with the caller.  GEMMs run on tensor
+ * cores with fp16 operands and fp32 accumulation; the residual stream, the skip sum, eps and every gradient are fp32.
+ * The backward scales its fp16 gradient operands by a power of two S chosen on the device from amax |d_eps| (S amax in
+ * [2^5, 2^6), leaving about 2^10 of fp16 range above the largest scaled operand) and divides it out exactly, so the gradients for 2^k d_eps are exactly 2^k times those for d_eps, and
+ * d_eps = 0 gives exact zeros.  Gradients are bitwise reproducible (fixed-order reductions, no atomics).  No call
+ * synchronises the host or allocates: the tape and the scratch workspace are the caller's.  A training handle is independent of the other handles. */
+typedef struct dsx_train dsx_train;
+
+typedef struct {
+  int M;                   /* in_dims: 80                                     */
+  int C;                   /* residual_channels: 256                          */
+  int H;                   /* hidden_size (cond channels): 256                */
+  int L;                   /* residual_layers: >= 1                           */
+  int dilation_cycle;      /* dilation_cycle_length: dilation 2^(l % cycle)   */
+} dsx_train_config;
+
+/* Validates the configuration (DSX_E_INVALID). */
+int dsx_train_create(int device, const dsx_train_config* cfg, dsx_train** out);
+void dsx_train_destroy(dsx_train* h);
+
+/* Bytes of the tape of one forward over B utterances of T frames (F = B T), each region rounded up to 256 bytes
+ * (a256): a256(160 F) + a256(512 F) x 4 + a256(1024 B) + a256(9216 B) + L x (a256(512 F) x 2 + a256(1024 F)). */
+int dsx_train_tape_bytes(dsx_train* h, int B, int T, size_t* out);
+
+/* Bytes of the scratch workspace a forward or a backward over (B, T) needs.  The caller owns it (so a framework's
+ * allocator sees and reuses it); it holds nothing between calls, and calls that may overlap need separate workspaces. */
+int dsx_train_workspace_bytes(dsx_train* h, int B, int T, size_t* out);
+
+/* One forward: eps [B,1,M,T] (contiguous) of spec [B,1,M,T] (through ss: b, c = mel bin, t), t device int64 [B], cond
+ * [B,H,T] (through cs), with the activations the backward needs written to `tape` (caller-owned device memory of at
+ * least dsx_train_tape_bytes) and `workspace` (at least dsx_train_workspace_bytes) as scratch.  The weights
+ * (dsx_load_diffnet's pointer struct) are packed to fp16 inside the call, on the stream; the backward uses the packs of
+ * the latest forward on the handle, so the weights must not change between a forward and the backward of its tape.
+ * Several forwards may precede their backwards, each with its own tape. */
+int dsx_train_forward(dsx_train* h, const dsx_diffnet_params* w, const float* spec, dsx_strides ss, const int64_t* t,
+                      const float* cond, dsx_strides cs, int B, int T, void* tape, size_t tape_bytes, void* workspace,
+                      size_t workspace_bytes, float* eps, void* stream);
+
+/* The backward of the forward that wrote `tape` (same B, T): d_eps [B,1,M,T] contiguous.  Writes (does not accumulate)
+ * the fp32 gradient of every parameter through `grads` (same layout as w), and d_cond [B,H,T] contiguous unless NULL.
+ * The tape is only read; `workspace` (at least dsx_train_workspace_bytes) is scratch. */
+int dsx_train_backward(dsx_train* h, const dsx_diffnet_params* w, const void* tape, const float* d_eps,
+                       const dsx_diffnet_params* grads, float* d_cond, int B, int T, void* workspace,
+                       size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
