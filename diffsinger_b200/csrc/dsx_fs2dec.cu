@@ -60,6 +60,11 @@ struct Fs2ConvArgs {
   __half* ln16;                // [B][T][n] LayerNorm output, every row < T
   float* out;                  // non-null: LayerNorm * !pad -> out [B][T][n] fp32 instead of ln16
   int mask16;                  // with ln16: LayerNorm * !pad (the FFT denoiser's get_mel_out operand)
+  // training forward (Fs2Train); drop.site < 0 and null pointers otherwise
+  Fs2Drop drop;                // F2_FFN1: dropout after the activation; F2_RES: dropout of the GEMM output + bias
+  __half* vrow;                // F2_QKV: V as [B][heads][T][D] as well
+  __half* z16;                 // F2_FFN1: the activation's input [B][T][n]
+  float* xsave;                // F2_RES: a copy of the updated residual stream [B][T][n]
 };
 
 template <int NT>
@@ -99,6 +104,8 @@ __global__ void __launch_bounds__(128 * Fs2Shape<NT>::WG) k_fs2_conv(const Fs2Co
         __half* v = p.vt + (bh * p.D + d) * p.Tp + m;
         v[0] = __float2half_rn(acc[e]);
         v[p.Tp] = __float2half_rn(acc[e + 1]);
+        if (p.vrow && m < T)
+          *reinterpret_cast<__half2*>(p.vrow + (bh * T + m) * p.D + d) = __floats2half2_rn(acc[e], acc[e + 1]);
       } else {
         if (m >= T) continue;
         const float s = part == 0 ? p.qscale : 1.f;
@@ -114,11 +121,17 @@ __global__ void __launch_bounds__(128 * Fs2Shape<NT>::WG) k_fs2_conv(const Fs2Co
     for (int e = 0; e < NH / 2; e += 2) {
       const int col = c0 + acc_col(wtid, e), m = mrow[(e >> 1) & 1];
       if (col >= n || m >= T) continue;
-      float v[2];
+      float v[2], y[2];
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        const float y = (acc[e + i] + __ldg(p.g.b + col + i)) * p.ffn_scale;
-        v[i] = p.relu ? fmaxf(y, 0.f) : 0.5f * y * (1.f + erff(y * 0.70710678118654752f));
+        y[i] = (acc[e + i] + __ldg(p.g.b + col + i)) * p.ffn_scale;
+        v[i] = p.relu ? fmaxf(y[i], 0.f) : 0.5f * y[i] * (1.f + erff(y[i] * 0.70710678118654752f));
+      }
+      if (p.z16) {
+        *reinterpret_cast<__half2*>(p.z16 + (rbase + m) * n + col) = __floats2half2_rn(y[0], y[1]);
+        const float2 ds = dropout_scale2(p.drop, rbase + m, col);
+        v[0] *= ds.x;
+        v[1] *= ds.y;
       }
       *reinterpret_cast<__half2*>(p.o16 + (rbase + m) * n + col) = __floats2half2_rn(v[0], v[1]);
     }
@@ -149,10 +162,19 @@ __global__ void __launch_bounds__(128 * Fs2Shape<NT>::WG) k_fs2_conv(const Fs2Co
     if (col < n && keep[r]) {
       float* xp = p.xres + (rbase + m) * n + col;
       const float2 xo = *reinterpret_cast<const float2*>(xp);
-      v0 = xo.x + (acc[e] + __ldg(p.g.b + col));
-      v1 = xo.y + (acc[e + 1] + __ldg(p.g.b + col + 1));
+      if (p.drop.site >= 0) {
+        const float2 ds = dropout_scale2(p.drop, rbase + m, col);
+        v0 = xo.x + (acc[e] + __ldg(p.g.b + col)) * ds.x;
+        v1 = xo.y + (acc[e + 1] + __ldg(p.g.b + col + 1)) * ds.y;
+      } else {
+        v0 = xo.x + (acc[e] + __ldg(p.g.b + col));
+        v1 = xo.y + (acc[e + 1] + __ldg(p.g.b + col + 1));
+      }
     }
-    if (col < n && m < T) *reinterpret_cast<float2*>(p.xres + (rbase + m) * n + col) = make_float2(v0, v1);
+    if (col < n && m < T) {
+      *reinterpret_cast<float2*>(p.xres + (rbase + m) * n + col) = make_float2(v0, v1);
+      if (p.xsave) *reinterpret_cast<float2*>(p.xsave + (rbase + m) * n + col) = make_float2(v0, v1);
+    }
     acc[e] = v0;
     acc[e + 1] = v1;
   }
@@ -194,14 +216,15 @@ __global__ void __launch_bounds__(128 * Fs2Shape<NT>::WG) k_fs2_conv(const Fs2Co
 // through two cp.async stages in the 128-byte-swizzled layout; S = Q K^T and O += P V run on wgmma with both operands in
 // shared memory (P rounded to fp16 through a swizzled tile).  Padding keys and keys at or past T get -inf; the softmax
 // state (running max and sum per row) is fp32.  A row whose keys are all padding has sum 0 and is written as 0 (the
-// reference's 0 / 0 gives NaN there).
+// reference's 0 / 0 gives NaN there).  With lse (the training forward), the row's log-sum-exp max + log(sum) goes to
+// lse [B][heads][T], +inf for a row with no valid key.
 template <int D>
 constexpr int attn_smem() { return 64 * D * 2 * 3 + D * 64 * 2 * 2 + 64 * 64 * 2 + 1024; }
 
 template <int D>
 __global__ void __launch_bounds__(128) k_fs2_attn(const __half* __restrict__ q, const __half* __restrict__ k,
                                                  const __half* __restrict__ vt, const uint8_t* __restrict__ pad, int T,
-                                                 int Tp, int heads, __half* __restrict__ o) {
+                                                 int Tp, int heads, __half* __restrict__ o, float* __restrict__ lse) {
   constexpr int kQ = 64 * D * 2, kV = D * 64 * 2;   // bytes of a 64 x D tile (Q, K) and of a D x 64 tile (V^T)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -322,6 +345,13 @@ __global__ void __launch_bounds__(128) k_fs2_attn(const __half* __restrict__ q, 
   }
 
   const int H = heads * D;
+  if (lse && (tid & 3) == 0) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int m = m0 + acc_row(tid, 2 * r);
+      if (m < T) lse[bh * T + m] = lrun[r] > 0.f ? mrun[r] + logf(lrun[r]) : INFINITY;
+    }
+  }
 #pragma unroll
   for (int e = 0; e < D / 2; e += 2) {
     const int r = (e >> 1) & 1, m = m0 + acc_row(tid, e);
@@ -351,9 +381,11 @@ __global__ void k_fs2_pack(const float* x, dsx_strides xs, int B, int T, int H, 
 }
 
 // X = (X + alpha * table[pos]) * !pad (tts_modules.py:290-295), then LayerNorm (layer 0's layer_norm1) -> fp16 A.
-// One warp per frame, H / 32 <= 8 channels per lane.
+// One warp per frame, H / 32 <= 8 channels per lane.  Training: dropout (site `drop`) before the mask, and X copied to
+// xsave.
 __global__ void k_fs2_embed(float* X, const int* pos, const uint8_t* pad, const float* alpha, int rows, int H,
-                            float neg_emb, const float* ln_w, const float* ln_b, __half* A) {
+                            float neg_emb, const float* ln_w, const float* ln_b, __half* A, Fs2Drop drop,
+                            float* xsave) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= rows) return;
   const int ps = pos[warp], per = H / 32;
@@ -364,9 +396,11 @@ __global__ void k_fs2_embed(float* X, const int* pos, const uint8_t* pad, const 
   for (int i = 0; i < 8; ++i) {
     if (i >= per) break;
     const int c = lane + 32 * i;
-    const float y = xr[c] + alpha[0] * pos_table(ps, c, H, neg_emb);
+    float y = xr[c] + alpha[0] * pos_table(ps, c, H, neg_emb);
+    if (drop.site >= 0) y *= dropout_scale(drop, warp, c);
     v[i] = keep ? y : 0.f;
     xr[c] = v[i];
+    if (xsave) xsave[static_cast<size_t>(warp) * H + c] = v[i];
   }
   warp_row_ln16(v, per, H, kFs2LnEps, ln_w, ln_b, A + static_cast<size_t>(warp) * H);
 }
@@ -476,16 +510,18 @@ Fs2Bufs fs2_carve(const dsx_fs2dec* h, void* base, int B, int T) {
 
 int fs2_layers(const dsx_fs2dec* h) { return h->cfg.layers; }
 
-int fs2_stack_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s) {
+int fs2_stack_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s,
+                  const Fs2Train* tr) {
   const int H = h->cfg.hidden;
   const size_t frames = static_cast<size_t>(B) * T;
   const unsigned row_blocks = static_cast<unsigned>((frames * 32 + 255) / 256);
   k_pos_scan<<<B, kScanThreads, 0, s>>>(w.X, T, H, w.POS);
   DSX_TRY(launch_check("k_pos_scan"));
   k_fs2_embed<<<row_blocks, 256, 0, s>>>(w.X, w.POS, w.PAD, h->alpha, static_cast<int>(frames), H, pos_neg_emb(H),
-                                         h->layers[0].ln1_w, h->layers[0].ln1_b, w.A);
+                                         h->layers[0].ln1_w, h->layers[0].ln1_b, tr ? tr->a1[0] : w.A,
+                                         tr ? tr->drop(0) : Fs2Drop{}, tr ? tr->xin[0] : nullptr);
   DSX_TRY(launch_check("k_fs2_embed"));
-  return fs2_layers_run(h, w, B, T, out, out16, s);
+  return fs2_layers_run(h, w, B, T, out, out16, s, tr);
 }
 
 void fs2_first_ln(const dsx_fs2dec* h, const float** w, const float** b) {
@@ -493,7 +529,8 @@ void fs2_first_ln(const dsx_fs2dec* h, const float** w, const float** b) {
   *b = h->layers[0].ln1_b;
 }
 
-int fs2_layers_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s) {
+int fs2_layers_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s,
+                   const Fs2Train* tr) {
   const dsx_fs2dec_config& c = h->cfg;
   const int H = c.hidden, L = c.layers, heads = c.heads, D = H / heads;
   const int mtiles = (T + kConvRows - 1) / kConvRows, Tp = mtiles * kConvRows;
@@ -508,44 +545,65 @@ int fs2_layers_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* o
   base.xres = w.X;
   for (int i = 0; i < L; ++i) {
     const dsx_fs2dec::Layer& l = h->layers[i];
+    // the training forward keeps the GEMM operands on its tape; evaluation reuses the workspace's
+    __half* A1 = tr ? tr->a1[i] : w.A;
+    __half* A2 = tr ? tr->a2[i] : w.A;
+    __half* Q = tr ? tr->q[i] : w.Q;
+    __half* K = tr ? tr->k[i] : w.K;
+    __half* O = tr ? tr->o[i] : w.O;
+    __half* Fh = tr ? tr->hd[i] : w.F;
+    float* lse = tr ? tr->lse[i] : nullptr;
     // self-attention block (common_layers.py:569-580): x = (x + out_proj(MHA(LN1(x)))) * !pad
     Fs2ConvArgs a = base;
-    a.x = w.A;
+    a.x = A1;
     a.mode = F2_QKV;
     a.qscale = static_cast<float>(sqrt(1.0 / D));   // math.sqrt(1 / head_dim) of F.multi_head_attention_forward
-    a.q = w.Q;
-    a.k = w.K;
+    a.q = Q;
+    a.k = K;
     a.vt = w.VT;
+    if (tr) a.vrow = tr->v[i];
     DSX_TRY(f2_run(l.qkv, a, B, s));
     const dim3 agrid(mtiles, heads, B);
     if (D == 64) {
-      k_fs2_attn<64><<<agrid, 128, attn_smem<64>(), s>>>(w.Q, w.K, w.VT, w.PAD, T, Tp, heads, w.O);
+      k_fs2_attn<64><<<agrid, 128, attn_smem<64>(), s>>>(Q, K, w.VT, w.PAD, T, Tp, heads, O, lse);
     } else {
-      k_fs2_attn<128><<<agrid, 128, attn_smem<128>(), s>>>(w.Q, w.K, w.VT, w.PAD, T, Tp, heads, w.O);
+      k_fs2_attn<128><<<agrid, 128, attn_smem<128>(), s>>>(Q, K, w.VT, w.PAD, T, Tp, heads, O, lse);
     }
     DSX_TRY(launch_check("k_fs2_attn"));
     a = base;
-    a.x = w.O;
+    a.x = O;
     a.mode = F2_RES;
     a.ln_w = l.ln2_w;
     a.ln_b = l.ln2_b;
-    a.ln16 = w.A;
+    a.ln16 = A2;
+    if (tr) {
+      a.drop = tr->drop(1 + 3 * i);
+      a.xsave = tr->xin[2 * i + 1];
+    }
     DSX_TRY(f2_run(l.out, a, B, s));
     // FFN block (:582-587, TransformerFFNLayer :503-522): x = (x + ffn_2(act(ffn_1(LN2(x)) * k^-0.5))) * !pad
     a = base;
-    a.x = w.A;
+    a.x = A2;
     a.mode = F2_FFN1;
     a.ffn_scale = static_cast<float>(pow(static_cast<double>(c.kernel), -0.5));
     a.relu = c.act;
-    a.o16 = w.F;
+    a.o16 = Fh;
+    if (tr) {
+      a.drop = tr->drop(2 + 3 * i);
+      a.z16 = tr->z[i];
+    }
     DSX_TRY(f2_run(l.ffn1, a, B, s));
     a = base;
-    a.x = w.F;
+    a.x = Fh;
     a.mode = F2_RES;
+    if (tr) {
+      a.drop = tr->drop(3 + 3 * i);
+      a.xsave = tr->xin[2 * i + 2];
+    }
     if (i + 1 < L) {
       a.ln_w = h->layers[i + 1].ln1_w;
       a.ln_b = h->layers[i + 1].ln1_b;
-      a.ln16 = w.A;
+      a.ln16 = tr ? tr->a1[i + 1] : w.A;
     } else {   // tts_modules.py:300-301: layer_norm(x) * !pad
       a.ln_w = h->lnf_w;
       a.ln_b = h->lnf_b;
@@ -632,6 +690,75 @@ int fs2_load(dsx_fs2dec* h, const dsx_fs2dec_params* p, void* stream) {
   return DSX_OK;
 }
 
+int fs2_forward_run(const dsx_fs2dec* h, const float* x, dsx_strides xs, int B, int T, const Fs2Bufs& w, float* out,
+                    cudaStream_t s, const Fs2Train* tr) {
+  const size_t frames = static_cast<size_t>(B) * T;
+  k_fs2_pack<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(x, xs, B, T, h->cfg.hidden, w.X, w.PAD);
+  DSX_TRY(launch_check("k_fs2_pack"));
+  return fs2_stack_run(h, w, B, T, out, nullptr, s, tr);
+}
+
+const dsx_fs2dec_config& fs2_config(const dsx_fs2dec* h) { return h->cfg; }
+
+namespace {
+// g's tile shape as f2_pack gives it, with its packs allocated but not filled
+int f2_alloc(dsx_fs2dec* h, ConvGemm& g, int cin, int n, int k, int tap0) {
+  g.cin = cin;
+  g.n = n;
+  g.taps = k;
+  g.tap0 = tap0;
+  g.nt = conv_nt(n, 256);
+  g.ntiles = (n + g.nt - 1) / g.nt;
+  g.kc = (k * cin + 63) / 64;
+  DSX_TRY(h->mem.alloc(&g.w, static_cast<size_t>(g.ntiles) * g.kc * g.nt * 64 * sizeof(__half)));
+  return h->mem.alloc(&g.b, static_cast<size_t>(g.ntiles) * g.nt * sizeof(float));
+}
+
+int f2_refill(const ConvGemm& g, const float* w, const float* b, int k, const char* what, int layer, cudaStream_t s) {
+  DSX_CHECK(w, DSX_E_INVALID, "missing %s weight of layer %d", what, layer);
+  const size_t nw = static_cast<size_t>(g.ntiles) * g.kc * g.nt * 64;
+  k_pack_conv<<<static_cast<unsigned>(std::min<size_t>((nw + 255) / 256, 4096)), 256, 0, s>>>(
+      g, PackArgs{w, nullptr, b, g.cin, g.n, g.n, k, 1, 0});
+  return launch_check("k_pack_conv");
+}
+}  // namespace
+
+int fs2_train_alloc(dsx_fs2dec* h) {
+  const dsx_fs2dec_config& c = h->cfg;
+  const int H = c.hidden, L = c.layers, k = c.kernel;
+  const int tap0 = c.padding ? -(k - 1) : -(k / 2);
+  h->layers.assign(L, dsx_fs2dec::Layer{});
+  for (int i = 0; i < L; ++i) {
+    dsx_fs2dec::Layer& l = h->layers[i];
+    DSX_TRY(f2_alloc(h, l.qkv, H, 3 * H, 1, 0));
+    DSX_TRY(f2_alloc(h, l.out, H, H, 1, 0));
+    DSX_TRY(f2_alloc(h, l.ffn1, H, 4 * H, k, tap0));
+    DSX_TRY(f2_alloc(h, l.ffn2, 4 * H, H, 1, 0));
+  }
+  return DSX_OK;
+}
+
+int fs2_train_pack(dsx_fs2dec* h, const dsx_fs2dec_params* p, cudaStream_t s) {
+  const dsx_fs2dec_config& c = h->cfg;
+  const int L = c.layers;
+  for (int i = 0; i < L; ++i) {
+    dsx_fs2dec::Layer& l = h->layers[i];
+    DSX_TRY(f2_refill(l.qkv, p->in_proj_w[i], nullptr, 1, "self_attn.in_proj", i, s));
+    DSX_TRY(f2_refill(l.out, p->out_proj_w[i], nullptr, 1, "self_attn.out_proj", i, s));
+    DSX_TRY(f2_refill(l.ffn1, p->ffn1_w[i], p->ffn1_b[i], c.kernel, "ffn.ffn_1", i, s));
+    DSX_TRY(f2_refill(l.ffn2, p->ffn2_w[i], p->ffn2_b[i], 1, "ffn.ffn_2", i, s));
+    l.ln1_w = const_cast<float*>(p->ln1_w[i]);
+    l.ln1_b = const_cast<float*>(p->ln1_b[i]);
+    l.ln2_w = const_cast<float*>(p->ln2_w[i]);
+    l.ln2_b = const_cast<float*>(p->ln2_b[i]);
+  }
+  h->lnf_w = const_cast<float*>(p->ln_w);
+  h->lnf_b = const_cast<float*>(p->ln_b);
+  h->alpha = const_cast<float*>(p->pos_embed_alpha);
+  h->loaded = true;
+  return DSX_OK;
+}
+
 }  // namespace dsx
 
 extern "C" {
@@ -649,11 +776,7 @@ int dsx_fs2dec_forward(dsx_fs2dec* h, const float* x, dsx_strides xs, int B, int
   DSX_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   DSX_TRY(h->ws.reserve(fs2_workspace_bytes(h, B, T), s));
-  const Fs2Bufs w = fs2_carve(h, h->ws.ptr, B, T);
-  const size_t frames = static_cast<size_t>(B) * T;
-  k_fs2_pack<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(x, xs, B, T, H, w.X, w.PAD);
-  DSX_TRY(launch_check("k_fs2_pack"));
-  return fs2_stack_run(h, w, B, T, out, nullptr, s);
+  return fs2_forward_run(h, x, xs, B, T, fs2_carve(h, h->ws.ptr, B, T), out, s);
 }
 
 }  // extern "C"

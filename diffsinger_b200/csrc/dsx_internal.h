@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "../../include/dsx.h"
+#include "dsx_rng.cuh"
 
 namespace dsx {
 
@@ -352,10 +353,41 @@ size_t fs2_workspace_bytes(const dsx_fs2dec* h, int B, int T);
 Fs2Bufs fs2_carve(const dsx_fs2dec* h, void* ws, int B, int T);   // ws: fs2_workspace_bytes(h, B, T) bytes
 // the decoder's entry -- positions over channel 0, X = (X + alpha * table[pos]) * !pad and LN1 of layer 0 -> A -- then
 // fs2_layers_run.  2 + 5 L launches.
-int fs2_stack_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s);
+// What the training step's forward (dsx_fs2train.cu) saves, and its dropout: site 0 at the entry, then per layer i sites
+// 1 + 3 i (after out_proj), 2 + 3 i (after the FFN activation) and 3 + 3 i (after ffn_2).  Every pointer is a tape region.
+struct Fs2Train {
+  uint64_t seed = 0;
+  float p = 0.f;
+  std::vector<float*> xin;                          // LayerNorm inputs [F][H]: LN1 of layer i at 2 i, LN2 at 2 i + 1,
+                                                    // the final LayerNorm at 2 L
+  std::vector<__half*> a1, a2, q, k, v, o, z, hd;   // per layer: LN1 and LN2 outputs [F][H]; Q (scaled), K, V
+                                                    // [B][heads][T][D]; attention output [F][H]; ffn_1 output * k^-0.5
+                                                    // before the activation and the ffn_2 input after dropout [F][4H]
+  std::vector<float*> lse;                          // per layer: softmax log-sum-exp [B][heads][T] (+inf: no key)
+  Fs2Drop drop(int site) const {
+    Fs2Drop d;
+    d.seed = seed;
+    d.p = p;
+    d.inv_keep = 1.f / (1.f - p);
+    d.site = site;
+    return d;
+  }
+};
+int fs2_stack_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s,
+                  const Fs2Train* tr = nullptr);
+// k_fs2_pack of x (any strides) into w.X and w.PAD, then fs2_stack_run
+int fs2_forward_run(const dsx_fs2dec* h, const float* x, dsx_strides xs, int B, int T, const Fs2Bufs& w, float* out,
+                    cudaStream_t s, const Fs2Train* tr = nullptr);
+// The training step's packs: fs2_train_alloc sizes and allocates them once; fs2_train_pack refills them from the
+// caller's fp32 weights on the stream (no allocation, no synchronisation) and points the LayerNorm affines and
+// pos_embed_alpha at the caller's arrays.
+int fs2_train_alloc(dsx_fs2dec* h);
+int fs2_train_pack(dsx_fs2dec* h, const dsx_fs2dec_params* p, cudaStream_t s);
+const dsx_fs2dec_config& fs2_config(const dsx_fs2dec* h);
 // the L layers from X (masked), PAD and A = LN1 of layer 0 (fp16), then the final LayerNorm * !pad: to out [B][T][H] fp32,
 // or (out == NULL) to out16 as fp16.  5 L launches.
-int fs2_layers_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s);
+int fs2_layers_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s,
+                   const Fs2Train* tr = nullptr);
 int fs2_layers(const dsx_fs2dec* h);
 void fs2_first_ln(const dsx_fs2dec* h, const float** w, const float** b);   // layer 0's layer_norm1 (device)
 // dsx_fs2dec_load with pos_embed_alpha optional (the encoder's FFTBlocks have none)

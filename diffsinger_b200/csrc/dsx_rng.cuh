@@ -58,4 +58,35 @@ __device__ __forceinline__ size_t mel_noise_block(int b, int m, int t, int M, in
   return (static_cast<size_t>(b) * (M >> 2) + (m >> 2)) * T + t;
 }
 
+// ------------------------------------------------------------------------------------------
+// Dropout masks of the training steps: element (frame, channel) of dropout site `site` is kept when the 24-bit uniform u
+// of lane channel % 4 of the Philox4x32-10 block (channel / 4, frame, site, 0) under key seed is >= p, so
+// P(keep) = 1 - p to 2^-24 (torch's distribution, not its stream).  Kept elements are scaled by inv_keep = 1 / (1 - p).
+// ------------------------------------------------------------------------------------------
+struct Fs2Drop {
+  uint64_t seed = 0;
+  float p = 0.f, inv_keep = 1.f;
+  int site = -1;                 // < 0: no dropout (scale 1)
+};
+__device__ __forceinline__ uint4 dropout_block(const Fs2Drop& d, size_t frame, int channel) {
+  const uint4 ctr = make_uint4(static_cast<uint32_t>(channel >> 2), static_cast<uint32_t>(frame),
+                               static_cast<uint32_t>(d.site), static_cast<uint32_t>(frame >> 32));
+  return philox4x32_10(ctr, make_uint2(static_cast<uint32_t>(d.seed), static_cast<uint32_t>(d.seed >> 32)));
+}
+__device__ __forceinline__ float dropout_lane(const Fs2Drop& d, const uint4& r, int lane) {
+  const uint32_t v = lane == 0 ? r.x : lane == 1 ? r.y : lane == 2 ? r.z : r.w;
+  return static_cast<float>(v >> 8) * 5.9604644775390625e-8f >= d.p ? d.inv_keep : 0.f;
+}
+// the factor of element (frame, channel): 0 or inv_keep, or 1 without dropout
+__device__ __forceinline__ float dropout_scale(const Fs2Drop& d, size_t frame, int channel) {
+  if (d.site < 0) return 1.f;
+  return dropout_lane(d, dropout_block(d, frame, channel), channel & 3);
+}
+// the factors of channels c and c + 1 (c even)
+__device__ __forceinline__ float2 dropout_scale2(const Fs2Drop& d, size_t frame, int c) {
+  if (d.site < 0) return make_float2(1.f, 1.f);
+  const uint4 r = dropout_block(d, frame, c);
+  return make_float2(dropout_lane(d, r, c & 3), dropout_lane(d, r, (c & 3) + 1));
+}
+
 }  // namespace dsx

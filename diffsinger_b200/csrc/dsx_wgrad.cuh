@@ -1,0 +1,162 @@
+// Training helpers shared by the DiffNet (dsx_train.cu) and FastSpeech2 decoder (dsx_fs2train.cu) training steps: the
+// weight-gradient GEMM over the frame axis with its fixed-order split (k_wgrad), and the device-chosen power-of-two
+// gradient scale (k_amax, k_scale).
+#pragma once
+#include <algorithm>
+
+#include "dsx_internal.h"
+#include "dsx_ptx.cuh"
+
+namespace dsx {
+namespace {   // every translation unit has its own copies, like dsx_conv.cuh
+
+constexpr int kWgThreads = 256;
+
+// ---- weight gradients: D[m][n] = sum over frames f of A[f][m] B[f + shift][n], both operands MN-major ----------------
+struct WgradArgs {
+  const __half* a;             // [F][lda], output rows m are its columns [0, am)
+  int lda, am;
+  const __half* b[4];          // per 256-column tile (blockIdx.y): source [F][ldb], shift in frames, valid columns
+  int ldb[4], shift[4], bn[4];
+  int F, T, fchunk;            // frames, frames per utterance, frames per split (a multiple of 64)
+  float* part;                 // [splits][Mpad][Ntot]
+  float* bpart;                // [splits][Mpad] column sums of A (blockIdx.y == 0), or null
+  int Mpad, Ntot;
+};
+
+constexpr int kWgA = 64 * 128, kWgB = 64 * 128 * 4, kWgStage = kWgA + kWgB;
+constexpr int kWgSmem = 2 * kWgStage + 1024;
+
+__global__ void __launch_bounds__(kWgThreads) k_wgrad(const WgradArgs p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  __shared__ float bsum[2][64];
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const int mt = blockIdx.x, nt = blockIdx.y, split = blockIdx.z;
+  const int f_begin = split * p.fchunk, f_end = min(p.F, f_begin + p.fchunk);
+  const int chunks = (f_end - f_begin + 63) / 64;
+  const __half* bsrc = p.b[nt];
+  const int ldb = p.ldb[nt], shift = p.shift[nt], bn = p.bn[nt];
+
+  auto load = [&](int s, uint8_t* buf) {
+    const uint32_t da = smem_u32(buf), db = smem_u32(buf + kWgA);
+    const int f0 = f_begin + s * 64;
+    for (int i = tid; i < 64 * 8; i += kWgThreads) {          // A: 64 frames x 64 rows of the output
+      const int k = i >> 3, c = i & 7, f = f0 + k, m = mt * 64 + c * 8;
+      const bool ok = f < f_end && m < p.am;
+      cp16(da + sw128(k, c), p.a + (ok ? static_cast<size_t>(f) * p.lda + m : 0), ok);
+    }
+    for (int i = tid; i < 64 * 32; i += kWgThreads) {         // B: 64 frames x 256 columns, four 64-column atoms
+      const int k = i >> 5, c = i & 31, f = f0 + k, n = c * 8;
+      bool ok = f < f_end && n < bn;
+      int src = f + shift;
+      if (ok && shift != 0) {
+        const int t = f % p.T + shift;
+        ok = t >= 0 && t < p.T;
+      }
+      cp16(db + (c >> 3) * 8192 + sw128(k, c & 7), bsrc + (ok ? static_cast<size_t>(src) * ldb + n : 0), ok);
+    }
+  };
+
+  float acc[64];
+#pragma unroll
+  for (int e = 0; e < 64; ++e) acc[e] = 0.f;
+  float bs = 0.f;                                              // column sum of A: thread tid < 128, row tid & 63
+  if (chunks > 0) {
+    load(0, smem);
+    cp_commit();
+  }
+#pragma unroll 1
+  for (int s = 0; s < chunks; ++s) {
+    uint8_t* cur = smem + (s & 1) * kWgStage;
+    if (s + 1 < chunks) {
+      load(s + 1, smem + ((s + 1) & 1) * kWgStage);
+      cp_commit();
+      cp_wait<1>();
+    } else {
+      cp_wait<0>();
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    const uint32_t ua = smem_u32(cur), ub = smem_u32(cur + kWgA + wg * 2 * 8192);
+    wg_fence();
+#pragma unroll
+    for (int k4 = 0; k4 < 4; ++k4)
+      wgmma_n128_mn(acc, wg_desc_mn(ua + k4 * 2048, 8192), wg_desc_mn(ub + k4 * 2048, 8192), 1);
+    wg_commit();
+    if (p.bpart && nt == 0 && tid < 128) {
+      const int m = tid & 63, k0 = (tid >> 6) * 32;
+#pragma unroll 8
+      for (int k = k0; k < k0 + 32; ++k)
+        bs += __half2float(*reinterpret_cast<const __half*>(cur + sw128(k, m >> 3) + (m & 7) * 2));
+    }
+    wg_wait0();
+#pragma unroll
+    for (int e = 0; e < 64; ++e) asm volatile("" : "+f"(acc[e])::"memory");
+    __syncthreads();
+  }
+  const int wtid = tid & 127;
+  float* out = p.part + (static_cast<size_t>(split) * p.Mpad + mt * 64) * p.Ntot + nt * 256 + wg * 128;
+#pragma unroll
+  for (int e = 0; e < 64; e += 2) {
+    const int r = acc_row(wtid, e), c = acc_col(wtid, e);
+    *reinterpret_cast<float2*>(out + static_cast<size_t>(r) * p.Ntot + c) = make_float2(acc[e], acc[e + 1]);
+  }
+  if (p.bpart && nt == 0) {
+    if (tid < 128) bsum[tid >> 6][tid & 63] = bs;
+    __syncthreads();
+    if (tid < 64) p.bpart[static_cast<size_t>(split) * p.Mpad + mt * 64 + tid] = bsum[0][tid] + bsum[1][tid];
+  }
+}
+
+// ---- gradient scale: S from amax |g| ---------------------------------------------------------------------------------
+__global__ void k_amax(const float* g, size_t n, unsigned* amax_bits) {
+  float m = 0.f;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    m = fmaxf(m, fabsf(g[i]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) atomicMax(amax_bits, __float_as_uint(m));   // max of non-negative floats: order-free
+}
+
+// scal[0] = S, scal[1] = 1 / S: S * amax in [2^5, 2^6); S = 1 when amax is 0 or not finite
+__global__ void k_scale(const unsigned* amax_bits, float* scal) {
+  const float a = __uint_as_float(*amax_bits);
+  int e = 0;
+  if (a > 0.f && isfinite(a)) {
+    frexpf(a, &e);                        // a in [2^(e-1), 2^e)
+    e = min(max(6 - e, -126), 126);
+  }
+  scal[0] = ldexpf(1.f, e);
+  scal[1] = ldexpf(1.f, -e);
+}
+
+int sm_count(int device) {
+  int n = 0;
+  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device);
+  return n > 0 ? n : 132;
+}
+
+// frames per split of a wgrad over F frames with `tiles` output tiles: about two CTAs per SM in all
+int wgrad_fchunk(int F, int tiles, int device) {
+  const int fch = (F + 63) / 64;
+  const int sp = std::max(1, std::min(fch, (2 * sm_count(device) + tiles - 1) / tiles));
+  return ((fch + sp - 1) / sp) * 64;
+}
+
+// partials of D[am x ntiles*256] = A^T B over F frames, one [Mpad][Ntot] slab per split
+int run_wgrad(WgradArgs a, int ntiles, int device, float* part, float* bpart, cudaStream_t s) {
+  const int mtiles = (a.am + 63) / 64;
+  a.fchunk = wgrad_fchunk(a.F, mtiles * ntiles, device);
+  const int sp = (a.F + a.fchunk - 1) / a.fchunk;
+  a.part = part;
+  a.bpart = bpart;
+  a.Mpad = mtiles * 64;
+  a.Ntot = ntiles * 256;
+  k_wgrad<<<dim3(mtiles, ntiles, sp), kWgThreads, kWgSmem, s>>>(a);
+  return launch_check("k_wgrad");
+}
+
+}  // namespace
+}  // namespace dsx

@@ -4,8 +4,10 @@
 reference's constructor, submodule names, parameter and buffer shapes (modules/fastspeech/tts_modules.py:251-357 with
 modules/commons/common_layers.py:166-588), so the decoder of a FastSpeech2 checkpoint loads with ``strict=True``.  The
 modules only hold the parameters: ``forward`` packs them into the library (once per storage and version, so again after
-``load_state_dict`` or ``.to()``) and runs the whole decoder there.  There is no eager or CPU path and no training path:
-a CPU tensor or a module in training mode raises ``DsxError``.
+``load_state_dict`` or ``.to()``) and runs the whole decoder there.  There is no eager or CPU path: a CPU tensor raises
+``DsxError``.  A module in training mode raises ``DsxError`` too, unless the ``dsx_train`` opt-in (hparams key or
+``train=`` keyword) is set: then a training-mode forward under autograd runs the sm_90a training step of
+``diffsinger_b200.fs2train`` (dropout p = hparams['dropout'], gradients for every parameter and for x).
 """
 import torch
 import torch.nn as nn
@@ -107,7 +109,7 @@ def fs2dec_params(num_layers, padding, t, arr, alpha=True):
 
 
 class FastspeechDecoder(PackedModule):
-    def __init__(self, hidden_size=None, num_layers=None, kernel_size=None, num_heads=None, *, hparams=None):
+    def __init__(self, hidden_size=None, num_layers=None, kernel_size=None, num_heads=None, *, hparams=None, train=None):
         super().__init__()
         hp = _get_hparams(hparams)
         num_heads = hp['num_heads'] if num_heads is None else num_heads          # tts_modules.py:352-355
@@ -118,13 +120,29 @@ class FastspeechDecoder(PackedModule):
         self._cfg = _fs2dec_config(hidden_size, num_layers, kernel_size, num_heads, padding, act)
         self.hidden_size, self.num_layers, self.num_heads = self._cfg.hidden, self._cfg.layers, self._cfg.heads
         self.kernel_size, self.padding, self.act = self._cfg.kernel, padding, act
-        self.dropout = hp.get('dropout', 0.0)      # identity in eval mode, the only mode forward runs in
+        self.dropout = hp.get('dropout', 0.0)      # identity in eval mode; the training step's p under dsx_train
         self.padding_idx = 0
         self.pos_embed_alpha = nn.Parameter(torch.Tensor([1]))
         self.embed_positions = SinusoidalPositionalEmbedding(self.hidden_size, self.padding_idx)
         self.layers = nn.ModuleList([TransformerEncoderLayer(self.hidden_size, self.kernel_size, self.num_heads, padding, act)
                                      for _ in range(self.num_layers)])
         self.layer_norm = nn.LayerNorm(self.hidden_size)
+        self._dsx_train = bool(train if train is not None else hp.get("dsx_train", False))
+        self._dsx_trainer = None
+
+    def __getstate__(self):
+        # the library handles are ctypes pointers: copies (EMA deepcopy, torch.save of the module) make their own
+        state = self.__dict__.copy()
+        state["_dsx"], state["_wkey"], state["_keep"] = None, None, None
+        state["_dsx_trainer"] = None
+        return state
+
+    def _dsx_train_step(self):
+        if self._dsx_trainer is None:
+            from .fs2train import Fs2DecTrainStep
+            object.__setattr__(self, "_dsx_trainer", Fs2DecTrainStep(_fs2dec_config(
+                self.hidden_size, self.num_layers, self.kernel_size, self.num_heads, self.padding, self.act)))
+        return self._dsx_trainer
 
     # -- library handle ---------------------------------------------------------------------------
     _lib_create, _lib_load, _lib_destroy = lib.dsx_fs2dec_create, lib.dsx_fs2dec_load, lib.dsx_fs2dec_destroy
@@ -143,6 +161,9 @@ class FastspeechDecoder(PackedModule):
                            "supported (the padding mask is derived from x, as at inference)")
         if x is None or x.dim() != 3 or x.shape[-1] != self.hidden_size:
             raise DsxError(f"x must be [B, T, {self.hidden_size}] (got {None if x is None else tuple(x.shape)})")
+        if self.training and self._dsx_train and torch.is_grad_enabled():
+            from .fs2train import fs2dec_train_forward
+            return fs2dec_train_forward(self, x)
         if self.training:
             raise DsxError("the dsx FastSpeech2 decoder runs in eval mode only (call .eval()); training stays with the "
                            "reference's modules")

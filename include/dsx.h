@@ -621,6 +621,57 @@ int dsx_train_backward(dsx_train* h, const dsx_diffnet_params* w, const void* ta
                        const dsx_diffnet_params* grads, float* d_cond, int B, int T, void* workspace,
                        size_t workspace_bytes, void* stream);
 
+/* ---- FastSpeech2 decoder training step ------------------------------------------------------------------------------
+ * Replaces: FFTBlocks.forward(x) of FastspeechDecoder in training mode (tts_modules.py:282-307, EncSALayer of
+ * common_layers.py:542-588) and its autograd backward.  Dropout p at the reference's 1 + 3 L sites, in this order: site
+ * 0 after x + alpha * positions (before * !pad); per layer i, site 1 + 3 i after out_proj, 2 + 3 i after the FFN
+ * activation ([B, T, 4H]) and 3 + 3 i after ffn_2; attention probabilities have none (attention_dropout = 0).  Masks come
+ * from Philox4x32-10 keyed by (seed, site, frame, channel): the same seed and p give the same masks, with torch's
+ * distribution (keep 1 - p, kept values scaled by 1 / (1 - p)) but not its stream.  fp16 operands, fp32 accumulation,
+ * LayerNorm statistics, softmax state and residual streams; the backward's fp16 operands are scaled by a power of two S
+ * chosen on the device (S amax |d_out| in [2^5, 2^6)), divided out exactly, so 2^k d_out gives exactly 2^k times the
+ * gradients.  Gradients are bitwise reproducible (fixed-order reductions, no atomics).  No call allocates or synchronises
+ * the host: the tape and the workspace are the caller's.  A handle is independent of the other handles. */
+typedef struct dsx_fs2dec_train dsx_fs2dec_train;
+
+/* Accepts what dsx_fs2dec_create accepts (DSX_E_INVALID, "unsupported ..."). */
+int dsx_fs2dec_train_create(int device, const dsx_fs2dec_config* cfg, dsx_fs2dec_train** out);
+void dsx_fs2dec_train_destroy(dsx_fs2dec_train* h);
+
+/* Bytes of the tape of one forward over B utterances of T frames (F = B T, H = hidden, L = layers, each region rounded
+ * up to 256 bytes, a256):
+ *   a256(24) + a256(F) + a256(4 F) + (2 L + 1) a256(4 F H) + L (6 a256(2 F H) + a256(4 F heads) + 2 a256(8 F H)).
+ * The masks are not stored: the backward draws them again from the seed and p the tape records. */
+int dsx_fs2dec_train_tape_bytes(dsx_fs2dec_train* h, int B, int T, size_t* out);
+
+/* Bytes of the scratch workspace a forward or a backward over (B, T) needs; it holds nothing between calls. */
+int dsx_fs2dec_train_workspace_bytes(dsx_fs2dec_train* h, int B, int T, size_t* out);
+
+/* One training forward: out [B, T, H] contiguous fp32 of x (logically [B, T, H], any strides xs: b, c = channel, t), with
+ * dropout p_drop in [0, 1) drawn from `seed`, and what the backward needs written to `tape` (at least
+ * dsx_fs2dec_train_tape_bytes).  The weights (fp32 device pointers, pos_embed_alpha required) are packed to fp16 inside
+ * the call, on the stream; the backward uses the packs of the latest forward on the handle, so the weights must not
+ * change between a forward and the backward of its tape.  Several forwards may precede their backwards, each with its
+ * own tape. */
+int dsx_fs2dec_train_forward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const float* x, dsx_strides xs, int B,
+                             int T, float p_drop, uint64_t seed, void* tape, size_t tape_bytes, void* workspace,
+                             size_t workspace_bytes, float* out, void* stream);
+
+/* The backward of the forward that wrote `tape`, with that forward's B and T: d_out [B, T, H] contiguous.  Writes (does
+ * not accumulate) the fp32 gradient of every parameter through `grads` (same layout as w, pos_embed_alpha included), and
+ * d_x [B, T, H] contiguous (the gradient of decoder_inp; 0 on padding frames) unless NULL.  The tape is only read.  A
+ * (B, T) other than the tape's makes every gradient NaN (checked on the device).  The backward reads the handle's packs
+ * of the latest forward: a forward of other weights, on any stream, must not run before or during it. */
+int dsx_fs2dec_train_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* tape, const float* d_out,
+                              const dsx_fs2dec_params* grads, float* d_x, int B, int T, void* workspace,
+                              size_t workspace_bytes, void* stream);
+
+/* Test entry: the 1 + 3 L keep masks (1 kept, 0 dropped) that dsx_fs2dec_train_forward(seed, p_drop) draws, in site
+ * order; out is a HOST array of 1 + 3 L device pointers to uint8 [B, T, H] (sites 2 + 3 i: [B, T, 4H]).  It lets tests
+ * rebuild the same forward in fp32 autograd. */
+int dsx_fs2dec_train_masks(dsx_fs2dec_train* h, uint64_t seed, float p_drop, int B, int T, uint8_t* const* out,
+                           void* stream);
+
 #ifdef __cplusplus
 }
 #endif
