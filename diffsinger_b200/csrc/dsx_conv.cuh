@@ -171,17 +171,27 @@ __global__ void k_pack_conv(const ConvGemm g, const PackArgs p) {
   }
 }
 
-// Sizes g's tiles (g.cin, g.n and g.taps set, tile width at most nt_max), allocates its packs in mem and packs them.
-inline int conv_pack(DevAllocs& mem, ConvGemm& g, int nt_max, const PackArgs& a, cudaStream_t s) {
+// Sizes g's tiles (g.cin, g.n and g.taps set, tile width at most nt_max) and allocates its packs in mem.
+inline int conv_alloc(DevAllocs& mem, ConvGemm& g, int nt_max) {
   g.nt = conv_nt(g.n, nt_max);
   g.ntiles = (g.n + g.nt - 1) / g.nt;
   g.kc = (g.taps * g.cin + 63) / 64;
+  DSX_TRY(mem.alloc(&g.w, static_cast<size_t>(g.ntiles) * g.kc * g.nt * 64 * sizeof(__half)));
+  return mem.alloc(&g.b, static_cast<size_t>(g.ntiles) * g.nt * sizeof(float));
+}
+
+// (Re)fills g's allocated packs on the stream.
+inline int conv_repack(const ConvGemm& g, const PackArgs& a, cudaStream_t s) {
   const size_t nw = static_cast<size_t>(g.ntiles) * g.kc * g.nt * 64;
-  DSX_TRY(mem.alloc(&g.w, nw * sizeof(__half)));
-  DSX_TRY(mem.alloc(&g.b, static_cast<size_t>(g.ntiles) * g.nt * sizeof(float)));
   const int blocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 4096));
   k_pack_conv<<<blocks, 256, 0, s>>>(g, a);
   return launch_check("k_pack_conv");
+}
+
+// conv_alloc, then conv_repack.
+inline int conv_pack(DevAllocs& mem, ConvGemm& g, int nt_max, const PackArgs& a, cudaStream_t s) {
+  DSX_TRY(conv_alloc(mem, g, nt_max));
+  return conv_repack(g, a, s);
 }
 
 }  // namespace

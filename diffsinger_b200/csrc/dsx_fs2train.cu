@@ -47,13 +47,7 @@ constexpr float kLnEps = 1e-5f;
 
 enum { B_GC, B_F32, B_F16 };
 
-// the tape's first region: the forward's dropout, so that the backward draws the same masks from the tape alone, and
-// its (B, T), which the backward checks on the device
-struct TapeHdr {
-  uint64_t seed;
-  float p;
-  int B, T;
-};
+using TapeHdr = Fs2TapeHdr;
 
 __global__ void k_tape_hdr(TapeHdr* h, uint64_t seed, float p, int B, int T) {
   h->seed = seed;

@@ -373,6 +373,13 @@ struct Fs2Train {
     return d;
   }
 };
+// the first region of a dsx_fs2dec_train tape: the forward's dropout, so that the backward draws the same masks from the
+// tape alone, and its (B, T), which the backward checks on the device
+struct Fs2TapeHdr {
+  uint64_t seed;
+  float p;
+  int B, T;
+};
 int fs2_stack_run(const dsx_fs2dec* h, const Fs2Bufs& w, int B, int T, float* out, __half* out16, cudaStream_t s,
                   const Fs2Train* tr = nullptr);
 // k_fs2_pack of x (any strides) into w.X and w.PAD, then fs2_stack_run

@@ -381,49 +381,6 @@ __global__ void k_de_sum(const float* de_l, int L, int B, float* de) {
   de[i] = s;
 }
 
-// mlp.2: dW2[c][j] = sum_b de[b][c] mish[b][j], db2 = sum_b de; dh[b][j] = (W2^T de)[j] * mish'(h[b][j]).  Grid 4C / 256
-// blocks of 256 threads, thread j.
-__global__ void k_mlp2_grad(const float* de, int B, const float* save, const float* w2, const float* scal, float* dw2,
-                            float* db2, float* dh) {
-  const float is = scal[1];
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;   // < 4C
-  for (int b = 0; b < B; ++b) {
-    const float* sv = save + static_cast<size_t>(b) * 9 * kC;
-    float g = 0.f;
-    for (int c = 0; c < kC; ++c) g = fmaf(w2[static_cast<size_t>(c) * 4 * kC + j], de[b * kC + c], g);
-    const float x = sv[kC + j];
-    const float sp = x > 20.f ? x : log1pf(expf(x));
-    const float th = tanhf(sp);
-    const float dsp = x > 20.f ? 1.f : 1.f / (1.f + expf(-x));
-    dh[b * 4 * kC + j] = g * (th + x * (1.f - th * th) * dsp);
-  }
-  if (j < kC) {
-    float s = 0.f;
-    for (int b = 0; b < B; ++b) s += de[b * kC + j];
-    db2[j] = s * is;
-  }
-  // dW2 [C][4C]: this thread's column j for every row c
-  for (int c = 0; c < kC; ++c) {
-    float s = 0.f;
-    for (int b = 0; b < B; ++b) s = fmaf(de[b * kC + c], save[static_cast<size_t>(b) * 9 * kC + 5 * kC + j], s);
-    dw2[static_cast<size_t>(c) * 4 * kC + j] = s * is;
-  }
-}
-
-// mlp.0: dW0[j][k] = sum_b dh[b][j] sinusoid[b][k], db0[j] = sum_b dh[b][j].  Block j, thread k.
-__global__ void k_mlp0_grad(const float* dh, int B, const float* save, const float* scal, float* dw0, float* db0) {
-  const int j = blockIdx.x, k = threadIdx.x;
-  const float is = scal[1];
-  float s = 0.f, sb = 0.f;
-  for (int b = 0; b < B; ++b) {
-    const float d = dh[b * 4 * kC + j];
-    s = fmaf(d, save[static_cast<size_t>(b) * 9 * kC + k], s);
-    sb += d;
-  }
-  dw0[static_cast<size_t>(j) * kC + k] = s * is;
-  if (k == 0) db0[j] = sb * is;
-}
-
 // ---- tape layout --------------------------------------------------------------------------------------------------
 struct Tape {
   __half* spec;   // [F][M]
@@ -936,12 +893,9 @@ int dsx_train_backward(dsx_train* h, const dsx_diffnet_params* w, const void* ta
                 plain(kM, kM, const_cast<float*>(grads->in_w), const_cast<float*>(grads->in_b))));
   k_de_sum<<<(B * kC + 255) / 256, 256, 0, s>>>(DE, L, B, DESUM);
   DSX_TRY(launch_check("k_de_sum"));
-  k_mlp2_grad<<<4 * kC / 256, 256, 0, s>>>(DESUM, B, tp.save, w->mlp2_w, scal, const_cast<float*>(grads->mlp2_w),
-                                           const_cast<float*>(grads->mlp2_b), DHM);
-  DSX_TRY(launch_check("k_mlp2_grad"));
-  k_mlp0_grad<<<4 * kC, kC, 0, s>>>(DHM, B, tp.save, scal, const_cast<float*>(grads->mlp0_w),
-                                     const_cast<float*>(grads->mlp0_b));
-  DSX_TRY(launch_check("k_mlp0_grad"));
+  DSX_TRY(run_mlp_grad(DESUM, B, kC, tp.save, w->mlp2_w, scal, const_cast<float*>(grads->mlp2_w),
+                       const_cast<float*>(grads->mlp2_b), DHM, const_cast<float*>(grads->mlp0_w),
+                       const_cast<float*>(grads->mlp0_b), s));
   if (d_cond) {
     a.mode = B_COND;
     a.g = h->cond_t;

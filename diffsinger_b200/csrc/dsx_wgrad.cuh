@@ -1,6 +1,6 @@
-// Training helpers shared by the DiffNet (dsx_train.cu) and FastSpeech2 decoder (dsx_fs2train.cu) training steps: the
-// weight-gradient GEMM over the frame axis with its fixed-order split (k_wgrad), and the device-chosen power-of-two
-// gradient scale (k_amax, k_scale).
+// Training helpers shared by the DiffNet (dsx_train.cu), FastSpeech2 decoder (dsx_fs2train.cu) and FFT denoiser
+// (dsx_ffttrain.cu) training steps: the weight-gradient GEMM over the frame axis with its fixed-order split (k_wgrad), the
+// device-chosen power-of-two gradient scale (k_amax, k_scale) and the step-embedding MLP's backward (run_mlp_grad).
 #pragma once
 #include <algorithm>
 
@@ -130,6 +130,61 @@ __global__ void k_scale(const unsigned* amax_bits, float* scal) {
   }
   scal[0] = ldexpf(1.f, e);
   scal[1] = ldexpf(1.f, -e);
+}
+
+// ---- step-embedding MLP backward (mlp.0 -> Mish -> mlp.2 of C = residual_channels), from the saves of k_embed_table
+// ([b][9 C]: sinusoid, mlp.0 output, Mish of it) and de = the gradient of the MLP's output, both scaled by S ----------
+// mlp.2: dW2[c][j] = sum_b de[b][c] mish[b][j], db2 = sum_b de; dh[b][j] = (W2^T de)[j] * mish'(h[b][j]).  Thread j < 4C.
+__global__ void k_mlp2_grad(const float* de, int B, int C, const float* save, const float* w2, const float* scal,
+                            float* dw2, float* db2, float* dh) {
+  const float is = scal[1];
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= 4 * C) return;
+  for (int b = 0; b < B; ++b) {
+    const float* sv = save + static_cast<size_t>(b) * 9 * C;
+    float g = 0.f;
+    for (int c = 0; c < C; ++c) g = fmaf(w2[static_cast<size_t>(c) * 4 * C + j], de[b * C + c], g);
+    const float x = sv[C + j];
+    const float sp = x > 20.f ? x : log1pf(expf(x));
+    const float th = tanhf(sp);
+    const float dsp = x > 20.f ? 1.f : 1.f / (1.f + expf(-x));
+    dh[b * 4 * C + j] = g * (th + x * (1.f - th * th) * dsp);
+  }
+  if (j < C) {
+    float s = 0.f;
+    for (int b = 0; b < B; ++b) s += de[b * C + j];
+    db2[j] = s * is;
+  }
+  // dW2 [C][4C]: this thread's column j for every row c
+  for (int c = 0; c < C; ++c) {
+    float s = 0.f;
+    for (int b = 0; b < B; ++b) s = fmaf(de[b * C + c], save[static_cast<size_t>(b) * 9 * C + 5 * C + j], s);
+    dw2[static_cast<size_t>(c) * 4 * C + j] = s * is;
+  }
+}
+
+// mlp.0: dW0[j][k] = sum_b dh[b][j] sinusoid[b][k], db0[j] = sum_b dh[b][j].  Block j, thread k.
+__global__ void k_mlp0_grad(const float* dh, int B, int C, const float* save, const float* scal, float* dw0,
+                            float* db0) {
+  const int j = blockIdx.x, k = threadIdx.x;
+  const float is = scal[1];
+  float s = 0.f, sb = 0.f;
+  for (int b = 0; b < B; ++b) {
+    const float d = dh[b * 4 * C + j];
+    s = fmaf(d, save[static_cast<size_t>(b) * 9 * C + k], s);
+    sb += d;
+  }
+  dw0[static_cast<size_t>(j) * C + k] = s * is;
+  if (k == 0) db0[j] = sb * is;
+}
+
+// both, with dh [B][4 C] as scratch (C <= 1024)
+int run_mlp_grad(const float* de, int B, int C, const float* save, const float* w2, const float* scal, float* dw2,
+                 float* db2, float* dh, float* dw0, float* db0, cudaStream_t s) {
+  k_mlp2_grad<<<(4 * C + 255) / 256, 256, 0, s>>>(de, B, C, save, w2, scal, dw2, db2, dh);
+  DSX_TRY(launch_check("k_mlp2_grad"));
+  k_mlp0_grad<<<4 * C, C, 0, s>>>(dh, B, C, save, scal, dw0, db0);
+  return launch_check("k_mlp0_grad");
 }
 
 int sm_count(int device) {

@@ -11,7 +11,9 @@ whose ``forward(infer=True)`` runs the sm_90a sampler, and the ``'wavenet'`` ent
 ``diffsinger_b200.DiffNet``.  Construction arguments, parameter / buffer names, ``p_losses`` and the returned ``ret`` dict
 are the reference's own, so the task files run unchanged.  With ``diff_decoder_type: 'fft'`` the reference's own ``FFT``
 (usr/diff/candidate_decoder.py) stays the ``denoise_fn``: ``DsxSampler`` recognises it and runs its evaluations on dsx
-(``dsx_load_fft``), while training (``p_losses``) keeps calling the reference's module, so nothing is rebound for it.
+(``dsx_load_fft``).  Only when hparams set ``dsx_train`` does the ``'fft'`` entry of every ``DIFF_DECODERS`` registry
+build ``diffsinger_b200.FFT`` instead, so that training (``p_losses``) runs the sm_90a training step; ``uninstall()``
+restores the entry.
 
     dropin.install_vocoder()
 
@@ -152,7 +154,23 @@ def install():
         reg = getattr(mod, "DIFF_DECODERS", None)
         if isinstance(reg, dict) and "wavenet" in reg:
             reg["wavenet"] = wavenet
+        if isinstance(reg, dict) and "fft" in reg and name not in _fft_entries:
+            _fft_entries[name] = ref_fft = reg["fft"]
+            reg["fft"] = _fft_builder(ref_fft)
     return _installed["new_cls"]
+
+
+_fft_entries = {}   # module name -> the DIFF_DECODERS['fft'] entry install() replaced
+
+
+def _fft_builder(ref_fft):
+    """DIFF_DECODERS['fft']: diffsinger_b200.FFT under dsx_train, else the reference's entry (its own FFT)."""
+    def build(hp):
+        if not hp.get('dsx_train', False):
+            return ref_fft(hp)
+        from .fftdiff import FFT
+        return FFT(hp['hidden_size'], hp['dec_layers'], hp['dec_ffn_kernel_size'], hp['num_heads'], hparams=hp)
+    return build
 
 
 def uninstall():
@@ -161,6 +179,11 @@ def uninstall():
     back = {id(_installed[n]): _installed[r] for r, n in (("ref_cls", "new_cls"), ("ref_off", "new_off"), ("ref_old", "new_old"))
             if _installed[n] is not None}
     importlib.import_module("usr.diff.net").DiffNet = _installed["ref_net"]
+    for name, ref_fft in list(_fft_entries.items()):
+        reg = getattr(sys.modules.get(name), "DIFF_DECODERS", None)
+        if isinstance(reg, dict):
+            reg["fft"] = ref_fft
+        del _fft_entries[name]
     for name, mod in list(sys.modules.items()):
         if mod is None:
             continue

@@ -1,17 +1,19 @@
 """FFT diffusion denoiser whose evaluations run the sm_90a kernels of libdsx.so (dsx_load_fft in include/dsx.h).
 
-``FFT(hidden_size=None, num_layers=None, kernel_size=None, num_heads=None, *, hparams=None)`` keeps the constructor,
-submodule names and the state dict of the reference's ``FFT`` (usr/diff/candidate_decoder.py:35-100, the
+``FFT(hidden_size=None, num_layers=None, kernel_size=None, num_heads=None, *, hparams=None, train=None)`` keeps the
+constructor, submodule names and the state dict of the reference's ``FFT`` (usr/diff/candidate_decoder.py:35-100, the
 ``DIFF_DECODERS['fft']`` entry of usr/diffsinger_task.py), so it loads with ``strict=True``.  Besides the constructor's
 arguments it reads ``residual_channels``, ``audio_num_mel_bins``, ``ffn_padding``, ``ffn_act`` and ``dropout`` from
 hparams.  Its eval ``forward(spec, diffusion_step, cond)`` is one evaluation in the sampler handle of ``.dsx``
-(a ``DsxSampler``), which also runs whole sampling loops with it.  There is no eager or CPU path and no training path:
-a CPU tensor or a module in training mode raises ``DsxError``.
+(a ``DsxSampler``), which also runs whole sampling loops with it.  There is no eager or CPU path: a CPU tensor raises
+``DsxError``.  A module in training mode raises ``DsxError`` too, unless the ``dsx_train`` opt-in (hparams key or
+``train=`` keyword) is set: then a training-mode forward under autograd runs the sm_90a training step of
+``diffsinger_b200.ffttrain`` (dropout p = hparams['dropout'], gradients for every parameter and for cond).
 
 ``DsxSampler`` recognises an FFT denoiser by its ``get_decode_inp.weight`` parameter, whether it is this class or the
-reference's own ``FFT``, and takes the configuration from the module (``load_fft``).  So ``dropin.install()`` needs no
-rebinding for it: its sampler subclasses route ``forward(infer=True)`` through ``DsxInferMixin``, while training
-(``p_losses``) keeps calling the reference's module.
+reference's own ``FFT``, and takes the configuration from the module (``load_fft``).  So sampling needs no rebinding:
+``dropin.install()``'s sampler subclasses route ``forward(infer=True)`` through ``DsxInferMixin`` with either class.  For
+training, ``dropin.install()`` rebinds ``DIFF_DECODERS['fft']`` to build this class when hparams set ``dsx_train``.
 """
 import ctypes
 
@@ -79,8 +81,8 @@ def load_fft(h, net, sd, device):
 
 
 class FFT(FastspeechDecoder):
-    def __init__(self, hidden_size=None, num_layers=None, kernel_size=None, num_heads=None, *, hparams=None):
-        super().__init__(hidden_size, num_layers, kernel_size, num_heads, hparams=hparams)
+    def __init__(self, hidden_size=None, num_layers=None, kernel_size=None, num_heads=None, *, hparams=None, train=None):
+        super().__init__(hidden_size, num_layers, kernel_size, num_heads, hparams=hparams, train=train)
         hp = _get_hparams(hparams)
         self._fft_cfg = _fft_config(self._cfg, hp['residual_channels'], hp['audio_num_mel_bins'])
         dim, M = self._fft_cfg.residual_channels, self._fft_cfg.mel_bins
@@ -101,7 +103,14 @@ class FFT(FastspeechDecoder):
         # the sampler holds a ctypes handle: copies build their own
         state = self.__dict__.copy()
         state["_sampler"] = None
+        state["_dsx_trainer"] = None
         return state
+
+    def _dsx_train_step(self):
+        if self._dsx_trainer is None:
+            from .ffttrain import FftTrainStep
+            object.__setattr__(self, "_dsx_trainer", FftTrainStep(self._fft_cfg))
+        return self._dsx_trainer
 
     def forward(self, spec, diffusion_step, cond, padding_mask=None, attn_mask=None, return_hiddens=False):
         """spec [B, 1, 80, T], diffusion_step [B], cond [B, hidden_size, T] -> eps [B, 1, 80, T] fp32
@@ -109,6 +118,9 @@ class FFT(FastspeechDecoder):
         if padding_mask is not None or attn_mask is not None or return_hiddens:
             raise DsxError("the dsx FFT denoiser takes spec, diffusion_step and cond only: padding_mask, attn_mask and "
                            "return_hiddens are not supported")
+        if self.training and self._dsx_train and torch.is_grad_enabled():
+            from .ffttrain import fft_train_forward
+            return fft_train_forward(self, spec, diffusion_step, cond)
         if self.training:
             raise DsxError("the dsx FFT denoiser runs in eval mode only (call .eval()); training stays with the "
                            "reference's modules")

@@ -672,6 +672,53 @@ int dsx_fs2dec_train_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, c
 int dsx_fs2dec_train_masks(dsx_fs2dec_train* h, uint64_t seed, float p_drop, int B, int T, uint8_t* const* out,
                            void* stream);
 
+/* ---- FFT denoiser training step -------------------------------------------------------------------------------------
+ * Replaces: FFT.forward(spec, diffusion_step, cond) (usr/diff/candidate_decoder.py:50-100) in training mode, as
+ * GaussianDiffusion.p_losses calls it with diff_decoder_type 'fft', and its autograd backward: the gradient of every
+ * parameter and of cond (not of spec).  The entry and exit are dsx_load_fft's (input_projection folded into
+ * get_decode_inp in double, hi+lo fp16 operands for x_t and cond, the step embedding in fp32); the FFTBlocks stack is the
+ * decoder training step's, with its dropout: the same 1 + 3 L sites, the same (seed, site, frame, channel) keying and the
+ * same p, so dsx_fs2dec_train_masks on a dsx_fs2dec_train handle of the same dsx_fs2dec_config returns exactly the masks
+ * of a forward with that seed and p.  The backward's fp16 operands are scaled by powers of two chosen on the device
+ * (from amax |d_eps|, then from amax |d decoder_inp|) and divided out exactly, so 2^k d_eps gives exactly 2^k times the
+ * gradients and d_eps = 0 exact zeros.  Gradients are bitwise reproducible (fixed-order reductions, no atomics).  No call
+ * allocates or synchronises the host: the tape and the workspace are the caller's.  A handle is independent of the other
+ * handles. */
+typedef struct dsx_fft_train dsx_fft_train;
+
+/* Accepts what dsx_load_fft accepts (DSX_E_INVALID, "unsupported ..."). */
+int dsx_fft_train_create(int device, const dsx_fft_config* cfg, dsx_fft_train** out);
+void dsx_fft_train_destroy(dsx_fft_train* h);
+
+/* Bytes of the tape of one forward over B utterances of T frames (F = B T, H = hidden, dim = residual_channels, each
+ * region rounded up to 256 bytes, a256):
+ *   D + a256(4 B dim) + a256(36 B dim) + a256(480 F) + a256(6 F H) + a256(2 F H)
+ * with D = dsx_fs2dec_train_tape_bytes of the stack's configuration, whose tape comes first. */
+int dsx_fft_train_tape_bytes(dsx_fft_train* h, int B, int T, size_t* out);
+
+/* Bytes of the scratch workspace a forward or a backward over (B, T) needs; it holds nothing between calls. */
+int dsx_fft_train_workspace_bytes(dsx_fft_train* h, int B, int T, size_t* out);
+
+/* One training forward: eps [B,1,80,T] contiguous fp32 of spec [B,1,80,T] (through ss: b, c = mel bin, t), t device
+ * int64 [B] and cond [B,H,T] (through cs), with dropout p_drop in [0, 1) drawn from `seed` and what the backward needs
+ * written to `tape` (at least dsx_fft_train_tape_bytes).  The weights (fp32 device pointers, dsx_load_fft's struct,
+ * pos_embed_alpha required) are packed inside the call, on the stream; the backward uses the packs of the latest forward
+ * on the handle, so the weights must not change between a forward and the backward of its tape.  Several forwards may
+ * precede their backwards, each with its own tape. */
+int dsx_fft_train_forward(dsx_fft_train* h, const dsx_fft_params* w, const float* spec, dsx_strides ss,
+                          const int64_t* t, const float* cond, dsx_strides cs, int B, int T, float p_drop,
+                          uint64_t seed, void* tape, size_t tape_bytes, void* workspace, size_t workspace_bytes,
+                          float* eps, void* stream);
+
+/* The backward of the forward that wrote `tape`, with that forward's B and T: d_eps [B,1,80,T] contiguous.  Writes (does
+ * not accumulate) the fp32 gradient of every parameter through `grads` (same layout as w, pos_embed_alpha included), and
+ * d_cond unless NULL, frames-major [B, T, H] contiguous (the [B, H, T] gradient of cond, transposed).  The tape is only
+ * read.  A (B, T) other than the tape's makes every gradient NaN (checked on the device).  The backward reads the handle's
+ * packs of the latest forward: a forward of other weights, on any stream, must not run before or during it. */
+int dsx_fft_train_backward(dsx_fft_train* h, const dsx_fft_params* w, const void* tape, const float* d_eps,
+                           const dsx_fft_params* grads, float* d_cond, int B, int T, void* workspace,
+                           size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
