@@ -588,8 +588,8 @@ typedef struct {
   int M;                   /* in_dims: 80                                     */
   int C;                   /* residual_channels: 256                          */
   int H;                   /* hidden_size (cond channels): 256                */
-  int L;                   /* residual_layers: >= 1                           */
-  int dilation_cycle;      /* dilation_cycle_length: dilation 2^(l % cycle)   */
+  int L;                   /* residual_layers: 1..1024                        */
+  int dilation_cycle;      /* dilation_cycle_length: 1..24, dilation 2^(l % cycle) */
 } dsx_train_config;
 
 /* Validates the configuration (DSX_E_INVALID). */
@@ -606,7 +606,8 @@ int dsx_train_workspace_bytes(dsx_train* h, int B, int T, size_t* out);
 
 /* One forward: eps [B,1,M,T] (contiguous) of spec [B,1,M,T] (through ss: b, c = mel bin, t), t device int64 [B], cond
  * [B,H,T] (through cs), with the activations the backward needs written to `tape` (caller-owned device memory of at
- * least dsx_train_tape_bytes) and `workspace` (at least dsx_train_workspace_bytes) as scratch.  The weights
+ * least dsx_train_tape_bytes) and `workspace` (at least dsx_train_workspace_bytes) as scratch.  B <= 65535,
+ * B T <= 2^24 and L B T < 2^26 (DSX_E_INVALID otherwise).  The weights
  * (dsx_load_diffnet's pointer struct) are packed to fp16 inside the call, on the stream; the backward uses the packs of
  * the latest forward on the handle, so the weights must not change between a forward and the backward of its tape.
  * Several forwards may precede their backwards, each with its own tape. */

@@ -9,7 +9,8 @@ from oracle.fft_oracle import _p, decode_inp
 from oracle.fs2dec_train_oracle import decoder_train
 
 
-def forward_train(sd, spec, t, cond, hp, masks, p):
-    """FFT.forward(spec [B, 1, 80, T], t [B], cond [B, H, T]) in training -> eps [B, 1, 80, T]"""
-    x = decoder_train(sd, decode_inp(sd, spec, t, cond, hp), hp, masks, p)
+def forward_train(sd, spec, t, cond, hp, masks, p, layer_input=None):
+    """FFT.forward(spec [B, 1, 80, T], t [B], cond [B, H, T]) in training -> eps [B, 1, 80, T]; ``layer_input`` as in
+    decoder_train"""
+    x = decoder_train(sd, decode_inp(sd, spec, t, cond, hp), hp, masks, p, layer_input)
     return F.linear(x, _p(sd["get_mel_out.weight"]), sd["get_mel_out.bias"]).permute([0, 2, 1])[:, None, :, :]

@@ -35,13 +35,15 @@ def _ffn(sd, hp, i, x, mask, p):
     return F.linear(y, w2 if w2.requires_grad else torch.nn.Parameter(w2), sd[p2 + "bias"])
 
 
-def decoder_train(sd, x, hp, masks, p):
+def decoder_train(sd, x, hp, masks, p, layer_input=None):
+    """x [B, T, H] -> [B, T, H]; a float64 x gets a float64 position table.  ``layer_input(i, x)``, if given, replaces
+    the residual stream x ([T, B, H]) entering layer i (an identity autograd Function there can alter its backward)."""
     B, T, H = x.shape
     heads = int(hp['num_heads'])
     tb = lambda s: masks[s].transpose(0, 1)                        # [B, T, n] -> the layers' [T, B, n]
     pad = padding_mask(x)
     nonpad_TB = 1 - pad.transpose(0, 1).to(x.dtype)[:, :, None]
-    table = sinusoidal_table(max(2000, 1 + T), H).to(x)
+    table = sinusoidal_table(max(2000, 1 + T), H, dtype=torch.float64 if x.dtype == torch.float64 else torch.float).to(x)
     pos = make_positions(x[..., 0])
     x = x + sd["pos_embed_alpha"] * table.index_select(0, pos.view(-1)).view(B, T, -1)
     x = dropout(x, masks[0], p)
@@ -49,6 +51,8 @@ def decoder_train(sd, x, hp, masks, p):
     keep = (1 - pad.to(x.dtype)).transpose(0, 1)[..., None]
     for i in range(int(hp['dec_layers'])):
         pre = f"layers.{i}.op."
+        if layer_input is not None:
+            x = layer_input(i, x)
         residual = x
         y = F.layer_norm(x, (H,), sd[pre + "layer_norm1.weight"], sd[pre + "layer_norm1.bias"], LN_EPS)
         y, _ = F.multi_head_attention_forward(y, y, y, H, heads, sd[pre + "self_attn.in_proj_weight"], None, None, None,
