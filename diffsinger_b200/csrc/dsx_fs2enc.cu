@@ -40,10 +40,12 @@ __device__ __forceinline__ float rel_table(int ps, int c, float neg) {
 }
 
 // One warp per token, H / 32 <= 8 channels per lane.  mode 0: x + table[pos] (sinusoidal, pos from k_pos_scan_tokens);
-// mode 1: x * sqrt(H) + rel_table(P - 1 - t).  An id outside [0, vocab) reads a zero row.
+// mode 1: x * sqrt(H) + rel_table(P - 1 - t).  An id outside [0, vocab) reads a zero row.  Training (the encoder training
+// step, dsx_fs2enctrain.cu): dropout site `drop` before the * !pad, and X copied to xsave.
 __global__ void k_fs2enc_embed(const int64_t* tok, int rows, int T, int H, const float* E, int vocab, float scale,
                                EncAddends add, int mode, const int* pos, float neg_emb, int rel_len, float rel_neg,
-                               const float* ln_w, const float* ln_b, float* X, uint8_t* PAD, __half* A) {
+                               const float* ln_w, const float* ln_b, float* X, uint8_t* PAD, __half* A, Fs2Drop drop,
+                               float* xsave) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= rows) return;
   const int b = warp / T, t = warp - b * T, per = H / 32;
@@ -62,8 +64,10 @@ __global__ void k_fs2enc_embed(const int64_t* tok, int rows, int T, int H, const
       if (add.p[k]) x = x + add.p[k][b * add.s[k].b + c * add.s[k].c + t * add.s[k].t];
     }
     x = mode == 0 ? x + pos_table(pos[warp], c, H, neg_emb) : x * scale + rel_table(rel_len - 1 - t, c, rel_neg);
+    if (drop.site >= 0) x *= dropout_scale(drop, warp, c);
     v[i] = keep ? x : 0.f;
     xr[c] = v[i];
+    if (xsave) xsave[static_cast<size_t>(warp) * H + c] = v[i];
   }
   if (lane == 0) PAD[warp] = keep ? 0 : 1;
   warp_row_ln16(v, per, H, kEncLnEps, ln_w, ln_b, A + static_cast<size_t>(warp) * H);
@@ -115,6 +119,33 @@ __global__ void k_lr_fill(const int64_t* cum, const int64_t* totals, int B, int 
 }
 
 }  // namespace
+
+int fs2enc_entry(const dsx_fs2dec* stack, int pos_mode, const float* E, int vocab, const int64_t* tokens, int B, int T,
+                 const float* const* add, const dsx_strides* as, int rel_len, const Fs2Bufs& w, __half* A,
+                 const Fs2Drop& drop, float* xsave, cudaStream_t s) {
+  EncAddends ad{};
+  for (int k = 0; k < 3; ++k) {
+    ad.p[k] = add ? add[k] : nullptr;
+    if (ad.p[k]) {
+      DSX_CHECK(as, DSX_E_INVALID, "addend %d has no strides", k);
+      ad.s[k] = as[k];
+    }
+  }
+  const int H = fs2_config(stack).hidden;
+  if (pos_mode == 0) {
+    k_pos_scan_tokens<<<B, kScanThreads, 0, s>>>(tokens, T, w.POS);
+    DSX_TRY(launch_check("k_pos_scan_tokens"));
+  }
+  const float* ln_w;
+  const float* ln_b;
+  fs2_first_ln(stack, &ln_w, &ln_b);
+  const size_t frames = static_cast<size_t>(B) * T;
+  k_fs2enc_embed<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(
+      tokens, static_cast<int>(frames), T, H, E, vocab, static_cast<float>(sqrt(static_cast<double>(H))), ad, pos_mode,
+      w.POS, pos_neg_emb(H), rel_len, -static_cast<float>(log(10000.0) / H), ln_w, ln_b, w.X, w.PAD, A, drop, xsave);
+  return launch_check("k_fs2enc_embed");
+}
+
 }  // namespace dsx
 
 using namespace dsx;
@@ -181,35 +212,15 @@ int dsx_fs2enc_forward(dsx_fs2enc* h, const int64_t* tokens, int B, int T, const
   DSX_CHECK(B > 0 && T > 0, DSX_E_INVALID, "B and T must be positive (got %d, %d)", B, T);
   DSX_CHECK(B <= 65535, DSX_E_INVALID, "B = %d utterances per call is above the 65535 the launch grid holds", B);
   DSX_CHECK(h->cfg.pos == 0 || rel_len >= T, DSX_E_INVALID, "rel_len %d is shorter than T = %d", rel_len, T);
-  const int H = h->cfg.stack.hidden;
   const int Tp = (T + kConvRows - 1) / kConvRows * kConvRows;
-  DSX_CHECK(static_cast<long long>(B) * Tp * 4 * H < (1ll << 31), DSX_E_INVALID, "B * T = %lld tokens is too large",
-            static_cast<long long>(B) * T);
-  EncAddends ad{};
-  for (int k = 0; k < 3; ++k) {
-    ad.p[k] = add ? add[k] : nullptr;
-    if (ad.p[k]) {
-      DSX_CHECK(as, DSX_E_INVALID, "addend %d has no strides", k);
-      ad.s[k] = as[k];
-    }
-  }
+  DSX_CHECK(static_cast<long long>(B) * Tp * 4 * h->cfg.stack.hidden < (1ll << 31), DSX_E_INVALID,
+            "B * T = %lld tokens is too large", static_cast<long long>(B) * T);
   DSX_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   DSX_TRY(h->ws.reserve(fs2_workspace_bytes(h->stack, B, T), s));
   const Fs2Bufs w = fs2_carve(h->stack, h->ws.ptr, B, T);
-  if (h->cfg.pos == 0) {
-    k_pos_scan_tokens<<<B, kScanThreads, 0, s>>>(tokens, T, w.POS);
-    DSX_TRY(launch_check("k_pos_scan_tokens"));
-  }
-  const float* ln_w;
-  const float* ln_b;
-  fs2_first_ln(h->stack, &ln_w, &ln_b);
-  const size_t frames = static_cast<size_t>(B) * T;
-  k_fs2enc_embed<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(
-      tokens, static_cast<int>(frames), T, H, h->embed, h->cfg.vocab, static_cast<float>(sqrt(static_cast<double>(H))),
-      ad, h->cfg.pos, w.POS, pos_neg_emb(H), rel_len, -static_cast<float>(log(10000.0) / H), ln_w, ln_b, w.X, w.PAD,
-      w.A);
-  DSX_TRY(launch_check("k_fs2enc_embed"));
+  DSX_TRY(fs2enc_entry(h->stack, h->cfg.pos, h->embed, h->cfg.vocab, tokens, B, T, add, as, rel_len, w, w.A, Fs2Drop{},
+                       nullptr, s));
   return fs2_layers_run(h->stack, w, B, T, out, nullptr, s);
 }
 

@@ -130,7 +130,7 @@ struct LnArgs {
   __half* o16;                 // G * dropout(drop) -> fp16 [F][H], or null
   int entry;                   // layer 0: d_x = G * dropout(drop) / S and the d alpha partials
   float* dx;                   // entry: [F][H] fp32, or null
-  const int* pos;
+  const int* pos;              // entry: the positions of d alpha, or null (no d alpha)
   float neg_emb;
   const TapeHdr* hdr;          // the dropout of o16 or of the entry: site `site` of the tape's seed and p
   int site;
@@ -201,7 +201,7 @@ __global__ void __launch_bounds__(256) k_f2b_ln(const LnArgs p) {
       if (p.entry) {
         const float d = v * dropout_scale(drop, f, c);
         if (p.dx) p.dx[rb + c] = d * is;
-        dal += d * pos_table(p.pos[f], c, H, p.neg_emb);
+        if (p.pos) dal += d * pos_table(p.pos[f], c, H, p.neg_emb);
       }
     }
   }
@@ -538,12 +538,7 @@ __global__ void k_f2_masks(Fs2Drop d, size_t F, int n, uint8_t* out) {
 }
 
 // ---- tape -------------------------------------------------------------------------------------------------------------
-struct Tape {
-  TapeHdr* hdr;
-  uint8_t* pad;                // [F]
-  int* pos;                    // [F]
-  Fs2Train tr;
-};
+using Tape = Fs2TrainTape;
 
 // every region of the tape for (config, B, T), in order; bytes of the whole tape
 size_t tape_carve(const dsx_fs2dec_config& c, int B, int T, uint8_t* base, Tape* t) {
@@ -662,18 +657,6 @@ int check_geom(const dsx_fs2dec_train* h, int B, int T) {
   return DSX_OK;
 }
 
-int check_params(const dsx_fs2dec_params* p, int L, const char* what) {
-  DSX_CHECK(p, DSX_E_INVALID, "%s is NULL", what);
-  DSX_CHECK(p->ln1_w && p->ln1_b && p->in_proj_w && p->out_proj_w && p->ln2_w && p->ln2_b && p->ffn1_w && p->ffn1_b &&
-                p->ffn2_w && p->ffn2_b && p->ln_w && p->ln_b && p->pos_embed_alpha,
-            DSX_E_INVALID, "a pointer of %s is NULL", what);
-  for (int l = 0; l < L; ++l)
-    DSX_CHECK(p->ln1_w[l] && p->ln1_b[l] && p->in_proj_w[l] && p->out_proj_w[l] && p->ln2_w[l] && p->ln2_b[l] &&
-                  p->ffn1_w[l] && p->ffn1_b[l] && p->ffn2_w[l] && p->ffn2_b[l],
-              DSX_E_INVALID, "a pointer of layer %d of %s is NULL", l, what);
-  return DSX_OK;
-}
-
 template <int D>
 int abwd_opt_in() {
   DSX_CUDA(cudaFuncSetAttribute(k_attn_bwd_kv<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, abwd_smem<D>()));
@@ -684,84 +667,29 @@ int abwd_opt_in() {
 }  // namespace
 }  // namespace dsx
 
-using namespace dsx;
+namespace dsx {
 
-extern "C" {
+dsx_fs2dec* fs2t_stack(dsx_fs2dec_train* h) { return h->dec; }
 
-int dsx_fs2dec_train_create(int device, const dsx_fs2dec_config* cfg, dsx_fs2dec_train** out) {
-  DSX_CHECK(out, DSX_E_INVALID, "out is NULL");
-  *out = nullptr;
-  dsx_fs2dec* dec = nullptr;
-  DSX_TRY(dsx_fs2dec_create(device, cfg, &dec));   // validates the configuration and selects the device
-  dsx_fs2dec_train* h = new dsx_fs2dec_train();
-  h->device = device;
-  h->cfg = *cfg;
-  h->dec = dec;
-  auto fail = [&](int rc) {
-    dsx_fs2dec_train_destroy(h);
-    return rc;
-  };
-  int rc = DSX_OK;
-  if ((rc = fs2_train_alloc(dec))) return fail(rc);
-  if ((rc = []() -> int {
-         DSX_CUDA(cudaFuncSetAttribute(k_f2b_gemm<kNT>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv_smem<kNT>()));
-         DSX_CUDA(cudaFuncSetAttribute(k_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem));
-         DSX_TRY(abwd_opt_in<64>());
-         return abwd_opt_in<128>();
-       }()))
-    return fail(rc);
-  const int H = cfg->hidden, k = cfg->kernel;
-  h->layers.resize(cfg->layers);
-  for (auto& l : h->layers) {
-    if ((rc = gemm_alloc(h->mem, l.in_t, 3 * H, H, 1)) || (rc = gemm_alloc(h->mem, l.out_t, H, H, 1)) ||
-        (rc = gemm_alloc(h->mem, l.ffn1_t, 4 * H, H, k)) || (rc = gemm_alloc(h->mem, l.ffn2_t, H, 4 * H, 1)))
-      return fail(rc);
-    l.ffn1_t.tap0 = -tap0_of(*cfg);   // gA[t] = sum_j W_j^T gC[t - tap0 - j]
-    l.ffn1_t.tstep = -1;
-  }
-  *out = h;
+size_t fs2t_tape_carve(const dsx_fs2dec_train* h, int B, int T, void* base, Fs2TrainTape* t) {
+  return tape_carve(h->cfg, B, T, static_cast<uint8_t*>(base), t);
+}
+
+int fs2t_check_params(const dsx_fs2dec_params* p, int L, int alpha, const char* what) {
+  DSX_CHECK(p, DSX_E_INVALID, "%s is NULL", what);
+  DSX_CHECK(p->ln1_w && p->ln1_b && p->in_proj_w && p->out_proj_w && p->ln2_w && p->ln2_b && p->ffn1_w && p->ffn1_b &&
+                p->ffn2_w && p->ffn2_b && p->ln_w && p->ln_b && (p->pos_embed_alpha || !alpha),
+            DSX_E_INVALID, "a pointer of %s is NULL", what);
+  for (int l = 0; l < L; ++l)
+    DSX_CHECK(p->ln1_w[l] && p->ln1_b[l] && p->in_proj_w[l] && p->out_proj_w[l] && p->ln2_w[l] && p->ln2_b[l] &&
+                  p->ffn1_w[l] && p->ffn1_b[l] && p->ffn2_w[l] && p->ffn2_b[l],
+              DSX_E_INVALID, "a pointer of layer %d of %s is NULL", l, what);
   return DSX_OK;
 }
 
-void dsx_fs2dec_train_destroy(dsx_fs2dec_train* h) {
-  if (!h) return;
-  cudaSetDevice(h->device);
-  cudaDeviceSynchronize();
-  h->mem.free_all();
-  dsx_fs2dec_destroy(h->dec);
-  delete h;
-}
-
-int dsx_fs2dec_train_tape_bytes(dsx_fs2dec_train* h, int B, int T, size_t* out) {
-  DSX_CHECK(h && out, DSX_E_INVALID, "null handle or out");
-  DSX_TRY(check_geom(h, B, T));
-  *out = tape_carve(h->cfg, B, T, nullptr, nullptr);
-  return DSX_OK;
-}
-
-int dsx_fs2dec_train_workspace_bytes(dsx_fs2dec_train* h, int B, int T, size_t* out) {
-  DSX_CHECK(h && out, DSX_E_INVALID, "null handle or out");
-  DSX_TRY(check_geom(h, B, T));
-  *out = ws_bytes(h, B, T);
-  return DSX_OK;
-}
-
-int dsx_fs2dec_train_forward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const float* x, dsx_strides xs, int B,
-                             int T, float p_drop, uint64_t seed, void* tape, size_t tape_bytes, void* workspace,
-                             size_t workspace_bytes, float* out, void* stream) {
-  DSX_TRY(check_geom(h, B, T));
+int fs2t_begin(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, int B, int T, float p_drop, uint64_t seed, void* tape,
+               cudaStream_t s, Fs2TrainTape* tp) {
   const dsx_fs2dec_config& c = h->cfg;
-  DSX_TRY(check_params(w, c.layers, "the parameters"));
-  DSX_CHECK(x && tape && workspace && out, DSX_E_INVALID, "x, tape, workspace and out must not be NULL");
-  DSX_CHECK(p_drop >= 0.f && p_drop < 1.f, DSX_E_INVALID, "dropout p = %g is outside [0, 1)", static_cast<double>(p_drop));
-  const size_t need = tape_carve(c, B, T, nullptr, nullptr);
-  DSX_CHECK(tape_bytes >= need, DSX_E_INVALID, "tape of %zu bytes is below the %zu this (B, T) needs", tape_bytes, need);
-  const size_t wneed = ws_bytes(h, B, T);
-  DSX_CHECK(workspace_bytes >= wneed, DSX_E_INVALID, "workspace of %zu bytes is below the %zu this (B, T) needs",
-            workspace_bytes, wneed);
-  DSX_CUDA(cudaSetDevice(h->device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-
   // round-to-nearest fp16 packs of this step's weights, and the transposed packs of the backward
   DSX_TRY(fs2_train_pack(h->dec, w, s));
   for (int l = 0; l < c.layers; ++l) {
@@ -771,31 +699,17 @@ int dsx_fs2dec_train_forward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, co
     DSX_TRY(pack_t(pk.ffn1_t, w->ffn1_w[l], c.kernel, s));
     DSX_TRY(pack_t(pk.ffn2_t, w->ffn2_w[l], 1, s));
   }
-  Tape tp;
-  tape_carve(c, B, T, static_cast<uint8_t*>(tape), &tp);
-  tp.tr.seed = seed;
-  tp.tr.p = p_drop;
-  k_tape_hdr<<<1, 1, 0, s>>>(tp.hdr, seed, p_drop, B, T);
-  DSX_TRY(launch_check("k_tape_hdr"));
-  Fs2Bufs fb = fs2_carve(h->dec, workspace, B, T);
-  fb.PAD = tp.pad;
-  fb.POS = tp.pos;
-  return fs2_forward_run(h->dec, x, xs, B, T, fb, out, s, &tp.tr);
+  tape_carve(c, B, T, static_cast<uint8_t*>(tape), tp);
+  tp->tr.seed = seed;
+  tp->tr.p = p_drop;
+  k_tape_hdr<<<1, 1, 0, s>>>(tp->hdr, seed, p_drop, B, T);
+  return launch_check("k_tape_hdr");
 }
 
-int dsx_fs2dec_train_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* tape, const float* d_out,
-                              const dsx_fs2dec_params* grads, float* d_x, int B, int T, void* workspace,
-                              size_t workspace_bytes, void* stream) {
-  DSX_TRY(check_geom(h, B, T));
+int fs2t_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* tape, const float* d_out,
+                  const dsx_fs2dec_params* grads, float* d_x, float* d_alpha, int B, int T, void* workspace,
+                  cudaStream_t s) {
   const dsx_fs2dec_config& c = h->cfg;
-  DSX_TRY(check_params(w, c.layers, "the parameters"));
-  DSX_TRY(check_params(grads, c.layers, "the gradients"));
-  DSX_CHECK(tape && d_out && workspace, DSX_E_INVALID, "tape, d_out and workspace must not be NULL");
-  const size_t wneed = ws_bytes(h, B, T);
-  DSX_CHECK(workspace_bytes >= wneed, DSX_E_INVALID, "workspace of %zu bytes is below the %zu this (B, T) needs",
-            workspace_bytes, wneed);
-  DSX_CUDA(cudaSetDevice(h->device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int H = c.hidden, L = c.layers, heads = c.heads, D = H / heads, k = c.kernel, F = B * T;
   const int mtiles = (T + kConvRows - 1) / kConvRows;
   Tape tp;
@@ -841,7 +755,7 @@ int dsx_fs2dec_train_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, c
     a.o16 = o16;
     a.entry = entry;
     a.dx = d_x;
-    a.pos = tp.pos;
+    a.pos = dalpha ? tp.pos : nullptr;
     a.neg_emb = pos_neg_emb(H);
     a.hdr = tp.hdr;
     a.site = site;
@@ -983,9 +897,112 @@ int dsx_fs2dec_train_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, c
     DSX_TRY(wgrad(GQKV, 3 * H, 3 * H, single(tr.a1[i], H, H), 1, rows(gp(grads->in_proj_w[i]), H, H, nullptr)));
     // LN1, then the operand of the layer below, or the entry: x + alpha * table[pos] -> dropout -> * !pad
     DSX_TRY(ln(GA, 0, tr.xin[2 * i], w->ln1_w[i], 1, i > 0 ? GY : nullptr, i > 0 ? 3 * i : 0, i == 0,
-               gp(grads->ln1_w[i]), gp(grads->ln1_b[i]), i == 0 ? gp(grads->pos_embed_alpha) : nullptr));
+               gp(grads->ln1_w[i]), gp(grads->ln1_b[i]), i == 0 ? d_alpha : nullptr));
   }
   return DSX_OK;
+}
+
+}  // namespace dsx
+
+using namespace dsx;
+
+extern "C" {
+
+int dsx_fs2dec_train_create(int device, const dsx_fs2dec_config* cfg, dsx_fs2dec_train** out) {
+  DSX_CHECK(out, DSX_E_INVALID, "out is NULL");
+  *out = nullptr;
+  dsx_fs2dec* dec = nullptr;
+  DSX_TRY(dsx_fs2dec_create(device, cfg, &dec));   // validates the configuration and selects the device
+  dsx_fs2dec_train* h = new dsx_fs2dec_train();
+  h->device = device;
+  h->cfg = *cfg;
+  h->dec = dec;
+  auto fail = [&](int rc) {
+    dsx_fs2dec_train_destroy(h);
+    return rc;
+  };
+  int rc = DSX_OK;
+  if ((rc = fs2_train_alloc(dec))) return fail(rc);
+  if ((rc = []() -> int {
+         DSX_CUDA(cudaFuncSetAttribute(k_f2b_gemm<kNT>, cudaFuncAttributeMaxDynamicSharedMemorySize, conv_smem<kNT>()));
+         DSX_CUDA(cudaFuncSetAttribute(k_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem));
+         DSX_TRY(abwd_opt_in<64>());
+         return abwd_opt_in<128>();
+       }()))
+    return fail(rc);
+  const int H = cfg->hidden, k = cfg->kernel;
+  h->layers.resize(cfg->layers);
+  for (auto& l : h->layers) {
+    if ((rc = gemm_alloc(h->mem, l.in_t, 3 * H, H, 1)) || (rc = gemm_alloc(h->mem, l.out_t, H, H, 1)) ||
+        (rc = gemm_alloc(h->mem, l.ffn1_t, 4 * H, H, k)) || (rc = gemm_alloc(h->mem, l.ffn2_t, H, 4 * H, 1)))
+      return fail(rc);
+    l.ffn1_t.tap0 = -tap0_of(*cfg);   // gA[t] = sum_j W_j^T gC[t - tap0 - j]
+    l.ffn1_t.tstep = -1;
+  }
+  *out = h;
+  return DSX_OK;
+}
+
+void dsx_fs2dec_train_destroy(dsx_fs2dec_train* h) {
+  if (!h) return;
+  cudaSetDevice(h->device);
+  cudaDeviceSynchronize();
+  h->mem.free_all();
+  dsx_fs2dec_destroy(h->dec);
+  delete h;
+}
+
+int dsx_fs2dec_train_tape_bytes(dsx_fs2dec_train* h, int B, int T, size_t* out) {
+  DSX_CHECK(h && out, DSX_E_INVALID, "null handle or out");
+  DSX_TRY(check_geom(h, B, T));
+  *out = tape_carve(h->cfg, B, T, nullptr, nullptr);
+  return DSX_OK;
+}
+
+int dsx_fs2dec_train_workspace_bytes(dsx_fs2dec_train* h, int B, int T, size_t* out) {
+  DSX_CHECK(h && out, DSX_E_INVALID, "null handle or out");
+  DSX_TRY(check_geom(h, B, T));
+  *out = ws_bytes(h, B, T);
+  return DSX_OK;
+}
+
+int dsx_fs2dec_train_forward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const float* x, dsx_strides xs, int B,
+                             int T, float p_drop, uint64_t seed, void* tape, size_t tape_bytes, void* workspace,
+                             size_t workspace_bytes, float* out, void* stream) {
+  DSX_TRY(check_geom(h, B, T));
+  const dsx_fs2dec_config& c = h->cfg;
+  DSX_TRY(fs2t_check_params(w, c.layers, 1, "the parameters"));
+  DSX_CHECK(x && tape && workspace && out, DSX_E_INVALID, "x, tape, workspace and out must not be NULL");
+  DSX_CHECK(p_drop >= 0.f && p_drop < 1.f, DSX_E_INVALID, "dropout p = %g is outside [0, 1)", static_cast<double>(p_drop));
+  const size_t need = tape_carve(c, B, T, nullptr, nullptr);
+  DSX_CHECK(tape_bytes >= need, DSX_E_INVALID, "tape of %zu bytes is below the %zu this (B, T) needs", tape_bytes, need);
+  const size_t wneed = ws_bytes(h, B, T);
+  DSX_CHECK(workspace_bytes >= wneed, DSX_E_INVALID, "workspace of %zu bytes is below the %zu this (B, T) needs",
+            workspace_bytes, wneed);
+  DSX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  Tape tp;
+  DSX_TRY(fs2t_begin(h, w, B, T, p_drop, seed, tape, s, &tp));
+  Fs2Bufs fb = fs2_carve(h->dec, workspace, B, T);
+  fb.PAD = tp.pad;
+  fb.POS = tp.pos;
+  return fs2_forward_run(h->dec, x, xs, B, T, fb, out, s, &tp.tr);
+}
+
+int dsx_fs2dec_train_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* tape, const float* d_out,
+                              const dsx_fs2dec_params* grads, float* d_x, int B, int T, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+  DSX_TRY(check_geom(h, B, T));
+  const dsx_fs2dec_config& c = h->cfg;
+  DSX_TRY(fs2t_check_params(w, c.layers, 1, "the parameters"));
+  DSX_TRY(fs2t_check_params(grads, c.layers, 1, "the gradients"));
+  DSX_CHECK(tape && d_out && workspace, DSX_E_INVALID, "tape, d_out and workspace must not be NULL");
+  const size_t wneed = ws_bytes(h, B, T);
+  DSX_CHECK(workspace_bytes >= wneed, DSX_E_INVALID, "workspace of %zu bytes is below the %zu this (B, T) needs",
+            workspace_bytes, wneed);
+  DSX_CUDA(cudaSetDevice(h->device));
+  return fs2t_backward(h, w, tape, d_out, grads, d_x, const_cast<float*>(grads->pos_embed_alpha), B, T, workspace,
+                       static_cast<cudaStream_t>(stream));
 }
 
 int dsx_fs2dec_train_masks(dsx_fs2dec_train* h, uint64_t seed, float p_drop, int B, int T, uint8_t* const* out,

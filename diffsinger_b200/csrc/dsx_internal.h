@@ -400,6 +400,40 @@ void fs2_first_ln(const dsx_fs2dec* h, const float** w, const float** b);   // l
 // dsx_fs2dec_load with pos_embed_alpha optional (the encoder's FFTBlocks have none)
 int fs2_load(dsx_fs2dec* h, const dsx_fs2dec_params* p, void* stream);
 
+// ---- dsx_fs2enc.cu: the encoder's entry, shared by the eval forward and the encoder training step ----------------------
+// Positions (pos_mode 0, to w.POS), then x = sqrt(H) E[tok] + the addends + the position term, * dropout(drop) (site < 0:
+// none), * !pad -> w.X, w.PAD, xsave (or NULL) and layer 0's layer_norm1 of the stack -> A (fp16).  2 launches, 1 for
+// pos_mode 1.
+int fs2enc_entry(const dsx_fs2dec* stack, int pos_mode, const float* E, int vocab, const int64_t* tokens, int B, int T,
+                 const float* const* add, const dsx_strides* as, int rel_len, const Fs2Bufs& w, __half* A,
+                 const Fs2Drop& drop, float* xsave, cudaStream_t s);
+
+// ---- dsx_fs2train.cu: the decoder training step's stack, which the encoder training step (dsx_fs2enctrain.cu) also
+// drives -----------------------------------------------------------------------------------------------------------------
+// the regions of a dsx_fs2dec_train tape
+struct Fs2TrainTape {
+  Fs2TapeHdr* hdr;
+  uint8_t* pad;                // [F] padding flags
+  int* pos;                    // [F] positions of the decoder's entry (unused by the encoder step)
+  Fs2Train tr;
+};
+dsx_fs2dec* fs2t_stack(dsx_fs2dec_train* h);   // the forward's packs and kernels
+// dsx_fs2dec_train_tape_bytes for a (B, T) the caller has checked; with base, the regions of the tape at base to *t
+size_t fs2t_tape_carve(const dsx_fs2dec_train* h, int B, int T, void* base, Fs2TrainTape* t);
+// DSX_E_INVALID when a pointer of p is NULL (pos_embed_alpha only when alpha)
+int fs2t_check_params(const dsx_fs2dec_params* p, int L, int alpha, const char* what);
+// the training forward's steps before the stack's entry: packs w (forward and transposed backward packs), carves the tape
+// to *tp and writes its header (seed, p, B, T).  No allocation, no synchronisation.
+int fs2t_begin(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, int B, int T, float p_drop, uint64_t seed, void* tape,
+               cudaStream_t s, Fs2TrainTape* tp);
+// The backward of dsx_fs2dec_train_backward from d_out through the final LayerNorm and the L layers, with the tape's PAD
+// as the forward wrote it: every stack gradient through grads (pos_embed_alpha not read), d_x = the gradient at the entry's
+// dropout input, * !pad, * dropout(0) (or NULL), and d_alpha = sum d_x . table[pos] over the tape's positions (or NULL:
+// not computed).  workspace: dsx_fs2dec_train_workspace_bytes(B, T); B and T checked by the caller.
+int fs2t_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* tape, const float* d_out,
+                  const dsx_fs2dec_params* grads, float* d_x, float* d_alpha, int B, int T, void* workspace,
+                  cudaStream_t s);
+
 // ---- dsx_fftdiff.cu: the FFT denoiser of the sampler handle ---------------------------------------------------------
 int fft_create(int device, const dsx_fft_config* c, const dsx_fft_params* p, cudaStream_t s, FftDenoiser** out);
 void fft_destroy(FftDenoiser* f);

@@ -42,7 +42,10 @@ rebinds ``FastspeechEncoder``, ``FastspeechMIDIEncoder``, ``DurationPredictor`` 
 classes of ``diffsinger_b200.fs2enc``.  ``FS_ENCODERS['fft']`` looks the encoder up when it is called and
 ``FastSpeech2.__init__`` the other two, so the next ``FastSpeech2`` / ``FastSpeech2MIDI`` runs its encoder, duration
 predictor and length regulator on dsx; ``FastSpeech2.forward`` itself (the MIDI embeddings, the ``decoder_inp`` gather)
-stays the reference's.  ``modules.fastspeech.tts_modules`` keeps the reference's classes.
+stays the reference's.  ``modules.fastspeech.tts_modules`` keeps the reference's classes.  The dsx duration predictor
+runs in eval mode only, so training (``dsx_train``, where the encoders run their sm_90a training step) installs with
+``install_fs2_encoder(duration_predictor=False)``: the reference's ``DurationPredictor`` stays, and
+``FastSpeech2.add_dur`` trains it in eager PyTorch.  ``uninstall_fs2_encoder()`` restores whatever was swapped.
 """
 import importlib
 import sys
@@ -274,8 +277,9 @@ _fs2enc = {}
 _FS2ENC_NAMES = ("FastspeechEncoder", "FastspeechMIDIEncoder", "DurationPredictor", "LengthRegulator")
 
 
-def install_fs2_encoder():
+def install_fs2_encoder(duration_predictor=True):
     from . import fs2enc
+    names = _FS2ENC_NAMES if duration_predictor else tuple(n for n in _FS2ENC_NAMES if n != "DurationPredictor")
     for name in _FS2_MODULES:
         try:
             mod = importlib.import_module(name)
@@ -283,7 +287,7 @@ def install_fs2_encoder():
             if e.name is None or not name.startswith(e.name):      # a missing dependency, not a missing module
                 raise
             continue
-        for attr in _FS2ENC_NAMES:
+        for attr in names:
             if not hasattr(mod, attr):
                 continue
             _fs2enc.setdefault((name, attr), getattr(mod, attr))

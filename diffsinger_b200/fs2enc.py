@@ -12,8 +12,12 @@
 
 So a FastSpeech2 checkpoint loads with ``strict=True``.  The modules only hold the parameters: ``forward`` packs them into
 the library (once per storage and version, so again after ``load_state_dict`` or ``.to()``) and runs there.  There is no
-eager or CPU path and no training path: a CPU tensor or a module in training mode raises ``DsxError``.  Construction
-does not touch the GPU (FastSpeech2MIDI.__init__ builds and deletes a non-MIDI encoder).
+eager or CPU path: a CPU tensor raises ``DsxError``, and so does a module in training mode, except the encoders under the
+``dsx_train`` opt-in (hparams key or ``train=`` keyword): then a training-mode forward under autograd runs the sm_90a
+training step of ``diffsinger_b200.fs2enctrain`` (dropout p = hparams['dropout'], gradients for every parameter,
+``embed_tokens.weight`` included, and for the MIDI addends).  ``DurationPredictor`` has no training step: training keeps
+the reference's (``install_fs2_encoder(duration_predictor=False)``).  Construction does not touch the GPU
+(FastSpeech2MIDI.__init__ builds and deletes a non-MIDI encoder).
 """
 import ctypes
 import math
@@ -49,7 +53,8 @@ class RelPositionalEncoding(nn.Module):
 class FastspeechEncoder(PackedModule):
     _what = "FastSpeech2 encoder"
 
-    def __init__(self, embed_tokens, hidden_size=None, num_layers=None, kernel_size=None, num_heads=2, *, hparams=None):
+    def __init__(self, embed_tokens, hidden_size=None, num_layers=None, kernel_size=None, num_heads=2, *, hparams=None,
+                 train=None):
         super().__init__()
         hp = _get_hparams(hparams)
         hidden_size = hp['hidden_size'] if hidden_size is None else hidden_size          # tts_modules.py:311-314
@@ -64,7 +69,7 @@ class FastspeechEncoder(PackedModule):
             raise DsxError(f"embed_tokens must be an nn.Embedding of dim {stack.hidden}")
         self.hidden_size, self.num_layers, self.num_heads = stack.hidden, stack.layers, stack.heads
         self.kernel_size, self.padding, self.act = stack.kernel, padding, act
-        self.dropout = hp.get('dropout', 0.0)      # identity in eval mode, the only mode forward runs in
+        self.dropout = hp.get('dropout', 0.0)      # identity in eval mode; the training step's p under dsx_train
         self.layers = nn.ModuleList([TransformerEncoderLayer(self.hidden_size, self.kernel_size, self.num_heads, padding, act)
                                      for _ in range(self.num_layers)])
         self.layer_norm = nn.LayerNorm(self.hidden_size)
@@ -78,6 +83,27 @@ class FastspeechEncoder(PackedModule):
             self.embed_positions = SinusoidalPositionalEmbedding(self.hidden_size, self.padding_idx)
         self._rel_len = REL_POS_MAX_LEN
         self._cfg = _capi.Fs2EncConfig(stack=stack, vocab=embed_tokens.num_embeddings, pos=int(self.rel_pos))
+        self._dsx_train = bool(train if train is not None else hp.get("dsx_train", False))
+        self._dsx_trainer = None
+
+    def __getstate__(self):
+        # the library handles are ctypes pointers: copies (EMA deepcopy, torch.save of the module) make their own
+        state = self.__dict__.copy()
+        state["_dsx"], state["_wkey"], state["_keep"] = None, None, None
+        state["_dsx_trainer"] = None
+        return state
+
+    def _dsx_train_step(self):
+        vocab = self.embed_tokens.num_embeddings
+        if self._dsx_trainer is None or self._dsx_trainer.cfg.vocab != vocab:
+            from .fs2enctrain import Fs2EncTrainStep
+            cfg = _capi.Fs2EncConfig(stack=_fs2dec_config(self.hidden_size, self.num_layers, self.kernel_size,
+                                                          self.num_heads, self.padding, self.act, "enc", "encoder"),
+                                     vocab=vocab, pos=int(self.rel_pos))
+            if self._dsx_trainer is not None:
+                self._dsx_trainer.close()
+            object.__setattr__(self, "_dsx_trainer", Fs2EncTrainStep(cfg))
+        return self._dsx_trainer
 
     # -- library handle ---------------------------------------------------------------------------
     _lib_create, _lib_load, _lib_destroy = lib.dsx_fs2enc_create, lib.dsx_fs2enc_load, lib.dsx_fs2enc_destroy
@@ -99,7 +125,9 @@ class FastspeechEncoder(PackedModule):
         return self._run(txt_tokens, ())
 
     def _run(self, txt_tokens, addends):
-        _eval_only(self, self._what)
+        train = self.training and self._dsx_train and torch.is_grad_enabled()
+        if not train:
+            _eval_only(self, self._what)
         if txt_tokens is None or txt_tokens.dim() != 2 or txt_tokens.dtype.is_floating_point:
             raise DsxError(f"txt_tokens must be integer [B, T] (got {None if txt_tokens is None else tuple(txt_tokens.shape)})")
         _need_cuda(txt_tokens)
@@ -113,10 +141,11 @@ class FastspeechEncoder(PackedModule):
                 continue
             _need_cuda(a)
             try:
-                adds.append(a.float().expand(B, T, H))
+                a.expand(B, T, H)
             except RuntimeError:
                 raise DsxError(f"an embedding addend must broadcast to [B, T, {H}] = [{B}, {T}, {H}] "
                                f"(got {tuple(a.shape)})") from None
+            adds.append(a)
         out = torch.empty((B, T, H), device=dev, dtype=torch.float32)
         if B == 0 or T == 0:
             return out
@@ -125,9 +154,13 @@ class FastspeechEncoder(PackedModule):
         V = self.embed_tokens.num_embeddings
         if lo < 0 or hi >= V:
             raise DsxError(f"txt_tokens must be in [0, {V}) (got ids from {lo} to {hi})")
-        hnd = self._ensure(dev)
         if self.rel_pos:
             self._rel_len = max(self._rel_len, T)               # extend_pe keeps the longest table (:23-29)
+        if train:
+            from .fs2enctrain import fs2enc_train_forward
+            return fs2enc_train_forward(self, tok, adds + [None] * (3 - len(adds)))
+        adds = [None if a is None else a.float().expand(B, T, H) for a in adds]
+        hnd = self._ensure(dev)
         ptrs = (ctypes.c_void_p * 3)(*[a.data_ptr() if a is not None else None for a in adds + [None] * (3 - len(adds))])
         strides = (_capi.Strides * 3)(*[_strides_bct(a, (0, 2, 1)) if a is not None else _capi.Strides()
                                         for a in adds + [None] * (3 - len(adds))])

@@ -673,6 +673,61 @@ int dsx_fs2dec_train_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, c
 int dsx_fs2dec_train_masks(dsx_fs2dec_train* h, uint64_t seed, float p_drop, int B, int T, uint8_t* const* out,
                            void* stream);
 
+/* ---- FastSpeech2 encoder training step ------------------------------------------------------------------------------
+ * Replaces: FastspeechEncoder.forward(txt_tokens) (modules/fastspeech/tts_modules.py:310-347) and
+ * FastspeechMIDIEncoder.forward(txt_tokens, midi_embedding, midi_dur_embedding, slur_embedding)
+ * (modules/diffsinger_midi/fs2.py:11-36) in training mode, and their autograd backward: the gradient of every encoder
+ * parameter, embed_tokens.weight included, and of the MIDI addends.  The forward is dsx_fs2enc_forward's with dropout:
+ *   x = sqrt(H) E[tok] (+ midi_embedding + midi_dur_embedding + slur_embedding, left to right)
+ *       + positions (pos 0)  |  x * sqrt(H) + pe[t] (pos 1, RelPositionalEncoding, whose own dropout has p = 0)
+ *   x = dropout(x) (site 0), then FFTBlocks without pos_embed_alpha, padding mask txt_tokens == 0.
+ * Dropout is the decoder training step's: the same 1 + 3 L sites (site 0 above; per layer i, 1 + 3 i after out_proj,
+ * 2 + 3 i after the FFN activation, 3 + 3 i after ffn_2), the same (seed, site, frame, channel) keying and the same p, so
+ * dsx_fs2dec_train_masks on a dsx_fs2dec_train handle of cfg.stack returns exactly the masks of a forward with that seed
+ * and p.  The layers are the decoder step's (fp16 operands, fp32 accumulation, LayerNorm statistics, softmax state and
+ * residual stream).  The backward's fp16 operands are scaled by a power of two chosen on the device (from amax |d_out|)
+ * and divided out exactly, and the embedding gradient is that fp32 result times sqrt(H), so 2^k d_out gives exactly 2^k
+ * times every gradient and d_out = 0 exact zeros.  Gradients are bitwise reproducible: the embedding gradient sums each
+ * row's frames in a fixed order (a sort of the frames by token, then per-row sums; no atomics), at a cost that grows
+ * with B T and with vocab, not with their product.  No call allocates or synchronises the host: the tape and the
+ * workspace are the caller's.  A handle is independent of the other handles. */
+typedef struct dsx_fs2enc_train dsx_fs2enc_train;
+
+/* Accepts what dsx_fs2enc_create accepts (DSX_E_INVALID, "unsupported ..."). */
+int dsx_fs2enc_train_create(int device, const dsx_fs2enc_config* cfg, dsx_fs2enc_train** out);
+void dsx_fs2enc_train_destroy(dsx_fs2enc_train* h);
+
+/* Bytes of the tape of one forward over B utterances of T tokens (F = B T, each region rounded up to 256 bytes, a256):
+ *   D + a256(8 F)
+ * with D = dsx_fs2dec_train_tape_bytes of cfg.stack, whose tape comes first; the second region is a copy of the tokens,
+ * so the backward reads nothing the caller may have changed since the forward. */
+int dsx_fs2enc_train_tape_bytes(dsx_fs2enc_train* h, int B, int T, size_t* out);
+
+/* Bytes of the scratch workspace a forward or a backward over (B, T) needs; it holds nothing between calls. */
+int dsx_fs2enc_train_workspace_bytes(dsx_fs2enc_train* h, int B, int T, size_t* out);
+
+/* One training forward: out [B, T, H] contiguous fp32 from tokens, add, as and rel_len as dsx_fs2enc_forward takes them,
+ * with dropout p_drop in [0, 1) drawn from `seed`, and what the backward needs written to `tape` (at least
+ * dsx_fs2enc_train_tape_bytes).  The weights (fp32 device pointers; pos_embed_alpha not used) are packed to fp16 inside
+ * the call, on the stream; the backward uses the packs of the latest forward on the handle, so the weights must not
+ * change between a forward and the backward of its tape.  Several forwards may precede their backwards, each with its
+ * own tape. */
+int dsx_fs2enc_train_forward(dsx_fs2enc_train* h, const dsx_fs2enc_params* w, const int64_t* tokens, int B, int T,
+                             const float* const* add, const dsx_strides* as, int rel_len, float p_drop, uint64_t seed,
+                             void* tape, size_t tape_bytes, void* workspace, size_t workspace_bytes, float* out,
+                             void* stream);
+
+/* The backward of the forward that wrote `tape`, with that forward's B and T: d_out [B, T, H] contiguous.  Writes (does
+ * not accumulate) the fp32 gradient of every stack parameter through grads->stack (pos_embed_alpha not written) and
+ * grads->embed_w [vocab, H], every row: rows no token of the tape uses, and row 0 (padding_idx), are 0.  d_add, unless
+ * NULL, is [B, T, H] contiguous: the gradient of the sum of the addends, so of each addend (0 on padding tokens).  The
+ * tape is only read.  A (B, T) other than the tape's makes every gradient NaN (checked on the device).  The backward
+ * reads the handle's packs of the latest forward: a forward of other weights, on any stream, must not run before or
+ * during it. */
+int dsx_fs2enc_train_backward(dsx_fs2enc_train* h, const dsx_fs2enc_params* w, const void* tape, const float* d_out,
+                              const dsx_fs2enc_params* grads, float* d_add, int B, int T, void* workspace,
+                              size_t workspace_bytes, void* stream);
+
 /* ---- FFT denoiser training step -------------------------------------------------------------------------------------
  * Replaces: FFT.forward(spec, diffusion_step, cond) (usr/diff/candidate_decoder.py:50-100) in training mode, as
  * GaussianDiffusion.p_losses calls it with diff_decoder_type 'fft', and its autograd backward: the gradient of every
