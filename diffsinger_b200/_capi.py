@@ -37,10 +37,13 @@ SYMBOLS = (
     "dsx_fft_train_forward", "dsx_fft_train_backward",
     "dsx_fs2enc_train_create", "dsx_fs2enc_train_destroy", "dsx_fs2enc_train_tape_bytes",
     "dsx_fs2enc_train_workspace_bytes", "dsx_fs2enc_train_forward", "dsx_fs2enc_train_backward",
+    "dsx_durpred_train_create", "dsx_durpred_train_destroy", "dsx_durpred_train_tape_bytes",
+    "dsx_durpred_train_workspace_bytes", "dsx_durpred_train_forward", "dsx_durpred_train_backward",
+    "dsx_durpred_train_masks",
 )
 _VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy", "dsx_fs2dec_destroy",
          "dsx_fs2enc_destroy", "dsx_durpred_destroy", "dsx_train_destroy", "dsx_fs2dec_train_destroy",
-         "dsx_fft_train_destroy", "dsx_fs2enc_train_destroy")
+         "dsx_fft_train_destroy", "dsx_fs2enc_train_destroy", "dsx_durpred_train_destroy")
 
 
 class DsxError(RuntimeError):
@@ -227,6 +230,16 @@ lib.dsx_fs2enc_train_forward.argtypes = [_vp, ctypes.POINTER(Fs2EncParams), _vp,
                                          ctypes.c_size_t, _vp, _vp]
 lib.dsx_fs2enc_train_backward.argtypes = [_vp, ctypes.POINTER(Fs2EncParams), _vp, _vp, ctypes.POINTER(Fs2EncParams), _vp,
                                           _i, _i, _vp, ctypes.c_size_t, _vp]
+lib.dsx_durpred_train_create.argtypes = [_i, ctypes.POINTER(DurPredConfig), ctypes.POINTER(_vp)]
+lib.dsx_durpred_train_destroy.argtypes = [_vp]
+lib.dsx_durpred_train_destroy.restype = None
+lib.dsx_durpred_train_tape_bytes.argtypes = [_vp, _i, _i, ctypes.POINTER(ctypes.c_size_t)]
+lib.dsx_durpred_train_workspace_bytes.argtypes = [_vp, _i, _i, ctypes.POINTER(ctypes.c_size_t)]
+lib.dsx_durpred_train_forward.argtypes = [_vp, ctypes.POINTER(DurPredParams), _vp, Strides, _vp, _i, _i, ctypes.c_float,
+                                          _u64, _vp, ctypes.c_size_t, _vp, ctypes.c_size_t, _vp, _vp]
+lib.dsx_durpred_train_backward.argtypes = [_vp, ctypes.POINTER(DurPredParams), _vp, _vp, ctypes.POINTER(DurPredParams),
+                                           _vp, _i, _i, _vp, ctypes.c_size_t, _vp]
+lib.dsx_durpred_train_masks.argtypes = [_vp, _u64, ctypes.c_float, _i, _i, ctypes.POINTER(_vp), _vp]
 for _n in SYMBOLS:
     if _n not in _VOID:
         getattr(lib, _n).restype = _i

@@ -434,6 +434,35 @@ int fs2t_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* t
                   const dsx_fs2dec_params* grads, float* d_x, float* d_alpha, int B, int T, void* workspace,
                   cudaStream_t s);
 
+// ---- dsx_pe.cu: the duration predictor's layers, shared by its eval forward and its training step (dsx_durtrain.cu) ---
+// What the training forward saves, every pointer a tape region: layer i's fp16 input operand a[i] ([F][idim] for i = 0,
+// else [F][chans]; a[0] is the packed x), its LayerNorm input r[i] (conv + bias, ReLU; fp32 [F][chans]) and the head's
+// input hin (the last layer's output after dropout and * !mask, fp32 [F][chans]).  Dropout site i is layer i's.
+struct DurTrain {
+  uint64_t seed = 0;
+  float p = 0.f;
+  std::vector<__half*> a;
+  std::vector<float*> r;
+  float* hin = nullptr;
+  Fs2Drop drop(int site) const {
+    Fs2Drop d;
+    d.seed = seed;
+    d.p = p;
+    d.inv_keep = 1.f / (1.f - p);
+    d.site = site;
+    return d;
+  }
+};
+// The training step's forward packs live in a dsx_durpred handle: durpred_train_alloc sizes them once (the handle then
+// counts as loaded), durpred_train_pack refills them from the caller's fp32 weights on the stream (no allocation, no
+// synchronisation) and points the LayerNorm affines at the caller's arrays.
+int durpred_train_alloc(dsx_durpred* h);
+int durpred_train_pack(dsx_durpred* h, const dsx_durpred_params* p, cudaStream_t s);
+// x (any strides) -> tr.a[0], then the layers in training form (k_pe_conv<NT, true>): xs [B][T], 0 on padding.
+// 1 + n_layers launches.
+int durpred_train_run(const dsx_durpred* h, const float* x, dsx_strides xs_, const uint8_t* mask, int B, int T,
+                      const DurTrain& tr, float* xs, cudaStream_t s);
+
 // ---- dsx_fftdiff.cu: the FFT denoiser of the sampler handle ---------------------------------------------------------
 int fft_create(int device, const dsx_fft_config* c, const dsx_fft_params* p, cudaStream_t s, FftDenoiser** out);
 void fft_destroy(FftDenoiser* f);

@@ -62,6 +62,11 @@ struct PeConvArgs {
   float f0_mean, f0_std;
   int64_t* dur;                // PE_DUR: [B][T] or null (xs goes to o32 [B][T])
   float offset;
+  // the training form (k_pe_conv<NT, true>, PE_LN and PE_DUR): the LayerNorm input (bias + ReLU) -> r32 [B][T][n], the
+  // LayerNorm output * dropout(drop) before * !mask, and PE_DUR's head input (that, * !mask) -> h32 [B][T][n]
+  float* r32;
+  float* h32;
+  Fs2Drop drop;
 };
 
 template <int NT>
@@ -70,7 +75,7 @@ struct PeShape {
   static constexpr int NH = NT / WG;
 };
 
-template <int NT>
+template <int NT, bool TRAIN = false>
 __global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvArgs p) {
   constexpr int NH = PeShape<NT>::NH, WG = PeShape<NT>::WG;
   extern __shared__ uint8_t smem_raw[];
@@ -111,6 +116,13 @@ __global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvA
     float v = col < n ? acc[e] + __ldg(p.g.b + col) : 0.f;
     if (p.mode == PE_PRENET || p.mode == PE_LN || p.mode == PE_HEAD || p.mode == PE_DUR) v = fmaxf(v, 0.f);
     acc[e] = v;
+  }
+  if constexpr (TRAIN) {
+#pragma unroll
+    for (int e = 0; e < NH / 2; e += 2) {
+      const int col = c0 + acc_col(wtid, e), m = mrow[(e >> 1) & 1];
+      if (col < n && m < T) *reinterpret_cast<float2*>(p.r32 + (rbase + m) * n + col) = make_float2(acc[e], acc[e + 1]);
+    }
   }
 
   if (p.mode == PE_GN) {
@@ -177,6 +189,19 @@ __global__ void __launch_bounds__(128 * PeShape<NT>::WG) k_pe_conv(const PeConvA
       const bool hi = e & 2;
       acc[e] = col < n ? (acc[e] - (hi ? mean1 : mean0)) * (hi ? rstd1 : rstd0) * __ldg(p.scale + col) + __ldg(p.shift + col)
                        : 0.f;
+    }
+    if constexpr (TRAIN) {
+#pragma unroll
+      for (int e = 0; e < NH / 2; e += 2) {
+        const int col = c0 + acc_col(wtid, e), m = mrow[(e >> 1) & 1];
+        const float2 ds = dropout_scale2(p.drop, rbase + m, col);
+        acc[e] *= ds.x;
+        acc[e + 1] *= ds.y;
+        if (p.mode == PE_DUR && col < n && m < T) {
+          if (p.pad[rbase + m]) acc[e] = acc[e + 1] = 0.f;
+          *reinterpret_cast<float2*>(p.h32 + (rbase + m) * n + col) = make_float2(acc[e], acc[e + 1]);
+        }
+      }
     }
   }
 
@@ -620,6 +645,99 @@ struct dsx_durpred {
   GrowBuffer ws;
 };
 
+namespace {
+
+// DurationPredictor._forward (tts_modules.py:113-129): n_layers x [conv, ReLU, LayerNorm, (dropout), * !mask], then the
+// head, from layer 0's fp16 operand A[0].  Eval (tr == NULL) alternates A[0] and A[1]; training reads layer i's operand
+// from tr->a[i], writes layer i + 1's there, and saves the LayerNorm inputs and the head's input (DurTrain).
+int dp_layers(const dsx_durpred* h, __half* const* A, const uint8_t* mask, int B, int T, float* xs, int64_t* dur,
+              const DurTrain* tr, cudaStream_t s) {
+  const dsx_durpred_config& c = h->cfg;
+  const int P = c.chans;
+  int cur = 0;
+  for (int i = 0; i < c.layers; ++i) {
+    PeConvArgs a{};
+    a.T = T;
+    a.pad = mask;
+    a.x = tr ? tr->a[i] : A[cur];
+    a.scale = h->conv[i].s;
+    a.shift = h->conv[i].t;
+    if (i + 1 < c.layers) {
+      a.mode = PE_LN;
+      a.flags = PE_MASK | PE_OUT16;
+      a.o16 = tr ? tr->a[i + 1] : A[cur ^ 1];
+    } else {
+      a.mode = PE_DUR;
+      a.hw = h->head;
+      a.hb = h->head + P;
+      a.o32 = xs;
+      a.dur = dur;
+      a.offset = c.offset;
+    }
+    if (!tr) {
+      DSX_TRY(pe_run(h->conv[i], a, B, s));
+    } else {
+      a.r32 = tr->r[i];
+      a.h32 = tr->hin;
+      a.drop = tr->drop(i);
+      a.g = h->conv[i];
+      a.mtiles = (T + kConvRows - 1) / kConvRows;
+      DSX_TRY(conv_dispatch<256>(h->conv[i].nt, [&](auto k) {
+        constexpr int NT = decltype(k)::value;
+        k_pe_conv<NT, true><<<dim3(a.mtiles, B), 128 * PeShape<NT>::WG, conv_smem<NT>(), s>>>(a);
+        return launch_check("k_pe_conv");
+      }));
+    }
+    cur ^= 1;
+  }
+  return DSX_OK;
+}
+
+}  // namespace
+
+namespace dsx {
+
+int durpred_train_alloc(dsx_durpred* h) {
+  DSX_TRY(conv_opt_in<256>([](auto k) { return k_pe_conv<decltype(k)::value, true>; }));
+  const dsx_durpred_config& c = h->cfg;
+  for (int i = 0; i < c.layers; ++i) {
+    PePacked& pc = h->conv[i];
+    pc = PePacked{};
+    pc.cin = i ? c.chans : c.idim;
+    pc.n = c.chans;
+    pc.taps = c.kernel;
+    pc.tap0 = c.padding ? -(c.kernel - 1) : -(c.kernel - 1) / 2;
+    DSX_TRY(conv_alloc(h->mem, pc, 256));
+  }
+  DSX_TRY(h->mem.alloc(&h->head, (c.chans + 1) * sizeof(float)));
+  h->loaded = true;
+  return DSX_OK;
+}
+
+int durpred_train_pack(dsx_durpred* h, const dsx_durpred_params* p, cudaStream_t s) {
+  const dsx_durpred_config& c = h->cfg;
+  const int P = c.chans;
+  for (int i = 0; i < c.layers; ++i) {
+    PePacked& pc = h->conv[i];
+    DSX_TRY(conv_repack(pc, PackArgs{p->conv_w[i], nullptr, p->conv_b[i], pc.cin, P, P, c.kernel, 1, 0}, s));
+    pc.s = const_cast<float*>(p->ln_w[i]);
+    pc.t = const_cast<float*>(p->ln_b[i]);
+  }
+  DSX_CUDA(cudaMemcpyAsync(h->head, p->linear_w, P * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  DSX_CUDA(cudaMemcpyAsync(h->head + P, p->linear_b, sizeof(float), cudaMemcpyDeviceToDevice, s));
+  return DSX_OK;
+}
+
+int durpred_train_run(const dsx_durpred* h, const float* x, dsx_strides xs_, const uint8_t* mask, int B, int T,
+                      const DurTrain& tr, float* xs, cudaStream_t s) {
+  const size_t frames = static_cast<size_t>(B) * T;
+  k_dp_pack<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(x, xs_, B, T, h->cfg.idim, tr.a[0]);
+  DSX_TRY(launch_check("k_dp_pack"));
+  return dp_layers(h, nullptr, mask, B, T, xs, nullptr, &tr, s);
+}
+
+}  // namespace dsx
+
 extern "C" {
 
 int dsx_durpred_create(int device, const dsx_durpred_config* c, dsx_durpred** out) {
@@ -710,31 +828,7 @@ int dsx_durpred_forward(dsx_durpred* h, const float* x, dsx_strides xs_, const u
   __half* A[2] = {ws.take<__half>(frames * C * 2), ws.take<__half>(frames * C * 2)};
   k_dp_pack<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(x, xs_, B, T, c.idim, A[0]);
   DSX_TRY(launch_check("k_dp_pack"));
-  // DurationPredictor._forward (tts_modules.py:113-129): n_layers x [conv, ReLU, LayerNorm, * !mask], then the head
-  int cur = 0;
-  for (int i = 0; i < c.layers; ++i) {
-    PeConvArgs a{};
-    a.T = T;
-    a.pad = mask;
-    a.x = A[cur];
-    a.scale = h->conv[i].s;
-    a.shift = h->conv[i].t;
-    if (i + 1 < c.layers) {
-      a.mode = PE_LN;
-      a.flags = PE_MASK | PE_OUT16;
-      a.o16 = A[cur ^ 1];
-    } else {
-      a.mode = PE_DUR;
-      a.hw = h->head;
-      a.hb = h->head + P;
-      a.o32 = xs;
-      a.dur = dur;
-      a.offset = c.offset;
-    }
-    DSX_TRY(pe_run(h->conv[i], a, B, s));
-    cur ^= 1;
-  }
-  return DSX_OK;
+  return dp_layers(h, A, mask, B, T, xs, dur, nullptr, s);
 }
 
 }  // extern "C"

@@ -42,10 +42,11 @@ rebinds ``FastspeechEncoder``, ``FastspeechMIDIEncoder``, ``DurationPredictor`` 
 classes of ``diffsinger_b200.fs2enc``.  ``FS_ENCODERS['fft']`` looks the encoder up when it is called and
 ``FastSpeech2.__init__`` the other two, so the next ``FastSpeech2`` / ``FastSpeech2MIDI`` runs its encoder, duration
 predictor and length regulator on dsx; ``FastSpeech2.forward`` itself (the MIDI embeddings, the ``decoder_inp`` gather)
-stays the reference's.  ``modules.fastspeech.tts_modules`` keeps the reference's classes.  The dsx duration predictor
-runs in eval mode only, so training (``dsx_train``, where the encoders run their sm_90a training step) installs with
-``install_fs2_encoder(duration_predictor=False)``: the reference's ``DurationPredictor`` stays, and
-``FastSpeech2.add_dur`` trains it in eager PyTorch.  ``uninstall_fs2_encoder()`` restores whatever was swapped.
+stays the reference's.  ``modules.fastspeech.tts_modules`` keeps the reference's classes.  Under ``dsx_train`` the
+encoders and the duration predictor run their sm_90a training steps; ``FastSpeech2.add_dur``'s ``predictor_grad``
+scaling of the predictor's input stays in the reference's graph.  ``install_fs2_encoder(duration_predictor=False)``
+leaves the reference's ``DurationPredictor`` in place, so it trains in eager PyTorch.  ``uninstall_fs2_encoder()``
+restores whatever was swapped.
 """
 import importlib
 import sys

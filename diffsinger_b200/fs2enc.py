@@ -15,8 +15,9 @@ the library (once per storage and version, so again after ``load_state_dict`` or
 eager or CPU path: a CPU tensor raises ``DsxError``, and so does a module in training mode, except the encoders under the
 ``dsx_train`` opt-in (hparams key or ``train=`` keyword): then a training-mode forward under autograd runs the sm_90a
 training step of ``diffsinger_b200.fs2enctrain`` (dropout p = hparams['dropout'], gradients for every parameter,
-``embed_tokens.weight`` included, and for the MIDI addends).  ``DurationPredictor`` has no training step: training keeps
-the reference's (``install_fs2_encoder(duration_predictor=False)``).  Construction does not touch the GPU
+``embed_tokens.weight`` included, and for the MIDI addends).  ``DurationPredictor`` under the same opt-in runs the
+training step of ``diffsinger_b200.durtrain`` in ``forward`` (dropout p = its ``dropout_rate``, gradients for every
+parameter and for its input); ``.inference()`` stays eval-only.  Construction does not touch the GPU
 (FastSpeech2MIDI.__init__ builds and deletes a non-MIDI encoder).
 """
 import ctypes
@@ -200,7 +201,7 @@ def _durpred_config(idim, n_layers, n_chans, kernel_size, offset, padding):
 
 class DurationPredictor(PackedModule):
     def __init__(self, idim, n_layers=2, n_chans=384, kernel_size=3, dropout_rate=0.1, offset=1.0, padding='SAME', *,
-                 hparams=None):
+                 hparams=None, train=None):
         super().__init__()
         hp = _get_hparams(hparams)
         if hp['dur_loss'] != 'mse':
@@ -208,6 +209,9 @@ class DurationPredictor(PackedModule):
                            "the one out2dur implements)")
         self._cfg = _durpred_config(idim, n_layers, n_chans, kernel_size, offset, padding)
         self.offset, self.kernel_size, self.padding = offset, kernel_size, padding
+        self.dropout_rate = float(dropout_rate)      # identity in eval mode; the training step's p under dsx_train
+        self._dsx_train = bool(train if train is not None else hp.get("dsx_train", False))
+        self._dsx_trainer = None
         self.conv = nn.ModuleList()
         for idx in range(n_layers):                                          # tts_modules.py:82-93
             in_chans = idim if idx == 0 else n_chans
@@ -222,6 +226,19 @@ class DurationPredictor(PackedModule):
 
     _lib_create, _lib_load, _lib_destroy = lib.dsx_durpred_create, lib.dsx_durpred_load, lib.dsx_durpred_destroy
 
+    def __getstate__(self):
+        # the library handles are ctypes pointers: copies (EMA deepcopy, torch.save of the module) make their own
+        state = self.__dict__.copy()
+        state["_dsx"], state["_wkey"], state["_keep"] = None, None, None
+        state["_dsx_trainer"] = None
+        return state
+
+    def _dsx_train_step(self):
+        if self._dsx_trainer is None:
+            from .durtrain import DurTrainStep
+            object.__setattr__(self, "_dsx_trainer", DurTrainStep(self._cfg))
+        return self._dsx_trainer
+
     def _config(self):
         return self._cfg
 
@@ -234,12 +251,17 @@ class DurationPredictor(PackedModule):
                                    linear_w=t("linear.weight"), linear_b=t("linear.bias"))
 
     def _run(self, xs, x_masks, with_dur):
-        _eval_only(self, "DurationPredictor")
+        train = self.training and self._dsx_train and torch.is_grad_enabled() and not with_dur
+        if not train:
+            _eval_only(self, "DurationPredictor")
         if xs is None or xs.dim() != 3 or xs.shape[-1] != self._cfg.idim:
             raise DsxError(f"xs must be [B, T, {self._cfg.idim}] (got {None if xs is None else tuple(xs.shape)})")
         if x_masks is None or tuple(x_masks.shape) != tuple(xs.shape[:2]):
             raise DsxError("x_masks must be the [B, T] padding mask (the reference needs it too)")
         _need_cuda(xs, x_masks)
+        if train:
+            from .durtrain import durpred_train_forward
+            return durpred_train_forward(self, xs, x_masks), None
         dev = xs.device
         B, T, _ = xs.shape
         out = torch.empty((B, T), device=dev, dtype=torch.float32)

@@ -559,6 +559,60 @@ int dsx_durpred_load(dsx_durpred* h, const dsx_durpred_params* p, void* stream);
 int dsx_durpred_forward(dsx_durpred* h, const float* x, dsx_strides xs_, const uint8_t* mask, int B, int T, float* xs,
                         int64_t* dur, void* stream);
 
+/* ---- Duration predictor training step -------------------------------------------------------------------------------
+ * Replaces: DurationPredictor._forward(xs, x_masks) (modules/fastspeech/tts_modules.py:106-120, dur_loss 'mse') in
+ * training mode, and its autograd backward: the gradient of every parameter and of xs.  Layer i is ConstantPad1d + Conv1d,
+ * ReLU, LayerNorm over channels (eps 1e-12), Dropout(p) (site i), * !mask; then Linear(chans, 1), * !mask.  Masks come
+ * from Philox4x32-10 keyed by (seed, site, token, channel), as in the other training steps: the same seed and p give the
+ * same masks, with torch's distribution (keep 1 - p, kept values scaled by 1 / (1 - p)) but not its stream.  The
+ * convolutions run on dsx_durpred_forward's kernel with fp16 operands and fp32 accumulation; LayerNorm, the head and every
+ * gradient are fp32.  At p = 0 the training forward's xs equals dsx_durpred_forward's bit for bit.  The backward scales its
+ * fp16 gradient operands by a power of two S chosen on the device (S amax |d_xs * !mask| in [2^5, 2^6)) and divides it
+ * out exactly, so 2^k d_xs gives exactly 2^k times every gradient and d_xs = 0 exact zeros.  Gradients are bitwise
+ * reproducible (fixed-order reductions, no atomics).  No call allocates or synchronises the host: the tape and the
+ * workspace are the caller's.  A handle is independent of the other handles. */
+typedef struct dsx_durpred_train dsx_durpred_train;
+
+/* Accepts what dsx_durpred_create accepts (DSX_E_INVALID, "unsupported ...").  offset is not used. */
+int dsx_durpred_train_create(int device, const dsx_durpred_config* cfg, dsx_durpred_train** out);
+void dsx_durpred_train_destroy(dsx_durpred_train* h);
+
+/* Bytes of the tape of one forward over B utterances of T tokens (F = B T, P = chans, L = layers, each region rounded up
+ * to 256 bytes, a256):
+ *   a256(24) + a256(F) + a256(2 F idim) + L a256(4 F P) + (L - 1) a256(2 F P) + a256(4 F P)
+ * the header (seed, p, B, T), a copy of the mask, each layer's fp16 input, each layer's LayerNorm input and the head's
+ * input.  The masks are not stored: the backward draws them again from the seed and p the tape records. */
+int dsx_durpred_train_tape_bytes(dsx_durpred_train* h, int B, int T, size_t* out);
+
+/* Bytes of the scratch workspace a backward over (B, T) needs; it holds nothing between calls. */
+int dsx_durpred_train_workspace_bytes(dsx_durpred_train* h, int B, int T, size_t* out);
+
+/* One training forward: xs [B, T] contiguous fp32 (0 on padding tokens) of x (fp32, logically [B, T, idim], element
+ * strides xs_: b, c = channel, t) and mask (uint8 [B, T] contiguous, 1 = padding), with dropout p_drop in [0, 1) drawn
+ * from `seed`, and what the backward needs written to `tape` (at least dsx_durpred_train_tape_bytes).  The weights (fp32
+ * device pointers, dsx_durpred_load's struct) are packed to fp16 inside the call, on the stream, into the handle, so
+ * calls on one handle must not overlap on different streams.  The forward uses no workspace: workspace may be NULL and
+ * workspace_bytes 0.  Several forwards may precede their backwards, each with its own tape. */
+int dsx_durpred_train_forward(dsx_durpred_train* h, const dsx_durpred_params* w, const float* x, dsx_strides xs_,
+                              const uint8_t* mask, int B, int T, float p_drop, uint64_t seed, void* tape,
+                              size_t tape_bytes, void* workspace, size_t workspace_bytes, float* xs, void* stream);
+
+/* The backward of the forward that wrote `tape`, with that forward's B and T and weights w: d_xs [B, T] contiguous.
+ * Writes (does not accumulate) the fp32 gradient of every parameter through `grads` (same layout as w), and d_x
+ * [B, T, idim] contiguous unless NULL: autograd's gradient of x, which is nonzero on a padding token within the
+ * convolution's reach of a real one (the reference does not mask its input).  The tape is only read.  A (B, T) other than
+ * the tape's makes every gradient NaN (checked on the device).  The call packs w's transposed convolutions into the
+ * handle: calls on one handle must not overlap on different streams.  A scaled fp16 gradient operand beyond fp16's range
+ * saturates at +-65504 rather than becoming inf. */
+int dsx_durpred_train_backward(dsx_durpred_train* h, const dsx_durpred_params* w, const void* tape, const float* d_xs,
+                               const dsx_durpred_params* grads, float* d_x, int B, int T, void* workspace,
+                               size_t workspace_bytes, void* stream);
+
+/* Test entry: the n_layers keep masks (1 kept, 0 dropped) that dsx_durpred_train_forward(seed, p_drop) draws, in site
+ * (layer) order; out is a HOST array of n_layers device pointers to uint8 [B, T, chans]. */
+int dsx_durpred_train_masks(dsx_durpred_train* h, uint64_t seed, float p_drop, int B, int T, uint8_t* const* out,
+                            void* stream);
+
 /* ---- Length regulator ------------------------------------------------------------------------------------------------
  * Replaces: LengthRegulator.forward(dur, dur_padding, alpha) (modules/fastspeech/tts_modules.py:159-189) in two calls,
  * because T_mel depends on the data, without its [B, T_txt, T_mel] temporaries.  Both run on the current device.
