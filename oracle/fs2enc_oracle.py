@@ -39,11 +39,12 @@ def stack_hp(hp):
                 num_heads=hp['num_heads'], ffn_padding=hp['ffn_padding'], ffn_act=hp['ffn_act'])
 
 
-def rel_table(P, H):
-    """RelPositionalEncoding's table of length P (extend_pe with reverse=True, :23-45) -> [P, H]"""
-    pe = torch.zeros(P, H)
-    position = torch.arange(P - 1, -1, -1.0, dtype=torch.float32).unsqueeze(1)
-    div_term = torch.exp(torch.arange(0, H, 2, dtype=torch.float32) * -(math.log(10000.0) / H))
+def rel_table(P, H, dtype=torch.float32):
+    """RelPositionalEncoding's table of length P (extend_pe with reverse=True, :23-45) -> [P, H] (``dtype`` gives a
+    reference-precision table)"""
+    pe = torch.zeros(P, H, dtype=dtype)
+    position = torch.arange(P - 1, -1, -1.0, dtype=dtype).unsqueeze(1)
+    div_term = torch.exp(torch.arange(0, H, 2, dtype=dtype) * -(math.log(10000.0) / H))
     pe[:, 0::2] = torch.sin(position * div_term)
     pe[:, 1::2] = torch.cos(position * div_term)
     return pe
@@ -51,17 +52,18 @@ def rel_table(P, H):
 
 def embedding(sd, tokens, hp, addends=(), rel_len=REL_MAX_LEN):
     """forward_embedding (tts_modules.py:339-347, diffsinger_midi/fs2.py:12-23): [B, T, H], padding rows not masked.
-    ``addends``: midi_embedding, midi_dur_embedding, slur_embedding ([B, T, H] or 0) for the MIDI encoder."""
+    ``addends``: midi_embedding, midi_dur_embedding, slur_embedding ([B, T, H] or 0) for the MIDI encoder.  The position
+    tables are built in the embedding's dtype (float32 in the reference; float64 for the edge tests)."""
     H = int(hp['hidden_size'])
     x = math.sqrt(H) * F.embedding(tokens, sd["embed_tokens.weight"], 0)
     if addends:
         midi, dur, slur = addends
         x = x + midi + dur + slur
     if hp.get('rel_pos'):
-        x = x * math.sqrt(H) + rel_table(max(rel_len, tokens.shape[1]), H).to(x)[None, :tokens.shape[1]]
+        x = x * math.sqrt(H) + rel_table(max(rel_len, tokens.shape[1]), H, x.dtype).to(x)[None, :tokens.shape[1]]
     else:
         T = tokens.shape[1]
-        table = sinusoidal_table(max(2000, 1 + T), H).to(x)
+        table = sinusoidal_table(max(2000, 1 + T), H, dtype=x.dtype).to(x)
         x = x + table.index_select(0, make_positions(tokens).view(-1)).view(*tokens.shape, -1)
     return x
 

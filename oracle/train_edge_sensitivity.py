@@ -10,8 +10,9 @@ step's own); they change what a mutation hits by sampling noise only.
 
     python -m oracle.train_edge_sensitivity [mutation ...]
 
-Inside the oracles every linear, conv1d and attention runs through Mutable (F.linear, F.conv1d and
-F.multi_head_attention_forward are patched for the run), and so does the residual stream entering each layer.  With no
+Inside the oracles every linear, conv1d, attention, embedding and LayerNorm runs through Mutable (F.linear, F.conv1d,
+F.multi_head_attention_forward, F.embedding and F.layer_norm are patched for the run), and so does the residual stream
+entering each layer of the decoder, the FFT denoiser and DiffNet.  With no
 mutation switched on, Mutable's backward is autograd's own (tests/test_oracle_train_edges.py checks this exactly)."""
 import contextlib
 import importlib.util
@@ -21,8 +22,11 @@ import sys
 import torch
 import torch.nn.functional as F
 
+from oracle.fs2enc_oracle import REL_MAX_LEN
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_conv1d, _linear, _mha = F.conv1d, F.linear, F.multi_head_attention_forward
+_conv1d, _linear, _mha, _embedding, _layer_norm = (F.conv1d, F.linear, F.multi_head_attention_forward, F.embedding,
+                                                   F.layer_norm)
 CPU = torch.device("cpu")
 
 
@@ -174,22 +178,71 @@ def residual_gradient_zeroed(kind):
     return mutate
 
 
+def sorted_chunks(tokens, V):
+    """[F] per frame of tokens (flat): its token as the embedding gradient sorts it (ids outside [1, V) as 0) and the
+    64-frame chunk of the stable sort of the frames by token it lands in"""
+    tok = tokens.reshape(-1)
+    key = torch.where((tok > 0) & (tok < V), tok, torch.zeros_like(tok))
+    order = torch.argsort(key * tok.numel() + torch.arange(tok.numel(), device=tok.device))
+    chunk = torch.empty_like(order)
+    chunk[order] = torch.arange(tok.numel(), device=tok.device) // 64
+    return key, chunk
+
+
+def embedding_without_last_piece(tokens):
+    """7. the embedding gradient: a token whose sorted run spans several 64-frame chunks loses its piece in the last"""
+    def mutate(fn, xs, g):
+        key, chunk = sorted_chunks(tokens, xs[0].shape[0])
+        drop = torch.zeros_like(key, dtype=torch.bool)
+        for v in key.unique().tolist():
+            sel = key == v
+            if v != 0 and chunk[sel].min() < chunk[sel].max():
+                drop |= sel & (chunk == chunk[sel].max())
+        return autograd_grads(fn, xs, g * ~drop.view(*tokens.shape, 1))
+    return mutate
+
+
+def layer_norm_without_mean_term(fn, xs, g):
+    """8. LayerNorm's data gradient drops its mean term (rstd mean(w g)) on the last partial 64-row tile ([B, T, C])"""
+    grads = autograd_grads(fn, xs, g)
+    x, w, _ = xs
+    if grads[0] is None:
+        return grads
+    x = x.detach()
+    rstd = (x.var(-1, unbiased=False, keepdim=True) + fn.eps).rsqrt()
+    m = tile_mask(STATE["B"], STATE["T"]).to(x.device)[:, :, None]
+    grads[0] = grads[0] + rstd * (g * w.detach()).mean(-1, keepdim=True) * m
+    return grads
+
+
+# the shared layers' mutations (tests/test_oracle_train_edges.py checks each on the decoder, the dilated-conv one on
+# DiffNet), then the encoder's and the duration predictor's own
 MUTATIONS = ["wgrad: last partial 64-frame chunk missing", "conv wgrad: shifted operand reads the neighbour",
              "attention: dQ misses the last key block", "attention: dK, dV miss the last query block",
              "ffn_1 dgrad: last tap one frame off", "residual gradient zeroed on the last partial tile"]
+OWN_MUTATIONS = ["embedding: a run loses its last 64-frame chunk piece",
+                 "durpred LayerNorm dgrad: no mean term on the last partial tile"]
+ALL_MUTATIONS = MUTATIONS + OWN_MUTATIONS
+
+
+def kernel_size(step, c):
+    return {"diffnet": lambda: 3, "durpred": lambda: c["hp"]["k"],
+            "fs2enc": lambda: c["hp"]["enc_ffn_kernel_size"]}.get(step, lambda: c["hp"]["dec_ffn_kernel_size"])()
 
 
 def applies(mutation, step, c):
     B, T = c["B"], c["T"]
-    k = 3 if step == "diffnet" else c["hp"]["dec_ffn_kernel_size"]
-    return {MUTATIONS[0]: B * T % 64 != 0, MUTATIONS[1]: B > 1 and k > 1,
-            MUTATIONS[2]: step != "diffnet" and T % 64 != 0, MUTATIONS[3]: step != "diffnet" and T % 64 != 0,
-            MUTATIONS[4]: step != "diffnet" and k > 1, MUTATIONS[5]: T % 64 != 0}[mutation]
+    k = kernel_size(step, c)
+    attn = step in ("fs2", "fft", "fs2enc")
+    M = ALL_MUTATIONS
+    return {M[0]: B * T % 64 != 0, M[1]: B > 1 and k > 1, M[2]: attn and T % 64 != 0, M[3]: attn and T % 64 != 0,
+            M[4]: step != "diffnet" and k > 1, M[5]: step in ("fs2", "fft", "diffnet") and T % 64 != 0,
+            M[6]: step == "fs2enc" and B * T > 64, M[7]: step == "durpred" and T % 64 != 0}[mutation]
 
 
 # ---- the patched ops ------------------------------------------------------------------------------------------------
 def _on(i):
-    return STATE["mutation"] == MUTATIONS[i]
+    return STATE["mutation"] == ALL_MUTATIONS[i]
 
 
 def conv1d(x, w, b=None, stride=1, padding=0, dilation=1, groups=1):
@@ -216,6 +269,18 @@ def multi_head_attention_forward(query, key, value, embed_dim, num_heads, in_pro
     return linear(o.permute(2, 0, 1, 3).reshape(T, B, E), out_proj_weight, out_proj_bias), None
 
 
+def embedding(input, weight, padding_idx=None, *args, **kwargs):
+    fn = lambda w_: _embedding(input, w_, padding_idx, *args, **kwargs)
+    return Mutable.apply(fn, embedding_without_last_piece(input) if _on(6) else None, weight)
+
+
+def layer_norm(input, normalized_shape, weight=None, bias=None, eps=1e-5):
+    fn = lambda x_, w_, b_: _layer_norm(x_, normalized_shape, w_, b_, eps)
+    fn.eps = eps
+    mutate = layer_norm_without_mean_term if _on(7) and STATE["step"] == "durpred" else None
+    return Mutable.apply(fn, mutate, input, weight, bias)
+
+
 def layer_input(kind):
     """the residual stream entering layer i, through Mutable (zeroed on the last partial tile for one layer)"""
     def hook(i, x):
@@ -226,17 +291,18 @@ def layer_input(kind):
 
 @contextlib.contextmanager
 def patched():
-    saved = F.conv1d, F.linear, F.multi_head_attention_forward
-    F.conv1d, F.linear, F.multi_head_attention_forward = conv1d, linear, multi_head_attention_forward
+    saved = F.conv1d, F.linear, F.multi_head_attention_forward, F.embedding, F.layer_norm
+    F.conv1d, F.linear, F.multi_head_attention_forward, F.embedding, F.layer_norm = (
+        conv1d, linear, multi_head_attention_forward, embedding, layer_norm)
     try:
         yield
     finally:
-        F.conv1d, F.linear, F.multi_head_attention_forward = saved
+        F.conv1d, F.linear, F.multi_head_attention_forward, F.embedding, F.layer_norm = saved
 
 
 # ---- the cases -------------------------------------------------------------------------------------------------------
 def seeded_masks(hp, B, T, seed=5):
-    H, L, p = hp["hidden_size"], hp["dec_layers"], hp["dropout"]
+    H, L, p = hp["hidden_size"], hp.get("dec_layers", hp.get("enc_layers")), hp["dropout"]
     gen = torch.Generator().manual_seed(seed)
     return [torch.rand(B, T, n, generator=gen) >= p for n in [H] + [H, 4 * H, H] * L]
 
@@ -244,7 +310,7 @@ def seeded_masks(hp, B, T, seed=5):
 def case_runner(E, step, name):
     """run(mode) -> (primary, d_input, grads) of the case's reference in float64 on the CPU; and errors(res, ref)"""
     c = E.CASES[step][name]
-    STATE.update(step=step, layer=(c["L"] if step == "diffnet" else c["hp"]["dec_layers"]) // 2)
+    STATE.update(step=step, layer=(c["L"] if step == "diffnet" else c["hp"].get("dec_layers", 0)) // 2)
     if step == "fs2":
         hp, sd, x, g = E.fs2_case(name)
         idx = [b for b in range(c["B"]) if b != c.get("empty")]
@@ -257,17 +323,38 @@ def case_runner(E, step, name):
         masks = seeded_masks(hp, c["B"], c["T"])
         run = lambda: E.fft_ref(hp, sd, spec, t, cond, g, masks, "f64", CPU, layer_input("linear"))
         keep, names = None, ("eps", "d_cond")
+    elif step == "fs2enc":
+        hp, sd, tok, adds, g = E.enc_case(name)
+        idx = [b for b in range(c["B"]) if b != c.get("empty")]
+        tok, adds, g = tok[idx], [a[idx] for a in adds], g[idx]
+        masks = seeded_masks(hp, len(idx), c["T"])
+        rel_len = c["T"] if c.get("rel_len") == "T" else max(REL_MAX_LEN, c["T"])
+        used = E.used_rows(tok, sd["encoder.embed_tokens.weight"].shape[0])
+
+        def run():
+            out, d_add, grads = E.enc_ref(hp, sd, tok, adds, g, masks, rel_len, "f64", CPU)
+            return out, d_add, E.embed_rows(grads, used)
+        keep, names = tok != 0, ("out", "d_add")
+    elif step == "durpred":
+        hp, sd, x, mask, g = E.dur_case(name)
+        gen = torch.Generator().manual_seed(5)
+        masks = [torch.rand(c["B"], c["T"], hp["P"], generator=gen) >= hp["p"] for _ in range(hp["L"])]
+
+        def run():
+            xs, d_x, grads = E.dur_ref(hp, sd, x, mask, g, masks, "f64", CPU)
+            return xs[..., None], d_x, grads
+        keep, names = (~mask, None), ("xs", "d_x")
     else:
         net, spec, t, cond, g = E.diffnet_case(name)
         run = lambda: E.diffnet_ref(net, spec, t, cond, g, "f64", CPU, layer_input("conv"))
         keep, names = None, ("eps", "d_cond")
-    STATE.update(B=len(keep) if keep is not None else c["B"], T=c["T"])
+    STATE.update(B=len(keep[0] if isinstance(keep, tuple) else keep) if keep is not None else c["B"], T=c["T"])
     return run, lambda res, ref: E.errors(res, ref, names, keep, c.get("peak", False))
 
 
 def main(argv):
     E = load_tests()
-    chosen = [m for m in MUTATIONS if not argv or any(a in m for a in argv)]
+    chosen = [m for m in ALL_MUTATIONS if not argv or any(a in m for a in argv)]
     print(f"{'mutation':50s} {'case':32s} {'rel':>8s} {'bound':>7s} {'frame':>8s} {'bound':>7s} {'row':>8s} "
           f"{'bound':>7s}  caught  by rel")
     summary = {m: [0, 0, 0] for m in chosen}           # cases run, caught, caught by rel

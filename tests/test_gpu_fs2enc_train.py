@@ -223,15 +223,27 @@ def test_several_forwards_before_their_backwards():
 def test_no_access_outside_the_buffers():
     """Every buffer of a step sits between NaN-filled guard regions; the results must equal an unguarded run's bit for
     bit and the guards must stay NaN."""
+    guarded_step(256, 2, 130, VOCAB, 77)
+
+
+@pytest.mark.parametrize("H,heads,T,vocab", [(64, 1, 65, 1), (64, 1, 65, 70000)])
+def test_no_access_outside_the_buffers_at_edges(H, heads, T, vocab):
+    """test_no_access_outside_the_buffers at H 64 with one head, over a one-row (all padding) and a 70000-row
+    vocabulary"""
+    guarded_step(H, heads, T, vocab, T - T // 4)
+
+
+def guarded_step(H, heads, T, vocab, tail):
+    """one step of B = 2 (utterance 1 padding from `tail` on) with every buffer between guard regions"""
     import ctypes
     from diffsinger_b200 import _capi, fs2enctrain
     from diffsinger_b200._capi import check, lib
     from diffsinger_b200.sampler import _ptr, _stream, _strides_bct
-    m, sd = model(HP)
+    m, sd = model(dict(HP, hidden_size=H, num_heads=heads), vocab=vocab)
     step = m._dsx_train_step()
     names = fs2enctrain.param_names(m.num_layers, m.padding)
-    B, T, H = 2, 130, 256
-    tok, adds, _ = inputs(B, T, (None, 77), sd)
+    B = 2
+    tok, adds, _ = inputs(B, T, (None, tail), sd, vocab=vocab)
     g = torch.randn(B, T, H, device=DEV)
     o_ref, g_ref, d_ref = raw_step(m, tok, adds, 8, g)
     GUARD = 4096
