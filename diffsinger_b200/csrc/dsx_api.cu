@@ -43,7 +43,7 @@ int ensure_workspace(dsx_handle* h, const Geom& g, int rows, cudaStream_t s) {
       if (cond_before[0] != w.CONDH || cond_before[1] != w.CP) h->cond_ready = false;
     } else {
       const void* cond_before = w.CONDF;
-      DSX_TRY(w.G1.reserve_zeroed(nf * 2 * m.C * 4, s));
+      DSX_TRY(w.G1.reserve_zeroed(nf * simt_g1_cols(m) * 4, s));
       DSX_TRY(w.Zf.reserve_zeroed(nf * m.C * 4, s));
       DSX_TRY(w.CONDF.reserve_zeroed(nf * m.H * 4, s));
       if (cond_before != w.CONDF) h->cond_ready = false;
@@ -346,6 +346,15 @@ int dsx_load_diffnet(dsx_handle* h, const dsx_diffnet_params* p, int M, int C, i
   DSX_CHECK(precision == DSX_PREC_FP32_SIMT || precision == DSX_PREC_FP16 || precision == DSX_PREC_FP16X2 ||
                 precision == DSX_PREC_FP16X3 || precision == DSX_PREC_FP16S,
             DSX_E_INVALID, "unknown precision %d", precision);
+  DSX_CHECK(M <= kSimtMaxM && C <= kSimtMaxC, DSX_E_INVALID,
+            "mel bins must be <= %d and residual channels <= %d (got M %d, C %d)", kSimtMaxM, kSimtMaxC, M, C);
+  if (precision != DSX_PREC_FP32_SIMT) {
+    DSX_CHECK(M == 80 && C == 256 && H == 256, DSX_E_INVALID,
+              "tensor-core path needs mel bins == 80 and residual_channels == hidden_size == 256 (got M %d, C %d, H %d); "
+              "use DSX_PREC_FP32_SIMT", M, C, H);
+    DSX_CHECK(dilation_cycle <= 4, DSX_E_INVALID,
+              "tensor-core path supports dilations up to 8 (dilation_cycle_length <= 4, got %d); use DSX_PREC_FP32_SIMT", dilation_cycle);
+  }
   DSX_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   free_model(h);
@@ -356,12 +365,8 @@ int dsx_load_diffnet(dsx_handle* h, const dsx_diffnet_params* p, int M, int C, i
   memset(&h->m, 0, sizeof(h->m));
   h->m.M = M; h->m.C = C; h->m.H = H; h->m.L = L; h->m.cycle = dilation_cycle;
   h->precision = precision;
-  if (precision != DSX_PREC_FP32_SIMT) {
+  if (precision != DSX_PREC_FP32_SIMT)
     DSX_CHECK(h->tc_group != 0, DSX_E_INVALID, "tensor-core precisions need an sm_90 (H100) device");
-    DSX_CHECK(tc_supported(h), DSX_E_INVALID, "tensor-core path needs residual_channels == hidden_size == 256");
-    DSX_CHECK(dilation_cycle <= 4, DSX_E_INVALID,
-              "tensor-core path supports dilations up to 8 (dilation_cycle_length <= 4, got %d); use DSX_PREC_FP32_SIMT", dilation_cycle);
-  }
   DSX_TRY(simt_pack_model(h, p, s));
   if (precision != DSX_PREC_FP32_SIMT) DSX_TRY(tc_pack_model(h, s));
   DSX_CUDA(cudaStreamSynchronize(s));

@@ -195,7 +195,7 @@ struct Workspace {
   Buf<float> X;         // [B][Tp][C] residual stream
   Buf<float> SKIP;      // [B][Tp][C]
   Buf<float> CONDF;     // [B][Tp][H] fp32 (SIMT path)
-  Buf<float> G1;        // [B][Tp][2C] SIMT GEMM output scratch
+  Buf<float> G1;        // [B][Tp][simt_g1_cols] SIMT GEMM output scratch: a layer's 2C columns, or the head's M
   Buf<float> Zf;        // [B][Tp][C]  SIMT gate output
   Buf<__half> Y;        // [2 buffers][2 planes][B][Tp][C]
   Buf<__half> CONDH;    // [2 planes][B][Tp][H]
@@ -277,6 +277,12 @@ inline int counted_launch(dsx_handle* h, const char* what, int n = 1) {
 }
 
 // ---- dsx_simt.cu -------------------------------------------------------------------------
+// Largest M and C of the fp32 path: k_inproj stages 16 frames x M and k_embed_table 5 C floats in the default 48 KB of
+// dynamic shared memory (dsx_load_diffnet refuses larger models)
+constexpr int kSimtMaxM = 768;
+constexpr int kSimtMaxC = 2448;
+// row stride of ws.G1: each layer's gate / filter and residual / skip GEMMs write 2C columns, the head's output projection M
+inline int simt_g1_cols(const ModelDev& m) { return m.M > 2 * m.C ? m.M : 2 * m.C; }
 int simt_pack_model(dsx_handle* h, const dsx_diffnet_params* p, cudaStream_t s);
 int launch_embed_table(dsx_handle* h, const int64_t* t_dev, int rows, cudaStream_t s);
 // emb[row] = mlp(SinusoidalPosEmb(m.C)(t[row])) for `rows` rows (m: C and the mlp weights)

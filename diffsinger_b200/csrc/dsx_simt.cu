@@ -427,9 +427,10 @@ int launch_head(dsx_handle* h, const Geom& g, float* eps, cudaStream_t s) {
   GemmA a2{};
   a2.X = h->ws.Zf; a2.lda = C; a2.Tp = g.Tp; a2.scale = 1.f;
   dim3 grid2(static_cast<unsigned>(nf / 64), (M + 63) / 64);
-  k_simt_gemm<0><<<grid2, 256, 0, s>>>(a2, m.fin_w, C, M, h->ws.G1, 2 * C);
+  const int ldg = simt_g1_cols(m);   // M > 2C: rows of 2C would overlap
+  k_simt_gemm<0><<<grid2, 256, 0, s>>>(a2, m.fin_w, C, M, h->ws.G1, ldg);
   dim3 grid3((g.T + 31) / 32, (M + 31) / 32, g.B), block3(32, 8);
-  k_eps_out<<<grid3, block3, 0, s>>>(h->ws.G1, m.fin_b, eps, M, g.T, g.Tp, 2 * C);
+  k_eps_out<<<grid3, block3, 0, s>>>(h->ws.G1, m.fin_b, eps, M, g.T, g.Tp, ldg);
   return counted_launch(h, "fp32 head (k_simt_gemm, k_bias_relu, k_simt_gemm, k_eps_out)", 4);
 }
 

@@ -111,7 +111,11 @@ void dsx_destroy(dsx_handle* h);
 /* Replaces: DiffNet.__init__ / load_state_dict (usr/diff/net.py:82-105; checkpoint keys
  * model.denoise_fn.*, utils/__init__.py:178-203).  (Re)packs the weights for the selected
  * precision; call again after every load_state_dict / .to().  M mel bins, C residual
- * channels, H conditioner channels, L layers, dilation 2^(l % cycle). */
+ * channels, H conditioner channels, L layers, dilation 2^(l % cycle).  M, C and H are multiples
+ * of 16, M <= 768 and C <= 2448 (the fp32 kernels stage an input frame block and the step
+ * embedding in the default 48 KB of shared memory; larger models are refused with DSX_E_INVALID
+ * rather than opted in).  The tensor-core precisions take M = 80, C = H = 256 and cycle <= 4
+ * only; DSX_PREC_FP32_SIMT takes any cycle. */
 int dsx_load_diffnet(dsx_handle* h, const dsx_diffnet_params* p, int M, int C, int H, int L,
                      int dilation_cycle, int precision, void* stream);
 

@@ -20,6 +20,22 @@ Pinning: ``oracle/gen_golden.py`` compares every function here against the live
 reference modules imported from a checkout of the reference (bit-exact or <=1e-6) and writes the
 vectors in ``tests/golden``; ``tests/test_oracle.py`` re-checks the oracle against those
 vectors wherever the tests run.
+
+Operand formats (``fmt=``).  ``diffnet_forward`` and every sampler built on it take ``fmt``: ``None`` is the
+reference computation above, unchanged; ``"fp16"``, ``"fp16x2"``, ``"fp16x3"`` and ``"fp16s"`` simulate what the
+tensor-core step kernel (dsx_hopper.cu) rounds in that precision, in the dtype of the inputs (float64 for a simulation
+whose only error is the operand rounding).  The simulation follows the kernel's header:
+
+  * conditioner projection: 3-pass, taken as exact;
+  * dilated conv and output projection: P = 1 (fp16) uses round-to-nearest fp16 weights, P = 2 (fp16x2) hi + lo fp16
+    weights, both with y = x + d and z rounded to fp16; P = 3 (fp16x3) also splits y and z into hi + lo; fp16s uses R
+    sets of stochastically rounded fp16 weights, evaluation row j (the FiLM-table row: the step of a loop, the
+    warm-up's second evaluation at row n, 0 for a single evaluation) on set j % R, with y and z rounded to fp16;
+  * input projection and head: hi + lo operands (HP = 3) except fp16 (HP = 1: both rounded to fp16); skip / sqrt(L)
+    reaches the head as hi + lo (S16), or its hi plane alone at HP = 1.
+
+The stochastic sets are drawn on the CPU (``OperandFormat(P, "fp16s", seed=...)``), not with the kernel's Philox
+stream, so a bound built on them takes the worst of a few draws.
 """
 from __future__ import annotations
 
@@ -104,10 +120,20 @@ def mish(x):
 def step_embedding(P, t):
     """net.py:119-120: e(t) = mlp(SinusoidalPosEmb(t)) -> [B, C]."""
     C = P["mlp.2.weight"].shape[0]
-    e = sinusoidal_embedding(t, C)
+    e = sinusoidal_embedding(t, C).to(P["mlp.0.weight"].dtype)     # integer t in a float64 model: fp32 angles
     e = F.linear(e, P["mlp.0.weight"], P["mlp.0.bias"])
     e = mish(e)
     return F.linear(e, P["mlp.2.weight"], P["mlp.2.bias"])
+
+
+def dilated_conv(y, w, b, dilation):
+    """The residual layers' conv (kernel 3, zero padding = dilation).  A dilation of at least T reaches wholly outside
+    the utterance with both outer taps, so only the centre tap remains; above 1024 (dilation cycles > 11) that is
+    computed directly rather than through a padding of 2 x dilation frames.  (Below, the padded conv is kept: the
+    centre-tap conv sums in another order.)"""
+    if dilation >= max(y.shape[-1], 1024):
+        return F.conv1d(y, w[..., 1:2], b)
+    return F.conv1d(y, w, b, padding=dilation, dilation=dilation)
 
 
 def residual_block(P, i, x, cond, e, dilation):
@@ -116,8 +142,7 @@ def residual_block(P, i, x, cond, e, dilation):
     d = F.linear(e, P[p + "diffusion_projection.weight"], P[p + "diffusion_projection.bias"]).unsqueeze(-1)
     c = F.conv1d(cond, P[p + "conditioner_projection.weight"], P[p + "conditioner_projection.bias"])
     y = x + d
-    y = F.conv1d(y, P[p + "dilated_conv.weight"], P[p + "dilated_conv.bias"],
-                 padding=dilation, dilation=dilation) + c
+    y = dilated_conv(y, P[p + "dilated_conv.weight"], P[p + "dilated_conv.bias"], dilation) + c
     gate, filt = torch.chunk(y, 2, dim=1)
     y = torch.sigmoid(gate) * torch.tanh(filt)
     y = F.conv1d(y, P[p + "output_projection.weight"], P[p + "output_projection.bias"])
@@ -125,12 +150,118 @@ def residual_block(P, i, x, cond, e, dilation):
     return (x + residual) / math.sqrt(2.0), skip
 
 
-def diffnet_forward(P, spec, t, cond, dilation_cycle_length=1, taps=None):
+# --------------------------------------------------------------------------------------
+# operand formats of the tensor-core kernels (see the module docstring)
+# --------------------------------------------------------------------------------------
+FORMATS = ("fp16", "fp16x2", "fp16x3", "fp16s")
+
+
+def rn16(x):
+    """round to nearest fp16, returned in x's dtype"""
+    return x.half().to(x.dtype)
+
+
+def hl16(x):
+    """hi + lo fp16 pair of x, summed in x's dtype"""
+    hi = rn16(x)
+    return hi + rn16(x - hi)
+
+
+def sr16(x, gen):
+    """Stochastic rounding to fp16 (returned in x's dtype): P(up) = distance to the lower neighbour / ulp.
+    gen: numpy RandomState."""
+    a = x.detach().cpu().numpy().astype(np.float32)
+    h = a.astype(np.float16)
+    hf = h.astype(np.float32)
+    up = np.nextafter(h, np.float16(np.inf)).astype(np.float32)
+    dn = np.nextafter(h, np.float16(-np.inf)).astype(np.float32)
+    lo = np.where(hf <= a, hf, dn)
+    hi = np.where(hf <= a, up, hf)
+    p = np.where(hi > lo, (a - lo) / np.maximum(hi - lo, 1e-30), 0.0)
+    u = gen.random_sample(a.shape).astype(np.float32)
+    return torch.from_numpy(np.where(u < p, hi, lo).astype(np.float32)).to(x.dtype)
+
+
+class OperandFormat:
+    """What one tensor-core precision rounds: ``act`` (y and z of the residual layers), ``head`` (operands of the input
+    projection and the head) and ``weights(row)`` (the residual layers' conv and output-projection weights of FiLM-table
+    row ``row``).  fp16s draws set r = row % sr_sets on first use, from numpy RandomState(seed + r)."""
+
+    def __init__(self, P, name, sr_sets=64, seed=0):
+        assert name in FORMATS, name
+        self.P, self.name, self.sr_sets, self.seed = P, name, sr_sets, seed
+        self.act = hl16 if name == "fp16x3" else rn16
+        self.head = rn16 if name == "fp16" else hl16
+        self._sets = {}
+
+    def weights(self, row):
+        key = row % self.sr_sets if self.name == "fp16s" else 0
+        if key not in self._sets:
+            gen = np.random.RandomState(self.seed + key)
+            rnd = {"fp16": rn16, "fp16x2": hl16, "fp16x3": hl16, "fp16s": lambda w: sr16(w, gen)}[self.name]
+            self._sets[key] = {k: rnd(v) for k, v in self.P.items()
+                               if k.startswith("residual_layers.") and
+                               k.endswith(("dilated_conv.weight", "output_projection.weight"))}
+        return self._sets[key]
+
+
+def operand_format(P, fmt):
+    """None, a name in FORMATS, or an OperandFormat (kept: a loop's stochastic sets persist across its steps)"""
+    return OperandFormat(P, fmt) if isinstance(fmt, str) else fmt
+
+
+# Steps of the simulated evaluation, one function each (oracle/diffnet_edge_sensitivity.py replaces them with
+# bug-shaped variants)
+def sim_input_projection(P, spec, f):
+    return F.relu(F.conv1d(f.head(spec[:, 0]), f.head(P["input_projection.weight"]), P["input_projection.bias"]))
+
+
+def sim_film(P, e, i):
+    """layer i's FiLM vectors d_i(t_b), [B, C, 1]"""
+    p = f"residual_layers.{i}."
+    return F.linear(e, P[p + "diffusion_projection.weight"], P[p + "diffusion_projection.bias"]).unsqueeze(-1)
+
+
+def sim_dilated_conv(y, w, b, dilation):
+    return dilated_conv(y, w, b, dilation)
+
+
+def sim_skip_sum(skips):
+    return sum(skips)
+
+
+def _forward_fmt(P, spec, t, cond, cycle, f, row):
+    L = num_layers(P)
+    W = f.weights(row)
+    x = sim_input_projection(P, spec, f)
+    e = step_embedding(P, t)
+    skips = []
+    for i in range(L):
+        p = f"residual_layers.{i}."
+        c = F.conv1d(cond, P[p + "conditioner_projection.weight"], P[p + "conditioner_projection.bias"])
+        y = sim_dilated_conv(f.act(x + sim_film(P, e, i)), W[p + "dilated_conv.weight"], P[p + "dilated_conv.bias"],
+                             2 ** (i % cycle)) + c
+        gate, filt = torch.chunk(y, 2, dim=1)
+        z = torch.sigmoid(gate) * torch.tanh(filt)
+        o = F.conv1d(f.act(z), W[p + "output_projection.weight"], P[p + "output_projection.bias"])
+        residual, skip = torch.chunk(o, 2, dim=1)
+        x = (x + residual) / math.sqrt(2.0)
+        skips.append(skip)
+    x = f.head(sim_skip_sum(skips) / math.sqrt(L))
+    x = F.relu(F.conv1d(x, f.head(P["skip_projection.weight"]), P["skip_projection.bias"]))
+    x = F.conv1d(f.head(x), f.head(P["output_projection.weight"]), P["output_projection.bias"])
+    return x[:, None, :, :]
+
+
+def diffnet_forward(P, spec, t, cond, dilation_cycle_length=1, taps=None, fmt=None, row=0):
     """net.py:107-130.  spec [B,1,M,T], t [B] int64, cond [B,H,T] -> eps [B,1,M,T].
 
     ``taps``: optional dict that receives the per-layer residual streams (``x{l}``: input of
     layer l, ``x{L}``: after the last layer) and the skip sum, for layer-by-layer checks.
+    ``fmt`` / ``row``: simulate a tensor-core precision (module docstring) at FiLM-table row ``row``.
     """
+    if fmt is not None:
+        return _forward_fmt(P, spec, t, cond, dilation_cycle_length, operand_format(P, fmt), row)
     L = num_layers(P)
     x = spec[:, 0]
     x = F.relu(F.conv1d(x, P["input_projection.weight"], P["input_projection.bias"]))
@@ -209,10 +340,10 @@ def _tvec(t, b):
     return torch.full((b,), int(t), dtype=torch.long)
 
 
-def p_sample(P, S, x, t, cond, noise, dilation_cycle_length=1, clip_denoised=True):
+def p_sample(P, S, x, t, cond, noise, dilation_cycle_length=1, clip_denoised=True, fmt=None, row=0):
     """shallow_diffusion_tts.py:149-166 with the noise passed in (noise_like is :38-41)."""
     b = x.shape[0]
-    eps = diffnet_forward(P, x, _tvec(t, b), cond, dilation_cycle_length)
+    eps = diffnet_forward(P, x, _tvec(t, b), cond, dilation_cycle_length, fmt=fmt, row=row)
     x_recon = S["sqrt_recip_alphas_cumprod"][t] * x - S["sqrt_recipm1_alphas_cumprod"][t] * eps
     if clip_denoised:
         x_recon = x_recon.clamp(-1., 1.)
@@ -234,21 +365,28 @@ def plms_x_pred(S, x, noise_t, t, interval):
     return x + x_delta
 
 
-def p_sample_plms(P, S, x, t, interval, cond, noise_list, dilation_cycle_length=1):
-    """shallow_diffusion_tts.py:168-204.  ``noise_list`` is the caller-owned history (list)."""
-    b = x.shape[0]
-    noise_pred = diffnet_forward(P, x, _tvec(t, b), cond, dilation_cycle_length)
+def plms_prime(noise_pred, noise_list):
+    """the linear multistep combination of the current eps with the history, after the warm-up (:191-197)"""
     n = len(noise_list)
-    if n == 0:
+    if n == 1:
+        return (3 * noise_pred - noise_list[-1]) / 2
+    if n == 2:
+        return (23 * noise_pred - 16 * noise_list[-1] + 5 * noise_list[-2]) / 12
+    return (55 * noise_pred - 59 * noise_list[-1] + 37 * noise_list[-2] - 9 * noise_list[-3]) / 24
+
+
+def p_sample_plms(P, S, x, t, interval, cond, noise_list, dilation_cycle_length=1, fmt=None, row=0, warm_row=1):
+    """shallow_diffusion_tts.py:168-204.  ``noise_list`` is the caller-owned history (list).
+    ``fmt``: a simulated precision; the evaluation at t is at table row ``row``, the warm-up's second at ``warm_row``."""
+    b = x.shape[0]
+    noise_pred = diffnet_forward(P, x, _tvec(t, b), cond, dilation_cycle_length, fmt=fmt, row=row)
+    if len(noise_list) == 0:
         x_pred = plms_x_pred(S, x, noise_pred, t, interval)
-        noise_pred_prev = diffnet_forward(P, x_pred, _tvec(max(t - interval, 0), b), cond, dilation_cycle_length)
+        noise_pred_prev = diffnet_forward(P, x_pred, _tvec(max(t - interval, 0), b), cond, dilation_cycle_length,
+                                          fmt=fmt, row=warm_row)
         prime = (noise_pred + noise_pred_prev) / 2
-    elif n == 1:
-        prime = (3 * noise_pred - noise_list[-1]) / 2
-    elif n == 2:
-        prime = (23 * noise_pred - 16 * noise_list[-1] + 5 * noise_list[-2]) / 12
     else:
-        prime = (55 * noise_pred - 59 * noise_list[-1] + 37 * noise_list[-2] - 9 * noise_list[-3]) / 24
+        prime = plms_prime(noise_pred, noise_list)
     x_prev = plms_x_pred(S, x, prime, t, interval)
     noise_list.append(noise_pred)
     if len(noise_list) > 4:          # deque(maxlen=4), :99
@@ -256,18 +394,24 @@ def p_sample_plms(P, S, x, t, interval, cond, noise_list, dilation_cycle_length=
     return x_prev
 
 
-def sample_ddpm(P, S, x, cond, K, noise, dilation_cycle_length=1):
-    """Loop :269-270.  noise[j] is used at the j-th executed step (t = K-1-j)."""
+def sample_ddpm(P, S, x, cond, K, noise, dilation_cycle_length=1, fmt=None, n_steps=None):
+    """Loop :269-270.  noise[j] is used at the j-th executed step (t = K-1-j), step j at table row j.
+    ``n_steps``: stop after that many steps (t = K-1 .. K-n_steps), as dsx_sample_ddpm does."""
+    fmt = operand_format(P, fmt)
     for j, t in enumerate(reversed(range(0, K))):
-        x = p_sample(P, S, x, t, cond, noise[j], dilation_cycle_length)
+        if n_steps is not None and j == n_steps:
+            break
+        x = p_sample(P, S, x, t, cond, noise[j], dilation_cycle_length, fmt=fmt, row=j)
     return x
 
 
-def sample_plms(P, S, x, cond, K, interval, dilation_cycle_length=1):
-    """Loop :261-267."""
+def sample_plms(P, S, x, cond, K, interval, dilation_cycle_length=1, fmt=None):
+    """Loop :261-267.  Step j at table row j, the warm-up's second evaluation at row n (the number of steps)."""
+    fmt = operand_format(P, fmt)
     hist = []
-    for t in reversed(range(0, K, interval)):
-        x = p_sample_plms(P, S, x, t, interval, cond, hist, dilation_cycle_length)
+    steps = list(reversed(range(0, K, interval)))
+    for j, t in enumerate(steps):
+        x = p_sample_plms(P, S, x, t, interval, cond, hist, dilation_cycle_length, fmt=fmt, row=j, warm_row=len(steps))
     return x
 
 
@@ -288,7 +432,7 @@ def q_sample(S, x_start, t, noise):
 
 def infer_loop(P, S, cond, K_step, spec_min, spec_max, *, fs2_mel=None, start_noise=None,
                x_start=None, step_noise=None, pndm_speedup=None, mel2ph=None,
-               dilation_cycle_length=1):
+               dilation_cycle_length=1, fmt=None):
     """The infer branch of GaussianDiffusion.forward, :248-275, after ``self.fs2``.
 
     cond [B,H,T].  Shallow start: fs2_mel [B,T,M] + start_noise [B,1,M,T];
@@ -300,9 +444,9 @@ def infer_loop(P, S, cond, K_step, spec_min, spec_max, *, fs2_mel=None, start_no
     else:
         x = x_start
     if pndm_speedup:
-        x = sample_plms(P, S, x, cond, K_step, pndm_speedup, dilation_cycle_length)
+        x = sample_plms(P, S, x, cond, K_step, pndm_speedup, dilation_cycle_length, fmt=fmt)
     else:
-        x = sample_ddpm(P, S, x, cond, K_step, step_noise, dilation_cycle_length)
+        x = sample_ddpm(P, S, x, cond, K_step, step_noise, dilation_cycle_length, fmt=fmt)
     x = x[:, 0].transpose(1, 2)
     out = denorm_spec(x, spec_min, spec_max)
     if mel2ph is not None:

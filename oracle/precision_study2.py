@@ -17,27 +17,7 @@ from . import diffnet_oracle as O
 from .gen_golden import rs_normal, OUT
 
 
-def rn16(x):
-    return x.half().float()
-
-
-def hl16(x):
-    hi = x.half().float()
-    return hi + (x - hi).half().float()
-
-
-def sr16(x, gen):
-    """Stochastic rounding of fp32 -> fp16 (returned as fp32): P(up) = distance to the lower neighbour / ulp."""
-    a = x.numpy().astype(np.float32)
-    h = a.astype(np.float16)
-    hf = h.astype(np.float32)
-    up = np.nextafter(h, np.float16(np.inf)).astype(np.float32)
-    dn = np.nextafter(h, np.float16(-np.inf)).astype(np.float32)
-    lo = np.where(hf <= a, hf, dn)
-    hi = np.where(hf <= a, up, hf)
-    p = np.where(hi > lo, (a - lo) / np.maximum(hi - lo, 1e-30), 0.0)
-    u = gen.random_sample(a.shape).astype(np.float32)
-    return torch.from_numpy(np.where(u < p, hi, lo).astype(np.float32))
+rn16, hl16, sr16 = O.rn16, O.hl16, O.sr16
 
 
 def make_sets(P, mode1, mode2, R, seed=1234):
