@@ -27,7 +27,7 @@
 // starts (j - 1) d rows away from the warpgroup's rows.  Both chunks read it, so each element of y crosses L2 -> SM once
 // per layer instead of six times.  fp16x3 (R = 2) reads y's lo plane too and keeps streaming its taps.
 // Each warpgroup's rows go through the same instruction sequence whatever NWG is, so 64- and 128-frame CTAs give
-// bit-identical results.  While GEMM1 runs, the warpgroup prefetches the CP, x and skip rows its epilogues read into L2,
+// bit-identical results.  While GEMM1 runs, the warpgroup prefetches the CP rows its gate epilogues read into L2,
 // and the epilogues issue their global loads in batches ahead of their stores: every operand of a batch, including the
 // residual and skip epilogues' bias and FiLM pairs, is loaded before the batch's first store.
 //
@@ -213,7 +213,8 @@ __device__ __forceinline__ void load_w(uint8_t* dst, const __half* src0, const _
   }
 }
 // 64 frames [t0, t0 + 64) of utterance b, channels [ch0, ch0 + 64) of a frames-major [B][Tp][256] fp16 plane; frames
-// outside [0, T) read as zero.  Called by the 128 threads of one warpgroup.
+// outside [0, T) read as zero.  Called by the 128 threads of one warpgroup.  (Unlike the window, a streamed tap is read
+// again by the layer's other taps and chunk, so it carries no eviction hint.)
 __device__ __forceinline__ void load_a(uint8_t* dst, const __half* src, int b, int t0, int ch0, int T, int Tp, int wtid) {
   const uint32_t d = smem_u32(dst);
 #pragma unroll
@@ -226,7 +227,8 @@ __device__ __forceinline__ void load_a(uint8_t* dst, const __half* src, int b, i
 }
 // One channel block of a conv-input window: rows r < rows hold frame t_first + r of one utterance (utt: its [Tp][256]
 // frames), channels [ch0, ch0 + 64); frames outside [0, T) read as zero.  dst is 1024-aligned, so a wgmma descriptor
-// started at any row reads 64 consecutive frames.  Called by the NT threads of the CTA.
+// started at any row reads 64 consecutive frames.  Called by the NT threads of the CTA.  The lines leave L2 first: a layer
+// reads its conv input once per tile (the neighbour tiles' halo rows aside) and the layer after overwrites it.
 template <int NT>
 __device__ __forceinline__ void load_wblock(uint8_t* dst, const __half* utt, int t_first, int ch0, int rows, int T, int tid) {
   const uint32_t d = smem_u32(dst);
@@ -234,7 +236,7 @@ __device__ __forceinline__ void load_wblock(uint8_t* dst, const __half* utt, int
   for (int i = tid; i < rows * 8; i += NT) {
     const int r = i >> 3, c = i & 7, t = t_first + r;
     const bool valid = t >= 0 && t < T;
-    cp16(d + sw128(r, c), utt + static_cast<size_t>(valid ? t : 0) * kC + ch0 + c * 8, valid);
+    cp16_hint(d + sw128(r, c), utt + static_cast<size_t>(valid ? t : 0) * kC + ch0 + c * 8, valid, l2_evict_first());
   }
 }
 
@@ -525,13 +527,13 @@ __device__ __forceinline__ void layer_tile(const HpParams& p, int l, int u, Smem
   // ---- GEMM1 + gate, chunk by chunk ----
 #pragma unroll 1
   for (int h = 0; h < 2; ++h) {
-    // L2 prefetch of this warpgroup's epilogue operands, 16 KB per stage: its CP rows (64 x 2 KB, both chunks) during
-    // chunk 0, its X and SKIP rows (64 x 1 KB each) during chunk 1
+    // L2 prefetch of this warpgroup's CP rows (64 x 2 KB, both chunks) during chunk 0, 16 KB per stage.  They are
+    // marked evict_last so that the weight stream and the other group's epilogue traffic do not push chunk 1's rows out
+    // before its gate epilogue reads them; that read (ld_stream_f2, evict_first) releases them.  x and skip are not
+    // prefetched: with the CP rows held, a chunk-1 prefetch of them cost more than it saved (DESIGN.md).
     auto pre = [&](int s) {
-      if (wtid != 0 || s >= 8) return;
-      if (h == 0) prefetch_l2(p.CP + (static_cast<size_t>(l) * NF + fbase) * 512 + s * 4096, 16384);
-      else if (s < 4) prefetch_l2(p.X + fbase * kC + s * 4096, 16384);
-      else if (l > 0) prefetch_l2(p.SKIP + fbase * kC + (s - 4) * 4096, 16384);
+      if (wtid != 0 || s >= 8 || h != 0) return;
+      prefetch_l2_hint(p.CP + (static_cast<size_t>(l) * NF + fbase) * 512 + s * 4096, 16384, l2_evict_last());
     };
     gemm<2>(c0, c1, sm, p, Phase{PH_G1, l, u, h}, pre);
     // chunk 1's weights and taps do not depend on this epilogue; GEMM2's weights do not depend on either

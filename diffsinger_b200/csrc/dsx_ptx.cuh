@@ -163,6 +163,12 @@ __device__ __forceinline__ int acc_col(int wtid, int e) { return ((e >> 2) << 3)
 __device__ __forceinline__ void cp16(uint32_t dst, const void* src, bool valid) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
 }
+// cp16 with a policy for the source lines
+__device__ __forceinline__ void cp16_hint(uint32_t dst, const void* src, bool valid, uint64_t pol) {
+  asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2, %3;" ::"r"(dst), "l"(src),
+               "r"(valid ? 16 : 0), "l"(pol)
+               : "memory");
+}
 __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
@@ -219,10 +225,6 @@ __device__ __forceinline__ void wait_geq(const unsigned* p, unsigned n) {
 }
 
 // ---- global memory hints ------------------------------------------------------------------------
-// bytes (a multiple of 16) at a 16-byte aligned global address -> L2, asynchronously; nothing waits for it
-__device__ __forceinline__ void prefetch_l2(const void* src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-}
 // load of data that is read once and never written by the kernel: no L1 allocation, first out of L2.  Not volatile, so
 // the compiler may move it across the stores around it.
 __device__ __forceinline__ float2 ld_stream_f2(const float* src) {
@@ -232,6 +234,24 @@ __device__ __forceinline__ float2 ld_stream_f2(const float* src) {
       : "=f"(v.x), "=f"(v.y)
       : "l"(src));
   return v;
+}
+// L2 cache policies, the 64-bit operand of the .L2::cache_hint forms below.  Each is one createpolicy with immediate
+// operands, so the kernels create it where they use it.
+// evict_last: lines a later phase of the same tile reads, which the traffic in between must not push out of L2
+__device__ __forceinline__ uint64_t l2_evict_last() {
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+// evict_first: lines that are dead once read
+__device__ __forceinline__ uint64_t l2_evict_first() {
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+// bytes (a multiple of 16) at a 16-byte aligned global address -> L2 with policy pol, asynchronously; nothing waits for it
+__device__ __forceinline__ void prefetch_l2_hint(const void* src, uint32_t bytes, uint64_t pol) {
+  asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(src), "r"(bytes), "l"(pol) : "memory");
 }
 
 // ---- math ---------------------------------------------------------------------------------------
