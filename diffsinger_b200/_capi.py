@@ -40,10 +40,15 @@ SYMBOLS = (
     "dsx_durpred_train_create", "dsx_durpred_train_destroy", "dsx_durpred_train_tape_bytes",
     "dsx_durpred_train_workspace_bytes", "dsx_durpred_train_forward", "dsx_durpred_train_backward",
     "dsx_durpred_train_masks",
+    "dsx_pitchpred_create", "dsx_pitchpred_destroy", "dsx_pitchpred_load", "dsx_pitchpred_forward",
+    "dsx_pitchpred_train_create", "dsx_pitchpred_train_destroy", "dsx_pitchpred_train_tape_bytes",
+    "dsx_pitchpred_train_workspace_bytes", "dsx_pitchpred_train_forward", "dsx_pitchpred_train_backward",
+    "dsx_pitchpred_train_masks",
 )
 _VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy", "dsx_fs2dec_destroy",
          "dsx_fs2enc_destroy", "dsx_durpred_destroy", "dsx_train_destroy", "dsx_fs2dec_train_destroy",
-         "dsx_fft_train_destroy", "dsx_fs2enc_train_destroy", "dsx_durpred_train_destroy")
+         "dsx_fft_train_destroy", "dsx_fs2enc_train_destroy", "dsx_durpred_train_destroy", "dsx_pitchpred_destroy",
+         "dsx_pitchpred_train_destroy")
 
 
 class DsxError(RuntimeError):
@@ -130,6 +135,16 @@ class DurPredConfig(ctypes.Structure):
 class DurPredParams(ctypes.Structure):
     _fields_ = [("conv_w", _fpp), ("conv_b", _fpp), ("ln_w", _fpp), ("ln_b", _fpp), ("linear_w", _fp),
                 ("linear_b", _fp)]
+
+
+class PitchPredConfig(ctypes.Structure):
+    _fields_ = [("idim", ctypes.c_int), ("chans", ctypes.c_int), ("layers", ctypes.c_int), ("kernel", ctypes.c_int),
+                ("padding", ctypes.c_int), ("odim", ctypes.c_int)]
+
+
+class PitchPredParams(ctypes.Structure):
+    _fields_ = [("conv_w", _fpp), ("conv_b", _fpp), ("ln_w", _fpp), ("ln_b", _fpp), ("linear_w", _fp),
+                ("linear_b", _fp), ("pos_embed_alpha", _fp)]
 
 
 class TrainConfig(ctypes.Structure):
@@ -240,6 +255,21 @@ lib.dsx_durpred_train_forward.argtypes = [_vp, ctypes.POINTER(DurPredParams), _v
 lib.dsx_durpred_train_backward.argtypes = [_vp, ctypes.POINTER(DurPredParams), _vp, _vp, ctypes.POINTER(DurPredParams),
                                            _vp, _i, _i, _vp, ctypes.c_size_t, _vp]
 lib.dsx_durpred_train_masks.argtypes = [_vp, _u64, ctypes.c_float, _i, _i, ctypes.POINTER(_vp), _vp]
+lib.dsx_pitchpred_create.argtypes = [_i, ctypes.POINTER(PitchPredConfig), ctypes.POINTER(_vp)]
+lib.dsx_pitchpred_destroy.argtypes = [_vp]
+lib.dsx_pitchpred_destroy.restype = None
+lib.dsx_pitchpred_load.argtypes = [_vp, ctypes.POINTER(PitchPredParams), _vp]
+lib.dsx_pitchpred_forward.argtypes = [_vp, _vp, _i, _i, _vp, _vp]
+lib.dsx_pitchpred_train_create.argtypes = [_i, ctypes.POINTER(PitchPredConfig), ctypes.POINTER(_vp)]
+lib.dsx_pitchpred_train_destroy.argtypes = [_vp]
+lib.dsx_pitchpred_train_destroy.restype = None
+lib.dsx_pitchpred_train_tape_bytes.argtypes = [_vp, _i, _i, ctypes.POINTER(ctypes.c_size_t)]
+lib.dsx_pitchpred_train_workspace_bytes.argtypes = [_vp, _i, _i, ctypes.POINTER(ctypes.c_size_t)]
+lib.dsx_pitchpred_train_forward.argtypes = [_vp, ctypes.POINTER(PitchPredParams), _vp, _i, _i, ctypes.c_float, _u64, _vp,
+                                            ctypes.c_size_t, _vp, ctypes.c_size_t, _vp, _vp]
+lib.dsx_pitchpred_train_backward.argtypes = [_vp, ctypes.POINTER(PitchPredParams), _vp, _vp,
+                                             ctypes.POINTER(PitchPredParams), _vp, _i, _i, _vp, ctypes.c_size_t, _vp]
+lib.dsx_pitchpred_train_masks.argtypes = [_vp, _u64, ctypes.c_float, _i, _i, ctypes.POINTER(_vp), _vp]
 for _n in SYMBOLS:
     if _n not in _VOID:
         getattr(lib, _n).restype = _i

@@ -10,7 +10,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = [os.path.join(HERE, "csrc", f) for f in ("dsx_api.cu", "dsx_simt.cu", "dsx_hopper.cu", "dsx_hifigan.cu", "dsx_pe.cu",
                                                 "dsx_fs2dec.cu", "dsx_fftdiff.cu", "dsx_fs2enc.cu", "dsx_train.cu",
-                                                "dsx_fs2train.cu", "dsx_ffttrain.cu", "dsx_fs2enctrain.cu", "dsx_durtrain.cu")]
+                                                "dsx_fs2train.cu", "dsx_ffttrain.cu", "dsx_fs2enctrain.cu", "dsx_durtrain.cu",
+                                                "dsx_pitchtrain.cu")]
 HDR = [os.path.join(HERE, "csrc", f) for f in ("dsx_internal.h", "dsx_ptx.cuh", "dsx_rng.cuh", "dsx_conv.cuh",
                                                "dsx_posemb.cuh", "dsx_wgrad.cuh", "dsx_fftentry.cuh")] + \
       [os.path.join(os.path.dirname(HERE), "include", "dsx.h")]

@@ -23,6 +23,9 @@
 //                          grids) summed in order, / S
 // 4 + 4 L launches for k <= 4.  No atomics touch a result, so two backwards of one tape are bitwise equal; every gradient
 // written is a fixed-order fp32 sum times 1 / S, so 2^k d_xs gives exactly 2^k times every gradient.
+//
+// The backward (dpt_backward) also serves the pitch predictor's step (dsx_pitchtrain.cu): there the mask is NULL and
+// the head has od <= 16 outputs, d_out [F][od] instead of d_xs.
 #include <math.h>
 
 #include <algorithm>
@@ -83,11 +86,13 @@ __global__ void k_dpt_hdr(TapeHdr* h, uint64_t seed, float p, int B, int T, cons
   }
 }
 
-// amax |d_xs| over the non-padding tokens, one CTA (F is a few thousand tokens)
-__global__ void __launch_bounds__(1024) k_dpt_amax(const float* g, const uint8_t* pad, size_t F, unsigned* amax_bits) {
+// amax |d_out| over the od columns of the non-padding tokens (pad NULL: every token), one CTA (F is a few thousand
+// tokens, tens of thousands of frames for the pitch predictor)
+__global__ void __launch_bounds__(1024) k_dpt_amax(const float* g, const uint8_t* pad, size_t F, int od,
+                                                   unsigned* amax_bits) {
   __shared__ float red[32];
   float m = 0.f;
-  for (size_t i = threadIdx.x; i < F; i += blockDim.x) m = fmaxf(m, pad[i] ? 0.f : fabsf(g[i]));
+  for (size_t i = threadIdx.x; i < F * od; i += blockDim.x) m = fmaxf(m, pad && pad[i / od] ? 0.f : fabsf(g[i]));
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
@@ -100,40 +105,64 @@ __global__ void __launch_bounds__(1024) k_dpt_amax(const float* g, const uint8_t
 
 // ---- the head and layer L - 1: one warp per token ---------------------------------------------------------------------
 struct DpHeadArgs {
-  const float* dxs;            // [F] d_xs, unscaled
-  const uint8_t* pad;
+  const float* dxs;            // [F][od] d_out, unscaled
+  const uint8_t* pad;          // [F] or NULL (no mask)
   const float* hin;            // the head's input [F][P] (tape)
   const float* r;              // layer L - 1's LayerNorm input [F][P] (tape)
-  const float* wl;             // linear.weight [P]
+  const float* wl;             // linear.weight [od][P]
   const float* gamma;          // layer L - 1's LayerNorm weight [P]
   const TapeHdr* hdr;
   int site;                    // L - 1
   const float* scal;
   __half* gu;                  // [F][P]
-  float* part;                 // [kHeadBlocks][3 P + 1]: d gamma, d beta, d linear.weight, d linear.bias of this CTA
-  int F, P;
+  float* part;                 // [kHeadBlocks][head_part_floats]: d gamma, d beta, d linear.weight, d linear.bias
+  int F, P, od;
 };
 
+// floats of one CTA's k_dpt_head partials: d gamma [P], d beta [P], d linear.weight [od][P], d linear.bias [od]
+__host__ __device__ inline int head_part_floats(int P, int od) { return (2 + od) * P + od; }
+
+// OD >= od outputs of the head (the duration predictor's 1, the pitch predictor's up to 16); the warps' partials are
+// added into the CTA's sums in warp order, so OD = 1 sums exactly as a per-warp table summed in order would
+template <int OD>
 __global__ void __launch_bounds__(256) k_dpt_head(const DpHeadArgs p) {
-  __shared__ float red[8][3 * 256 + 1];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, P = p.P;
+  __shared__ float tot[(2 + OD) * 256 + OD];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, P = p.P, od = p.od;
   const float S = p.scal[0], inv_p = 1.f / static_cast<float>(P);
   const Fs2Drop drop = hdr_drop(p.hdr, p.site);
-  float dgam[8], dbet[8], dwl[8], dbl = 0.f;
+  float dgam[8], dbet[8], dwl[OD][8], dbl[OD];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) dgam[i] = dbet[i] = dwl[i] = 0.f;
+  for (int i = 0; i < 8; ++i) {
+    dgam[i] = dbet[i] = 0.f;
+#pragma unroll
+    for (int o = 0; o < OD; ++o) dwl[o][i] = 0.f;
+  }
+#pragma unroll
+  for (int o = 0; o < OD; ++o) dbl[o] = 0.f;
   for (int f = blockIdx.x * 8 + warp; f < p.F; f += gridDim.x * 8) {
     const size_t rb = static_cast<size_t>(f) * P;
-    const float gx = p.pad[f] ? 0.f : S * p.dxs[f];
-    if (lane == 0) dbl += gx;
+    const bool padded = p.pad && p.pad[f];
+    float gx[OD];
+#pragma unroll
+    for (int o = 0; o < OD; ++o) gx[o] = padded || o >= od ? 0.f : S * p.dxs[static_cast<size_t>(f) * od + o];
+    if (lane == 0) {
+#pragma unroll
+      for (int o = 0; o < OD; ++o) dbl[o] += gx[o];
+    }
     float rv[8], gy[8], sum = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int c = lane + 32 * i;
       rv[i] = gy[i] = 0.f;
       if (c >= P) continue;
-      dwl[i] += gx * p.hin[rb + c];
-      gy[i] = gx * p.wl[c] * dropout_scale(drop, f, c);
+      const float h = p.hin[rb + c];
+      float g = gx[0] * p.wl[c];
+#pragma unroll
+      for (int o = 0; o < OD; ++o) {
+        dwl[o][i] += gx[o] * h;
+        if (o > 0 && o < od) g += gx[o] * p.wl[o * P + c];
+      }
+      gy[i] = g * dropout_scale(drop, f, c);
       rv[i] = p.r[rb + c];
       sum += rv[i];
     }
@@ -167,22 +196,29 @@ __global__ void __launch_bounds__(256) k_dpt_head(const DpHeadArgs p) {
       p.gu[rb + c] = sat_half(v);
     }
   }
+  const int W = head_part_floats(P, od);
+  for (int t = threadIdx.x; t < W; t += blockDim.x) tot[t] = 0.f;
+  for (int w = 0; w < 8; ++w) {
+    __syncthreads();
+    if (warp != w) continue;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int c = lane + 32 * i;
-    if (c >= P) continue;
-    red[warp][c] = dgam[i];
-    red[warp][P + c] = dbet[i];
-    red[warp][2 * P + c] = dwl[i];
+    for (int i = 0; i < 8; ++i) {
+      const int c = lane + 32 * i;
+      if (c >= P) continue;
+      tot[c] += dgam[i];
+      tot[P + c] += dbet[i];
+#pragma unroll
+      for (int o = 0; o < OD; ++o)
+        if (o < od) tot[(2 + o) * P + c] += dwl[o][i];
+    }
+    if (lane == 0) {
+#pragma unroll
+      for (int o = 0; o < OD; ++o)
+        if (o < od) tot[(2 + od) * P + o] += dbl[o];
+    }
   }
-  if (lane == 0) red[warp][3 * P] = dbl;
   __syncthreads();
-  for (int t = threadIdx.x; t < 3 * P + 1; t += blockDim.x) {
-    float s = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) s += red[w][t];
-    p.part[static_cast<size_t>(blockIdx.x) * (3 * P + 1) + t] = s;
-  }
+  for (int t = threadIdx.x; t < W; t += blockDim.x) p.part[static_cast<size_t>(blockIdx.x) * W + t] = tot[t];
 }
 
 // ---- data gradient of conv i, with layer i - 1's backward in the epilogue ---------------------------------------------
@@ -193,7 +229,7 @@ struct DgradArgs {
   float* dx;                   // layer 0: d_x [F][g.n] = the transposed conv / S
   const float* r;              // else layer i - 1's LayerNorm input [F][g.n] (tape)
   const float* gamma;          // layer i - 1's LayerNorm weight
-  const uint8_t* pad;
+  const uint8_t* pad;          // [F] or NULL (no mask)
   const TapeHdr* hdr;
   int site;                    // i - 1
   __half* gu;                  // GU of layer i - 1 [F][g.n]
@@ -248,7 +284,7 @@ __global__ void __launch_bounds__(128 * DgShape<NT>::WG) k_dpt_dgrad(const Dgrad
   const Fs2Drop drop = hdr_drop(p.hdr, p.site);
   bool keep[2];
 #pragma unroll
-  for (int r = 0; r < 2; ++r) keep[r] = mrow[r] < T && !p.pad[rbase + mrow[r]];
+  for (int r = 0; r < 2; ++r) keep[r] = mrow[r] < T && !(p.pad && p.pad[rbase + mrow[r]]);
   // g = the gradient at layer i - 1's LayerNorm output (in acc); its input r, then xhat, in the spent operand stages
   // (thread-private slots: NT / 2 floats per thread fit in conv_smem<NT>())
   float* rv = reinterpret_cast<float*>(smem) + tid;
@@ -365,7 +401,8 @@ __global__ void k_dpt_wreduce(const WredArgs p) {
 }
 
 // every LayerNorm affine gradient and the head's: layer l's partials part[l] (blocks[l] rows of stride[l] floats, d gamma
-// then d beta), the head's at columns 2 P .. 3 P of the last layer's rows, summed in row order, / S
+// then d beta), the head's (d linear.weight [od][P], then d linear.bias [od]) from column 2 P of the last layer's rows,
+// summed in row order, / S
 struct LnRedArgs {
   const float* part[kDpMaxLayers];
   int blocks[kDpMaxLayers], stride[kDpMaxLayers];
@@ -373,7 +410,7 @@ struct LnRedArgs {
   float* dbeta[kDpMaxLayers];
   float* dwl;
   float* dbl;
-  int L, P;
+  int L, P, od;
   const TapeHdr* hdr;
   int B, T;
   const float* scal;
@@ -381,14 +418,14 @@ struct LnRedArgs {
 
 __global__ void k_dpt_lnreduce(const LnRedArgs p) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x, P = p.P;
-  if (t >= (2 * p.L + 1) * P + 1) return;
+  if (t >= 2 * p.L * P + p.od * (P + 1)) return;
   const int l = t < 2 * p.L * P ? t / (2 * P) : p.L - 1, c = t < 2 * p.L * P ? t % (2 * P) : t - 2 * p.L * P + 2 * P;
   float s = 0.f;
   for (int k = 0; k < p.blocks[l]; ++k) s += p.part[l][static_cast<size_t>(k) * p.stride[l] + c];
   s *= inv_scale(p.hdr, p.B, p.T, p.scal);
   if (t >= 2 * p.L * P) {
-    if (c < 3 * P) p.dwl[c - 2 * P] = s;
-    else p.dbl[0] = s;
+    if (c < (2 + p.od) * P) p.dwl[c - 2 * P] = s;
+    else p.dbl[c - (2 + p.od) * P] = s;
   } else if (c < P) {
     p.dgamma[l][c] = s;
   } else {
@@ -403,11 +440,7 @@ __global__ void k_dpt_masks(Fs2Drop d, size_t F, int n, uint8_t* out) {
 }
 
 // ---- tape and workspace -------------------------------------------------------------------------------------------------
-struct Tape {
-  TapeHdr* hdr;
-  uint8_t* pad;                // [F] the forward's mask
-  DurTrain tr;
-};
+using Tape = DurTape;
 
 // every region of the tape for (config, B, T), in order; bytes of the whole tape
 size_t tape_carve(const dsx_durpred_config& c, int B, int T, uint8_t* base, Tape* t) {
@@ -461,7 +494,7 @@ size_t wgrad_part_floats(const dsx_durpred_config& c, int F, int device) {
 }
 
 struct Ws {
-  unsigned* amax;
+  unsigned* amax;   // the scale's words, then the gradient operands and partial sums of dpt_backward
   float* scal;
   __half* gu[2];
   float* hpart;
@@ -470,8 +503,8 @@ struct Ws {
   float* wpart;
 };
 
-// the backward's workspace (the forward uses none); bytes of it
-size_t ws_carve(const dsx_durpred_train* h, int B, int T, uint8_t* base, Ws* w) {
+// the backward's workspace (the forward uses none) for a head of od outputs; bytes of it
+size_t ws_carve(const dsx_durpred_train* h, int B, int T, int od, uint8_t* base, Ws* w) {
   const dsx_durpred_config& c = h->cfg;
   const size_t F = static_cast<size_t>(B) * T, P = c.chans, mt = (T + kConvRows - 1) / kConvRows;
   size_t n = 0;
@@ -486,7 +519,7 @@ size_t ws_carve(const dsx_durpred_train* h, int B, int T, uint8_t* base, Ws* w) 
   ws.scal = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ws.amax) + 16);
   ws.gu[0] = reinterpret_cast<__half*>(take(2 * F * P));
   ws.gu[1] = reinterpret_cast<__half*>(take(2 * F * P));
-  ws.hpart = reinterpret_cast<float*>(take(4 * static_cast<size_t>(kHeadBlocks) * (3 * P + 1)));
+  ws.hpart = reinterpret_cast<float*>(take(4 * static_cast<size_t>(kHeadBlocks) * head_part_floats(c.chans, od)));
   ws.lnp_stride = align256(4 * B * mt * 2 * P) / 4;
   ws.lnp = reinterpret_cast<float*>(take(4 * ws.lnp_stride * (c.layers - 1)));
   ws.wpart = reinterpret_cast<float*>(take(4 * wgrad_part_floats(c, static_cast<int>(F), h->device)));
@@ -525,112 +558,23 @@ int run_dgrad(DgradArgs a, const ConvGemm& g, int B, int T, cudaStream_t s) {
 }  // namespace
 }  // namespace dsx
 
-using namespace dsx;
+namespace dsx {
 
-extern "C" {
+dsx_durpred* dpt_forward_handle(dsx_durpred_train* h) { return h->fwd; }
 
-int dsx_durpred_train_create(int device, const dsx_durpred_config* cfg, dsx_durpred_train** out) {
-  DSX_CHECK(out, DSX_E_INVALID, "out is NULL");
-  *out = nullptr;
-  dsx_durpred* fwd = nullptr;
-  DSX_TRY(dsx_durpred_create(device, cfg, &fwd));   // validates the configuration and selects the device
-  dsx_durpred_train* h = new dsx_durpred_train();
-  h->device = device;
-  h->cfg = *cfg;
-  h->fwd = fwd;
-  int rc = [&]() -> int {
-    DSX_TRY(durpred_train_alloc(fwd));
-    DSX_TRY(conv_opt_in<256>([](auto k) { return k_dpt_dgrad<decltype(k)::value>; }));
-    DSX_CUDA(cudaFuncSetAttribute(k_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem));
-    const int P = cfg->chans;
-    for (int i = 0; i < cfg->layers; ++i) {   // gx[t] = sum_j W_j^T GU[t - tap0 - j]
-      ConvGemm& g = h->dgrad[i];
-      g.cin = P;
-      g.n = i ? P : cfg->idim;
-      g.taps = cfg->kernel;
-      g.tap0 = -tap0_of(*cfg);
-      g.tstep = -1;
-      DSX_TRY(conv_alloc(h->mem, g, 256));
-    }
-    return DSX_OK;
-  }();
-  if (rc != DSX_OK) {
-    dsx_durpred_train_destroy(h);
-    return rc;
-  }
-  *out = h;
-  return DSX_OK;
+size_t dpt_workspace_bytes(const dsx_durpred_train* h, int B, int T, int od) {
+  return ws_carve(h, B, T, od, nullptr, nullptr);
 }
 
-void dsx_durpred_train_destroy(dsx_durpred_train* h) {
-  if (!h) return;
-  cudaSetDevice(h->device);
-  cudaDeviceSynchronize();
-  h->mem.free_all();
-  dsx_durpred_destroy(h->fwd);
-  delete h;
-}
-
-int dsx_durpred_train_tape_bytes(dsx_durpred_train* h, int B, int T, size_t* out) {
-  DSX_CHECK(h && out, DSX_E_INVALID, "null handle or out");
-  DSX_TRY(check_geom(h, B, T));
-  *out = tape_carve(h->cfg, B, T, nullptr, nullptr);
-  return DSX_OK;
-}
-
-int dsx_durpred_train_workspace_bytes(dsx_durpred_train* h, int B, int T, size_t* out) {
-  DSX_CHECK(h && out, DSX_E_INVALID, "null handle or out");
-  DSX_TRY(check_geom(h, B, T));
-  *out = ws_carve(h, B, T, nullptr, nullptr);
-  return DSX_OK;
-}
-
-int dsx_durpred_train_forward(dsx_durpred_train* h, const dsx_durpred_params* w, const float* x, dsx_strides xs_,
-                              const uint8_t* mask, int B, int T, float p_drop, uint64_t seed, void* tape,
-                              size_t tape_bytes, void* workspace, size_t workspace_bytes, float* xs, void* stream) {
-  (void)workspace;   // the forward writes only the tape and xs
-  (void)workspace_bytes;
-  DSX_TRY(check_geom(h, B, T));
-  DSX_TRY(check_params(h, w, "the parameters"));
-  DSX_CHECK(x && mask && tape && xs, DSX_E_INVALID, "x, mask, tape and xs must not be NULL");
-  DSX_CHECK(p_drop >= 0.f && p_drop < 1.f, DSX_E_INVALID, "dropout p = %g is outside [0, 1)", static_cast<double>(p_drop));
-  const size_t need = tape_carve(h->cfg, B, T, nullptr, nullptr);
-  DSX_CHECK(tape_bytes >= need, DSX_E_INVALID, "tape of %zu bytes is below the %zu this (B, T) needs", tape_bytes, need);
-  DSX_CUDA(cudaSetDevice(h->device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  Tape tp;
-  tape_carve(h->cfg, B, T, static_cast<uint8_t*>(tape), &tp);
-  tp.tr.seed = seed;
-  tp.tr.p = p_drop;
-  const size_t F = static_cast<size_t>(B) * T;
-  k_dpt_hdr<<<static_cast<unsigned>(std::min<size_t>((F + 255) / 256, 1024)), 256, 0, s>>>(tp.hdr, seed, p_drop, B, T,
-                                                                                          mask, tp.pad);
-  DSX_TRY(launch_check("k_dpt_hdr"));
-  DSX_TRY(durpred_train_pack(h->fwd, w, s));
-  return durpred_train_run(h->fwd, x, xs_, tp.pad, B, T, tp.tr, xs, s);
-}
-
-int dsx_durpred_train_backward(dsx_durpred_train* h, const dsx_durpred_params* w, const void* tape, const float* d_xs,
-                               const dsx_durpred_params* grads, float* d_x, int B, int T, void* workspace,
-                               size_t workspace_bytes, void* stream) {
-  DSX_TRY(check_geom(h, B, T));
-  DSX_TRY(check_params(h, w, "the parameters"));
-  DSX_TRY(check_params(h, grads, "the gradients"));
-  DSX_CHECK(tape && d_xs && workspace, DSX_E_INVALID, "tape, d_xs and workspace must not be NULL");
-  const size_t wneed = ws_carve(h, B, T, nullptr, nullptr);
-  DSX_CHECK(workspace_bytes >= wneed, DSX_E_INVALID, "workspace of %zu bytes is below the %zu this (B, T) needs",
-            workspace_bytes, wneed);
-  DSX_CUDA(cudaSetDevice(h->device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
+int dpt_backward(dsx_durpred_train* h, const dsx_durpred_params* w, const DurTape& tp, const float* d_out, int od,
+                 const dsx_durpred_params* grads, float* d_x, int B, int T, void* workspace, cudaStream_t s) {
   const dsx_durpred_config& c = h->cfg;
   const int P = c.chans, L = c.layers, k = c.kernel, F = B * T, mtiles = (T + kConvRows - 1) / kConvRows;
-  Tape tp;
-  tape_carve(c, B, T, static_cast<uint8_t*>(const_cast<void*>(tape)), &tp);
   Ws ws;
-  ws_carve(h, B, T, static_cast<uint8_t*>(workspace), &ws);
+  ws_carve(h, B, T, od, static_cast<uint8_t*>(workspace), &ws);
   auto gp = [](const float* q) { return const_cast<float*>(q); };
 
-  k_dpt_amax<<<1, 1024, 0, s>>>(d_xs, tp.pad, static_cast<size_t>(F), ws.amax);
+  k_dpt_amax<<<1, 1024, 0, s>>>(d_out, tp.pad, static_cast<size_t>(F), od, ws.amax);
   DSX_TRY(launch_check("k_dpt_amax"));
   k_scale<<<1, 1, 0, s>>>(ws.amax, ws.scal);
   DSX_TRY(launch_check("k_scale"));
@@ -640,7 +584,7 @@ int dsx_durpred_train_backward(dsx_durpred_train* h, const dsx_durpred_params* w
   }
 
   DpHeadArgs ha{};
-  ha.dxs = d_xs;
+  ha.dxs = d_out;
   ha.pad = tp.pad;
   ha.hin = tp.tr.hin;
   ha.r = tp.tr.r[L - 1];
@@ -653,7 +597,12 @@ int dsx_durpred_train_backward(dsx_durpred_train* h, const dsx_durpred_params* w
   ha.part = ws.hpart;
   ha.F = F;
   ha.P = P;
-  k_dpt_head<<<kHeadBlocks, 256, 0, s>>>(ha);
+  ha.od = od;
+  if (od == 1) k_dpt_head<1><<<kHeadBlocks, 256, 0, s>>>(ha);
+  else if (od == 2) k_dpt_head<2><<<kHeadBlocks, 256, 0, s>>>(ha);
+  else if (od <= 4) k_dpt_head<4><<<kHeadBlocks, 256, 0, s>>>(ha);
+  else if (od <= 8) k_dpt_head<8><<<kHeadBlocks, 256, 0, s>>>(ha);
+  else k_dpt_head<16><<<kHeadBlocks, 256, 0, s>>>(ha);
   DSX_TRY(launch_check("k_dpt_head"));
 
   int cur = 0;
@@ -723,7 +672,7 @@ int dsx_durpred_train_backward(dsx_durpred_train* h, const dsx_durpred_params* w
     const bool last = l == L - 1;
     lr.part[l] = last ? ws.hpart : ws.lnp + static_cast<size_t>(l) * ws.lnp_stride;
     lr.blocks[l] = last ? kHeadBlocks : B * mtiles;
-    lr.stride[l] = last ? 3 * P + 1 : 2 * P;
+    lr.stride[l] = last ? head_part_floats(P, od) : 2 * P;
     lr.dgamma[l] = gp(grads->ln_w[l]);
     lr.dbeta[l] = gp(grads->ln_b[l]);
   }
@@ -731,13 +680,117 @@ int dsx_durpred_train_backward(dsx_durpred_train* h, const dsx_durpred_params* w
   lr.dbl = gp(grads->linear_b);
   lr.L = L;
   lr.P = P;
+  lr.od = od;
   lr.hdr = tp.hdr;
   lr.B = B;
   lr.T = T;
   lr.scal = ws.scal;
-  const int nout = (2 * L + 1) * P + 1;
+  const int nout = 2 * L * P + od * (P + 1);
   k_dpt_lnreduce<<<(nout + 255) / 256, 256, 0, s>>>(lr);
   return launch_check("k_dpt_lnreduce");
+}
+
+}  // namespace dsx
+
+using namespace dsx;
+
+extern "C" {
+
+int dsx_durpred_train_create(int device, const dsx_durpred_config* cfg, dsx_durpred_train** out) {
+  DSX_CHECK(out, DSX_E_INVALID, "out is NULL");
+  *out = nullptr;
+  dsx_durpred* fwd = nullptr;
+  DSX_TRY(dsx_durpred_create(device, cfg, &fwd));   // validates the configuration and selects the device
+  dsx_durpred_train* h = new dsx_durpred_train();
+  h->device = device;
+  h->cfg = *cfg;
+  h->fwd = fwd;
+  int rc = [&]() -> int {
+    DSX_TRY(durpred_train_alloc(fwd));
+    DSX_TRY(conv_opt_in<256>([](auto k) { return k_dpt_dgrad<decltype(k)::value>; }));
+    DSX_CUDA(cudaFuncSetAttribute(k_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmem));
+    const int P = cfg->chans;
+    for (int i = 0; i < cfg->layers; ++i) {   // gx[t] = sum_j W_j^T GU[t - tap0 - j]
+      ConvGemm& g = h->dgrad[i];
+      g.cin = P;
+      g.n = i ? P : cfg->idim;
+      g.taps = cfg->kernel;
+      g.tap0 = -tap0_of(*cfg);
+      g.tstep = -1;
+      DSX_TRY(conv_alloc(h->mem, g, 256));
+    }
+    return DSX_OK;
+  }();
+  if (rc != DSX_OK) {
+    dsx_durpred_train_destroy(h);
+    return rc;
+  }
+  *out = h;
+  return DSX_OK;
+}
+
+void dsx_durpred_train_destroy(dsx_durpred_train* h) {
+  if (!h) return;
+  cudaSetDevice(h->device);
+  cudaDeviceSynchronize();
+  h->mem.free_all();
+  dsx_durpred_destroy(h->fwd);
+  delete h;
+}
+
+int dsx_durpred_train_tape_bytes(dsx_durpred_train* h, int B, int T, size_t* out) {
+  DSX_CHECK(h && out, DSX_E_INVALID, "null handle or out");
+  DSX_TRY(check_geom(h, B, T));
+  *out = tape_carve(h->cfg, B, T, nullptr, nullptr);
+  return DSX_OK;
+}
+
+int dsx_durpred_train_workspace_bytes(dsx_durpred_train* h, int B, int T, size_t* out) {
+  DSX_CHECK(h && out, DSX_E_INVALID, "null handle or out");
+  DSX_TRY(check_geom(h, B, T));
+  *out = ws_carve(h, B, T, 1, nullptr, nullptr);
+  return DSX_OK;
+}
+
+int dsx_durpred_train_forward(dsx_durpred_train* h, const dsx_durpred_params* w, const float* x, dsx_strides xs_,
+                              const uint8_t* mask, int B, int T, float p_drop, uint64_t seed, void* tape,
+                              size_t tape_bytes, void* workspace, size_t workspace_bytes, float* xs, void* stream) {
+  (void)workspace;   // the forward writes only the tape and xs
+  (void)workspace_bytes;
+  DSX_TRY(check_geom(h, B, T));
+  DSX_TRY(check_params(h, w, "the parameters"));
+  DSX_CHECK(x && mask && tape && xs, DSX_E_INVALID, "x, mask, tape and xs must not be NULL");
+  DSX_CHECK(p_drop >= 0.f && p_drop < 1.f, DSX_E_INVALID, "dropout p = %g is outside [0, 1)", static_cast<double>(p_drop));
+  const size_t need = tape_carve(h->cfg, B, T, nullptr, nullptr);
+  DSX_CHECK(tape_bytes >= need, DSX_E_INVALID, "tape of %zu bytes is below the %zu this (B, T) needs", tape_bytes, need);
+  DSX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  Tape tp;
+  tape_carve(h->cfg, B, T, static_cast<uint8_t*>(tape), &tp);
+  tp.tr.seed = seed;
+  tp.tr.p = p_drop;
+  const size_t F = static_cast<size_t>(B) * T;
+  k_dpt_hdr<<<static_cast<unsigned>(std::min<size_t>((F + 255) / 256, 1024)), 256, 0, s>>>(tp.hdr, seed, p_drop, B, T,
+                                                                                          mask, tp.pad);
+  DSX_TRY(launch_check("k_dpt_hdr"));
+  DSX_TRY(durpred_train_pack(h->fwd, w, s));
+  return durpred_train_run(h->fwd, x, xs_, tp.pad, B, T, tp.tr, xs, s);
+}
+
+int dsx_durpred_train_backward(dsx_durpred_train* h, const dsx_durpred_params* w, const void* tape, const float* d_xs,
+                               const dsx_durpred_params* grads, float* d_x, int B, int T, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  DSX_TRY(check_geom(h, B, T));
+  DSX_TRY(check_params(h, w, "the parameters"));
+  DSX_TRY(check_params(h, grads, "the gradients"));
+  DSX_CHECK(tape && d_xs && workspace, DSX_E_INVALID, "tape, d_xs and workspace must not be NULL");
+  const size_t wneed = ws_carve(h, B, T, 1, nullptr, nullptr);
+  DSX_CHECK(workspace_bytes >= wneed, DSX_E_INVALID, "workspace of %zu bytes is below the %zu this (B, T) needs",
+            workspace_bytes, wneed);
+  DSX_CUDA(cudaSetDevice(h->device));
+  Tape tp;
+  tape_carve(h->cfg, B, T, static_cast<uint8_t*>(const_cast<void*>(tape)), &tp);
+  return dpt_backward(h, w, tp, d_xs, 1, grads, d_x, B, T, workspace, static_cast<cudaStream_t>(stream));
 }
 
 int dsx_durpred_train_masks(dsx_durpred_train* h, uint64_t seed, float p_drop, int B, int T, uint8_t* const* out,

@@ -461,13 +461,37 @@ struct DurTrain {
 };
 // The training step's forward packs live in a dsx_durpred handle: durpred_train_alloc sizes them once (the handle then
 // counts as loaded), durpred_train_pack refills them from the caller's fp32 weights on the stream (no allocation, no
-// synchronisation) and points the LayerNorm affines at the caller's arrays.
+// synchronisation) and points the LayerNorm affines at the caller's arrays; head = false leaves out the duration head's
+// weights (the pitch predictor's stack has a head of its own).
 int durpred_train_alloc(dsx_durpred* h);
-int durpred_train_pack(dsx_durpred* h, const dsx_durpred_params* p, cudaStream_t s);
+int durpred_train_pack(dsx_durpred* h, const dsx_durpred_params* p, cudaStream_t s, bool head = true);
 // x (any strides) -> tr.a[0], then the layers in training form (k_pe_conv<NT, true>): xs [B][T], 0 on padding.
 // 1 + n_layers launches.
 int durpred_train_run(const dsx_durpred* h, const float* x, dsx_strides xs_, const uint8_t* mask, int B, int T,
                       const DurTrain& tr, float* xs, cudaStream_t s);
+// DurationPredictor._forward's layers from layer 0's fp16 operand: eval (tr == NULL) from A[0], alternating A[0] and A[1];
+// training (tr) from tr->a[0], as durpred_train_run.  With a mask, the duration head follows -> xs, dur (see
+// dsx_durpred_forward).  mask == NULL is the pitch predictor's stack (tts_modules.py:222-235, dsx_pitchtrain.cu): nothing
+// is masked, and the last layer's output after dropout goes to hin [F][chans] fp32 instead of a head.  n_layers launches.
+int dp_stack_run(const dsx_durpred* h, __half* const* A, const uint8_t* mask, int B, int T, float* xs, int64_t* dur,
+                 const DurTrain* tr, float* hin, cudaStream_t s);
+
+// ---- dsx_durtrain.cu: the duration predictor step's backward, shared with the pitch predictor step (dsx_pitchtrain.cu)
+// the regions of a training tape the backward reads
+struct DurTape {
+  Fs2TapeHdr* hdr;
+  uint8_t* pad;                // [F] the forward's mask, or NULL: no mask
+  DurTrain tr;
+};
+dsx_durpred* dpt_forward_handle(dsx_durpred_train* h);   // the forward's packs and kernels
+// workspace bytes of dpt_backward over (B, T) with a head of od outputs (1..16)
+size_t dpt_workspace_bytes(const dsx_durpred_train* h, int B, int T, int od);
+// The backward from d_out [F][od] (unscaled) through a head Linear(chans, od) (* !mask when tp.pad) and the layers:
+// every gradient through grads (linear_w [od][chans], linear_b [od]) and d_x [F][idim] (or NULL), all written.  S is
+// the power of two from amax |d_out * !mask| over every column.  B, T and the pointers are checked by the caller.
+// 4 + 4 L launches for k <= 4; no allocation, no synchronisation.
+int dpt_backward(dsx_durpred_train* h, const dsx_durpred_params* w, const DurTape& tp, const float* d_out, int od,
+                 const dsx_durpred_params* grads, float* d_x, int B, int T, void* workspace, cudaStream_t s);
 
 // ---- dsx_fftdiff.cu: the FFT denoiser of the sampler handle ---------------------------------------------------------
 int fft_create(int device, const dsx_fft_config* c, const dsx_fft_params* p, cudaStream_t s, FftDenoiser** out);

@@ -645,13 +645,14 @@ struct dsx_durpred {
   GrowBuffer ws;
 };
 
-namespace {
+namespace dsx {
 
 // DurationPredictor._forward (tts_modules.py:113-129): n_layers x [conv, ReLU, LayerNorm, (dropout), * !mask], then the
 // head, from layer 0's fp16 operand A[0].  Eval (tr == NULL) alternates A[0] and A[1]; training reads layer i's operand
-// from tr->a[i], writes layer i + 1's there, and saves the LayerNorm inputs and the head's input (DurTrain).
-int dp_layers(const dsx_durpred* h, __half* const* A, const uint8_t* mask, int B, int T, float* xs, int64_t* dur,
-              const DurTrain* tr, cudaStream_t s) {
+// from tr->a[i], writes layer i + 1's there, and saves the LayerNorm inputs and the head's input (DurTrain).  Without a
+// mask (the pitch predictor), the last layer's output goes to hin (fp32) and no head runs.
+int dp_stack_run(const dsx_durpred* h, __half* const* A, const uint8_t* mask, int B, int T, float* xs, int64_t* dur,
+                 const DurTrain* tr, float* hin, cudaStream_t s) {
   const dsx_durpred_config& c = h->cfg;
   const int P = c.chans;
   int cur = 0;
@@ -664,8 +665,12 @@ int dp_layers(const dsx_durpred* h, __half* const* A, const uint8_t* mask, int B
     a.shift = h->conv[i].t;
     if (i + 1 < c.layers) {
       a.mode = PE_LN;
-      a.flags = PE_MASK | PE_OUT16;
+      a.flags = (mask ? PE_MASK : 0) | PE_OUT16;
       a.o16 = tr ? tr->a[i + 1] : A[cur ^ 1];
+    } else if (!mask) {
+      a.mode = PE_LN;
+      a.flags = PE_OUT32;
+      a.o32 = hin;
     } else {
       a.mode = PE_DUR;
       a.hw = h->head;
@@ -693,7 +698,7 @@ int dp_layers(const dsx_durpred* h, __half* const* A, const uint8_t* mask, int B
   return DSX_OK;
 }
 
-}  // namespace
+}  // namespace dsx
 
 namespace dsx {
 
@@ -714,7 +719,7 @@ int durpred_train_alloc(dsx_durpred* h) {
   return DSX_OK;
 }
 
-int durpred_train_pack(dsx_durpred* h, const dsx_durpred_params* p, cudaStream_t s) {
+int durpred_train_pack(dsx_durpred* h, const dsx_durpred_params* p, cudaStream_t s, bool head) {
   const dsx_durpred_config& c = h->cfg;
   const int P = c.chans;
   for (int i = 0; i < c.layers; ++i) {
@@ -723,6 +728,7 @@ int durpred_train_pack(dsx_durpred* h, const dsx_durpred_params* p, cudaStream_t
     pc.s = const_cast<float*>(p->ln_w[i]);
     pc.t = const_cast<float*>(p->ln_b[i]);
   }
+  if (!head) return DSX_OK;
   DSX_CUDA(cudaMemcpyAsync(h->head, p->linear_w, P * sizeof(float), cudaMemcpyDeviceToDevice, s));
   DSX_CUDA(cudaMemcpyAsync(h->head + P, p->linear_b, sizeof(float), cudaMemcpyDeviceToDevice, s));
   return DSX_OK;
@@ -733,7 +739,7 @@ int durpred_train_run(const dsx_durpred* h, const float* x, dsx_strides xs_, con
   const size_t frames = static_cast<size_t>(B) * T;
   k_dp_pack<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(x, xs_, B, T, h->cfg.idim, tr.a[0]);
   DSX_TRY(launch_check("k_dp_pack"));
-  return dp_layers(h, nullptr, mask, B, T, xs, nullptr, &tr, s);
+  return dp_stack_run(h, nullptr, mask, B, T, xs, nullptr, &tr, nullptr, s);
 }
 
 }  // namespace dsx
@@ -828,7 +834,7 @@ int dsx_durpred_forward(dsx_durpred* h, const float* x, dsx_strides xs_, const u
   __half* A[2] = {ws.take<__half>(frames * C * 2), ws.take<__half>(frames * C * 2)};
   k_dp_pack<<<static_cast<unsigned>((frames * 32 + 255) / 256), 256, 0, s>>>(x, xs_, B, T, c.idim, A[0]);
   DSX_TRY(launch_check("k_dp_pack"));
-  return dp_layers(h, A, mask, B, T, xs, dur, nullptr, s);
+  return dp_stack_run(h, A, mask, B, T, xs, dur, nullptr, nullptr, s);
 }
 
 }  // extern "C"

@@ -47,6 +47,16 @@ encoders and the duration predictor run their sm_90a training steps; ``FastSpeec
 scaling of the predictor's input stays in the reference's graph.  ``install_fs2_encoder(duration_predictor=False)``
 leaves the reference's ``DurationPredictor`` in place, so it trains in eager PyTorch.  ``uninstall_fs2_encoder()``
 restores whatever was swapped.
+
+    dropin.install_fs2_predictors()   # before the model is built
+
+rebinds ``PitchPredictor`` and ``EnergyPredictor`` in ``modules.fastspeech.fs2`` and ``modules.diffsinger_midi.fs2``
+(where the module has the name) to the classes of ``diffsinger_b200.pitchpred``, so the next ``FastSpeech2`` /
+``FastSpeech2MIDI`` builds its pitch predictor -- the one inside ``cwt_predictor``'s ``Sequential(Linear,
+PitchPredictor)`` included, whose ``Linear`` stays eager -- and its energy predictor on dsx.  Under ``dsx_train`` they run
+their sm_90a training steps.  ``modules.fastspeech.tts_modules`` and ``modules.fastspeech.pe`` keep the reference's
+classes, so the reference's ``PitchExtractor`` keeps its own predictor.  ``uninstall_fs2_predictors()`` restores
+whatever was swapped.
 """
 import importlib
 import sys
@@ -302,3 +312,32 @@ def uninstall_fs2_encoder():
         if mod is not None:
             setattr(mod, attr, ref)
         del _fs2enc[(name, attr)]
+
+
+_fs2pred = {}
+_FS2PRED_NAMES = ("PitchPredictor", "EnergyPredictor")
+
+
+def install_fs2_predictors():
+    from . import pitchpred
+    for name in _FS2_MODULES:
+        try:
+            mod = importlib.import_module(name)
+        except ModuleNotFoundError as e:
+            if e.name is None or not name.startswith(e.name):      # a missing dependency, not a missing module
+                raise
+            continue
+        for attr in _FS2PRED_NAMES:
+            if not hasattr(mod, attr):
+                continue
+            _fs2pred.setdefault((name, attr), getattr(mod, attr))
+            setattr(mod, attr, getattr(pitchpred, attr))
+    return pitchpred.PitchPredictor
+
+
+def uninstall_fs2_predictors():
+    for (name, attr), ref in list(_fs2pred.items()):
+        mod = sys.modules.get(name)
+        if mod is not None:
+            setattr(mod, attr, ref)
+        del _fs2pred[(name, attr)]

@@ -617,6 +617,97 @@ int dsx_durpred_train_backward(dsx_durpred_train* h, const dsx_durpred_params* w
 int dsx_durpred_train_masks(dsx_durpred_train* h, uint64_t seed, float p_drop, int B, int T, uint8_t* const* out,
                             void* stream);
 
+/* ---- Pitch and energy predictors -------------------------------------------------------------------------------------
+ * Replaces: PitchPredictor.forward and EnergyPredictor.forward (modules/fastspeech/tts_modules.py:192-240), as
+ * FastSpeech2.add_pitch / add_energy call them (modules/fastspeech/fs2.py:176-231): xs + pos_embed_alpha * table[pos]
+ * with pos = make_positions(xs[..., 0], 0) (utils/__init__.py:145-157) and the sinusoidal table of
+ * SinusoidalPositionalEmbedding(idim, 0) (modules/commons/common_layers.py:88-135, evaluated in fp32 without a size
+ * limit, so T past its init_size needs no regrowth), then n_layers x [ConstantPad1d + Conv1d, ReLU, LayerNorm over
+ * channels (eps 1e-12), Dropout], then Linear(chans, odim).  Nothing is masked: a padding frame gets what the reference
+ * gives it.  The convolutions run on the duration predictor's tensor-core kernel (fp16 operands, fp32 accumulation);
+ * the position term, LayerNorm and the head are fp32. */
+typedef struct dsx_pitchpred dsx_pitchpred;
+
+typedef struct {
+  int idim;              /* input channels (hidden_size, or 128 behind the CWT Linear): a multiple of 16 in [16, 256] */
+  int chans;             /* n_chans (predictor_hidden, or hidden_size when that is <= 0): same range                */
+  int layers;            /* n_layers (predictor_layers): 1..16                                                      */
+  int kernel;            /* kernel_size (predictor_kernel): 1..31, odd for SAME                                     */
+  int padding;           /* 0 'SAME' ((k - 1) / 2 each side), 1 'LEFT' (k - 1 on the left)                          */
+  int odim;              /* outputs of the head: 1..16 (2 for f0 and uv, 1 for energy or ph, 11 for CWT)            */
+} dsx_pitchpred_config;
+
+typedef struct {
+  const float* const* conv_w;        /* conv.i.1.weight [chans, C_in, k], HOST array of n_layers device pointers  */
+  const float* const* conv_b;        /* conv.i.1.bias [chans]                                                     */
+  const float* const* ln_w;          /* conv.i.3.weight [chans]                                                   */
+  const float* const* ln_b;          /* conv.i.3.bias [chans]                                                     */
+  const float* linear_w;             /* linear.weight [odim, chans]                                               */
+  const float* linear_b;             /* linear.bias [odim]                                                        */
+  const float* pos_embed_alpha;      /* pos_embed_alpha [1]                                                       */
+} dsx_pitchpred_params;
+
+/* DSX_E_INVALID ("unsupported ...") for a configuration outside the ranges above. */
+int dsx_pitchpred_create(int device, const dsx_pitchpred_config* cfg, dsx_pitchpred** out);
+void dsx_pitchpred_destroy(dsx_pitchpred* h);
+int dsx_pitchpred_load(dsx_pitchpred* h, const dsx_pitchpred_params* p, void* stream);
+
+/* Replaces: PitchPredictor.forward(xs) in eval mode (tts_modules.py:222-235).
+ *   x    fp32 [B, T, idim] contiguous;
+ *   out  [B, T, odim] contiguous fp32.
+ * The training forward's kernels with p = 0 and no tape: at p = 0 dsx_pitchpred_train_forward gives the same bits. */
+int dsx_pitchpred_forward(dsx_pitchpred* h, const float* x, int B, int T, float* out, void* stream);
+
+/* ---- Pitch and energy predictor training step ------------------------------------------------------------------------
+ * Replaces: PitchPredictor.forward(xs) (tts_modules.py:222-235) in training mode, and its autograd backward: the gradient
+ * of every parameter, pos_embed_alpha included, and of xs.  The forward is dsx_pitchpred_forward's with Dropout(p) at
+ * site i after layer i's LayerNorm, the masks from Philox4x32-10 keyed by (seed, site, frame, channel) as in the other
+ * training steps (torch's distribution, not its stream).  No gradient flows through the positions, which are integers:
+ * d_x is the gradient at the first convolution's input, and d_pos_embed_alpha = sum over frames and channels of that
+ * gradient times table[pos], summed in a fixed order.  The backward is the duration predictor step's with no mask and a
+ * head of odim outputs: the fp16 gradient operands are scaled by a power of two S chosen on the device (S amax |d_out|
+ * over all odim columns in [2^5, 2^6)) and divided out exactly, so 2^k d_out gives exactly 2^k times every gradient and
+ * d_out = 0 exact zeros.  Gradients are written, not accumulated, and bitwise reproducible (fixed-order reductions, no
+ * atomics).  No call allocates or synchronises the host: the tape and the workspace are the caller's.  Calls on one
+ * handle must not overlap on different streams (the weights are packed into it). */
+typedef struct dsx_pitchpred_train dsx_pitchpred_train;
+
+/* Accepts what dsx_pitchpred_create accepts (DSX_E_INVALID, "unsupported ..."). */
+int dsx_pitchpred_train_create(int device, const dsx_pitchpred_config* cfg, dsx_pitchpred_train** out);
+void dsx_pitchpred_train_destroy(dsx_pitchpred_train* h);
+
+/* Bytes of the tape of one forward over B utterances of T frames (F = B T, P = chans, L = layers, each region rounded up
+ * to 256 bytes, a256):
+ *   a256(24) + a256(4 F) + a256(2 F idim) + L a256(4 F P) + (L - 1) a256(2 F P) + a256(4 F P)
+ * the header (seed, p, B, T), the int32 positions, each layer's fp16 input (layer 0's is x plus the position term), each
+ * layer's LayerNorm input and the head's input.  The masks are not stored: the backward draws them again from the seed
+ * and p the tape records. */
+int dsx_pitchpred_train_tape_bytes(dsx_pitchpred_train* h, int B, int T, size_t* out);
+
+/* Bytes of the scratch workspace a backward over (B, T) needs; it holds nothing between calls. */
+int dsx_pitchpred_train_workspace_bytes(dsx_pitchpred_train* h, int B, int T, size_t* out);
+
+/* One training forward: out [B, T, odim] contiguous fp32 of x (fp32 [B, T, idim] contiguous), with dropout p_drop in
+ * [0, 1) drawn from `seed`, and what the backward needs written to `tape` (at least dsx_pitchpred_train_tape_bytes).
+ * The forward uses no workspace: workspace may be NULL and workspace_bytes 0.  Several forwards may precede their
+ * backwards, each with its own tape. */
+int dsx_pitchpred_train_forward(dsx_pitchpred_train* h, const dsx_pitchpred_params* w, const float* x, int B, int T,
+                                float p_drop, uint64_t seed, void* tape, size_t tape_bytes, void* workspace,
+                                size_t workspace_bytes, float* out, void* stream);
+
+/* The backward of the forward that wrote `tape`, with that forward's B and T and weights w: d_out [B, T, odim]
+ * contiguous.  Writes the fp32 gradient of every parameter through `grads` (same layout as w), and d_x [B, T, idim]
+ * contiguous unless NULL.  The tape is only read.  A (B, T) other than the tape's makes every gradient NaN (checked on
+ * the device).  A scaled fp16 gradient operand beyond fp16's range saturates at +-65504 rather than becoming inf. */
+int dsx_pitchpred_train_backward(dsx_pitchpred_train* h, const dsx_pitchpred_params* w, const void* tape,
+                                 const float* d_out, const dsx_pitchpred_params* grads, float* d_x, int B, int T,
+                                 void* workspace, size_t workspace_bytes, void* stream);
+
+/* Test entry: the n_layers keep masks (1 kept, 0 dropped) that dsx_pitchpred_train_forward(seed, p_drop) draws, in site
+ * (layer) order; out is a HOST array of n_layers device pointers to uint8 [B, T, chans]. */
+int dsx_pitchpred_train_masks(dsx_pitchpred_train* h, uint64_t seed, float p_drop, int B, int T, uint8_t* const* out,
+                              void* stream);
+
 /* ---- Length regulator ------------------------------------------------------------------------------------------------
  * Replaces: LengthRegulator.forward(dur, dur_padding, alpha) (modules/fastspeech/tts_modules.py:159-189) in two calls,
  * because T_mel depends on the data, without its [B, T_txt, T_mel] temporaries.  Both run on the current device.
