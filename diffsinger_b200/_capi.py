@@ -44,11 +44,12 @@ SYMBOLS = (
     "dsx_pitchpred_train_create", "dsx_pitchpred_train_destroy", "dsx_pitchpred_train_tape_bytes",
     "dsx_pitchpred_train_workspace_bytes", "dsx_pitchpred_train_forward", "dsx_pitchpred_train_backward",
     "dsx_pitchpred_train_masks",
+    "dsx_pwg_create", "dsx_pwg_destroy", "dsx_pwg_load", "dsx_pwg_forward",
 )
 _VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy", "dsx_fs2dec_destroy",
          "dsx_fs2enc_destroy", "dsx_durpred_destroy", "dsx_train_destroy", "dsx_fs2dec_train_destroy",
          "dsx_fft_train_destroy", "dsx_fs2enc_train_destroy", "dsx_durpred_train_destroy", "dsx_pitchpred_destroy",
-         "dsx_pitchpred_train_destroy")
+         "dsx_pitchpred_train_destroy", "dsx_pwg_destroy")
 
 
 class DsxError(RuntimeError):
@@ -82,6 +83,21 @@ class HifiganParams(ctypes.Structure):
     _fields_ = [("conv_pre_w", _fp), ("conv_pre_g", _fp), ("conv_pre_b", _fp), ("ups_w", _fpp), ("ups_g", _fpp),
                 ("ups_b", _fpp), ("rb_w", _fpp), ("rb_g", _fpp), ("rb_b", _fpp), ("noise_w", _fpp), ("noise_b", _fpp),
                 ("source_w", _fp), ("source_b", _fp), ("conv_post_w", _fp), ("conv_post_g", _fp), ("conv_post_b", _fp)]
+
+
+class PwgConfig(ctypes.Structure):
+    _fields_ = [("layers", ctypes.c_int), ("stacks", ctypes.c_int), ("kernel_size", ctypes.c_int),
+                ("residual_channels", ctypes.c_int), ("gate_channels", ctypes.c_int), ("skip_channels", ctypes.c_int),
+                ("aux_channels", ctypes.c_int), ("aux_context_window", ctypes.c_int), ("num_scales", ctypes.c_int),
+                ("upsample_scales", ctypes.c_int * 4), ("use_pitch_embed", ctypes.c_int)]
+
+
+class PwgParams(ctypes.Structure):
+    _fields_ = [("first_w", _fp), ("first_g", _fp), ("first_b", _fp), ("conv_in_w", _fp), ("conv_in_g", _fp),
+                ("up_w", _fpp), ("up_g", _fpp), ("conv_w", _fpp), ("conv_g", _fpp), ("conv_b", _fpp), ("aux_w", _fpp),
+                ("aux_g", _fpp), ("out_w", _fpp), ("out_g", _fpp), ("out_b", _fpp), ("skip_w", _fpp), ("skip_g", _fpp),
+                ("skip_b", _fpp), ("last1_w", _fp), ("last1_g", _fp), ("last1_b", _fp), ("last3_w", _fp),
+                ("last3_g", _fp), ("last3_b", _fp), ("pitch_embed", _fp), ("c_proj_w", _fp), ("c_proj_b", _fp)]
 
 
 class PeConfig(ctypes.Structure):
@@ -270,6 +286,11 @@ lib.dsx_pitchpred_train_forward.argtypes = [_vp, ctypes.POINTER(PitchPredParams)
 lib.dsx_pitchpred_train_backward.argtypes = [_vp, ctypes.POINTER(PitchPredParams), _vp, _vp,
                                              ctypes.POINTER(PitchPredParams), _vp, _i, _i, _vp, ctypes.c_size_t, _vp]
 lib.dsx_pitchpred_train_masks.argtypes = [_vp, _u64, ctypes.c_float, _i, _i, ctypes.POINTER(_vp), _vp]
+lib.dsx_pwg_create.argtypes = [_i, ctypes.POINTER(PwgConfig), ctypes.POINTER(_vp)]
+lib.dsx_pwg_destroy.argtypes = [_vp]
+lib.dsx_pwg_destroy.restype = None
+lib.dsx_pwg_load.argtypes = [_vp, ctypes.POINTER(PwgParams), _vp]
+lib.dsx_pwg_forward.argtypes = [_vp, _vp, _vp, Strides, _vp, _i, _i, _vp, _vp]
 for _n in SYMBOLS:
     if _n not in _VOID:
         getattr(lib, _n).restype = _i

@@ -20,6 +20,7 @@
 #include "dsx_internal.h"
 #include "dsx_ptx.cuh"
 #include "dsx_rng.cuh"
+#include "dsx_wnorm.cuh"
 
 namespace dsx {
 namespace {
@@ -128,27 +129,6 @@ __global__ void __launch_bounds__(128) k_conv(const ConvArgs p) {
 }
 
 // ---- weight packing ------------------------------------------------------------------------------
-// scale[i] = g[i] / ||v[i]|| over the `inner` elements of index i of dim 0 (torch._weight_norm, dim 0); 1 without g
-__global__ void k_wnorm(const float* v, const float* g, int inner, float* scale) {
-  const int i = blockIdx.x;
-  float s = 0.f;
-  if (g) {
-    for (int e = threadIdx.x; e < inner; e += blockDim.x) {
-      const float x = v[static_cast<size_t>(i) * inner + e];
-      s = fmaf(x, x, s);
-    }
-  }
-  __shared__ float red[32];
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) t += red[w];
-    scale[i] = g ? g[i] / sqrtf(t) : 1.f;
-  }
-}
-
 // dst[r][j] = src[r][j] * (scale ? scale[0] : 1) for r < rows, 0 for rows <= r < rows_p (noise_convs, conv_post)
 __global__ void k_pack_rows(float* dst, const float* src, const float* scale, int rows, int rows_p, int cols) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;

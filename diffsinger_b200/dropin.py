@@ -21,6 +21,14 @@ replaces ``modules.hifigan.hifigan.HifiGanGenerator`` -- and the name bound from
 imported -- by ``diffsinger_b200.HifiGanGenerator``, so ``vocoders/hifigan.py:load_model`` (strict ``load_state_dict``,
 ``remove_weight_norm``, ``.to(device)``) and ``spec2wav`` run the vocoder on dsx unchanged.
 
+    dropin.install_pwg()
+
+replaces ``ParallelWaveGANGenerator`` in ``modules.parallel_wavegan.models`` and
+``modules.parallel_wavegan.models.parallel_wavegan`` -- and the name bound from them in ``vocoders.*`` modules already
+imported (vocoders/pwg.py binds it at import) -- by ``diffsinger_b200.ParallelWaveGANGenerator``, so
+``vocoders/pwg.py:load_pwg_model`` (``load_state_dict``, ``remove_weight_norm``, ``.eval().to(device)``) and ``spec2wav``
+run the PWG vocoder on dsx unchanged.  ``uninstall_pwg()`` restores the reference's class.
+
     dropin.install_pitch_extractor()
 
 replaces ``modules.fastspeech.pe.PitchExtractor`` -- and the name bound from it in ``inference.*`` / ``tasks.*`` /
@@ -230,6 +238,33 @@ def _swap_vocoder(old, new):
             continue
         if getattr(mod, "HifiGanGenerator", None) is old:
             mod.HifiGanGenerator = new
+
+
+_pwg = {}
+_PWG_MODULES = ("modules.parallel_wavegan.models", "modules.parallel_wavegan.models.parallel_wavegan")
+
+
+def install_pwg():
+    from .pwg import ParallelWaveGANGenerator
+    mod = importlib.import_module("modules.parallel_wavegan.models.parallel_wavegan")
+    if mod.ParallelWaveGANGenerator is not ParallelWaveGANGenerator:
+        _pwg["ref"] = mod.ParallelWaveGANGenerator
+    _swap_pwg(_pwg["ref"], ParallelWaveGANGenerator)
+    return ParallelWaveGANGenerator
+
+
+def uninstall_pwg():
+    if _pwg:
+        from .pwg import ParallelWaveGANGenerator
+        _swap_pwg(ParallelWaveGANGenerator, _pwg["ref"])
+
+
+def _swap_pwg(old, new):
+    for name, mod in list(sys.modules.items()):
+        if mod is None or not (name in _PWG_MODULES or name.startswith("vocoders.")):
+            continue
+        if getattr(mod, "ParallelWaveGANGenerator", None) is old:
+            mod.ParallelWaveGANGenerator = new
 
 
 _pe = {}

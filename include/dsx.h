@@ -320,6 +320,92 @@ int dsx_hifigan_forward(dsx_hifigan* h, const float* mel, dsx_strides ms, const 
                         const float* phase0, const float* src_noise, uint64_t seed, int B, int T, float* wav,
                         void* stream);
 
+/* ---- Parallel WaveGAN vocoder: noise + mel (+ coarse pitch) -> waveform ---------------------------------------------
+ * Replaces: ParallelWaveGANGenerator (modules/parallel_wavegan/models/parallel_wavegan.py:21-191) with its
+ * ConvInUpsampleNetwork (modules/parallel_wavegan/layers/upsample.py:16-183) and ResidualBlock
+ * (modules/parallel_wavegan/layers/residual_block.py:15-129, eval mode), as vocoders/pwg.py runs them.  The residual
+ * layers run on tensor cores with fp16 operands (the x taps, the upsampled conditioning, the gate output and the weights)
+ * and fp32 accumulation; the conditioning network, the residual stream, the skip sum and the head stay fp32.  A PWG
+ * handle is independent of the other handles. */
+typedef struct dsx_pwg dsx_pwg;
+
+/* The generator's hyper-parameters (ParallelWaveGANGenerator.__init__'s generator_params).  The kernels implement the
+ * published widths only; anything else is DSX_E_INVALID ("unsupported ..."). */
+typedef struct {
+  int layers;               /* 1..64                                                        */
+  int stacks;               /* layers % stacks == 0 and layers / stacks <= 16 (dilation 2^(l % (layers / stacks))) */
+  int kernel_size;          /* 3                                                            */
+  int residual_channels;    /* 64                                                           */
+  int gate_channels;        /* 128                                                          */
+  int skip_channels;        /* 64                                                           */
+  int aux_channels;         /* 80                                                           */
+  int aux_context_window;   /* w: 0..16 (conv_in has 2w + 1 taps)                           */
+  int num_scales;           /* len(upsample_scales): 1..4                                   */
+  int upsample_scales[4];   /* each 1..16; hop = their product <= 1024                      */
+  int use_pitch_embed;      /* 1: pitch_embed and c_proj exist and the forward reads pitch   */
+} dsx_pwg_config;
+
+/* Parameters, fp32 device pointers, each tensor contiguous in the reference's state-dict layout.  A weight-normalised
+ * conv passes weight_v as `*_w` and weight_g as `*_g`; a plain conv (after remove_weight_norm) passes `.weight` and
+ * `*_g` = NULL.  Per-layer arrays are HOST arrays of device pointers:
+ *   up_*:                     num_scales entries (upsample_net.upsample.up_layers.{2i + 1}, Conv2d [1, 1, 1, 2s + 1]);
+ *   conv_*, aux_*, out_*, skip_*: `layers` entries (conv_layers.l.conv, .conv1x1_aux, .conv1x1_out, .conv1x1_skip).
+ * A *_g array may be NULL as a whole.  pitch_embed and c_proj are NULL without use_pitch_embed. */
+typedef struct {
+  const float* first_w;        /* first_conv [64, 1, 1]                  */
+  const float* first_g;
+  const float* first_b;
+  const float* conv_in_w;      /* upsample_net.conv_in [80, 80, 2w + 1]  */
+  const float* conv_in_g;
+  const float* const* up_w;
+  const float* const* up_g;
+  const float* const* conv_w;  /* [128, 64, 3]                           */
+  const float* const* conv_g;
+  const float* const* conv_b;
+  const float* const* aux_w;   /* [128, 80, 1], no bias                  */
+  const float* const* aux_g;
+  const float* const* out_w;   /* [64, 64, 1]                            */
+  const float* const* out_g;
+  const float* const* out_b;
+  const float* const* skip_w;  /* [64, 64, 1]                            */
+  const float* const* skip_g;
+  const float* const* skip_b;
+  const float* last1_w;        /* last_conv_layers.1 [64, 64, 1]         */
+  const float* last1_g;
+  const float* last1_b;
+  const float* last3_w;        /* last_conv_layers.3 [1, 64, 1]          */
+  const float* last3_g;
+  const float* last3_b;
+  const float* pitch_embed;    /* pitch_embed.weight [300, 80]           */
+  const float* c_proj_w;       /* c_proj.weight [80, 160]                */
+  const float* c_proj_b;       /* c_proj.bias [80]                       */
+} dsx_pwg_params;
+
+/* Replaces: ParallelWaveGANGenerator(**generator_params) (parallel_wavegan.py:24-137).  Validates the configuration
+ * (DSX_E_INVALID). */
+int dsx_pwg_create(int device, const dsx_pwg_config* cfg, dsx_pwg** out);
+void dsx_pwg_destroy(dsx_pwg* h);
+
+/* Replaces: load_state_dict (+ remove_weight_norm, parallel_wavegan.py:174-189).  Applies the weight norm g * v / ||v||
+ * (norm over every dim but 0) and packs the fp16 tensor-core tiles.  Call again after every change of the weights. */
+int dsx_pwg_load(dsx_pwg* h, const dsx_pwg_params* p, void* stream);
+
+/* Replaces: ParallelWaveGANGenerator.forward(x, c, pitch) (parallel_wavegan.py:139-172) as vocoders/pwg.py:82-103
+ * (spec2wav) calls it.
+ *   z      the noise [B, 1, T * hop], contiguous (hop = the product of upsample_scales);
+ *   c      logically [B, 80, T + 2w], any element strides cs (spec2wav hands over a transposed view of the edge-padded
+ *          mel);
+ *   pitch  int64 [B, T + 2w], contiguous: the edge-padded coarse pitch.  Required with use_pitch_embed, where a value
+ *          outside [0, 300) reads a zero embedding row; ignored (may be NULL) without, as the reference ignores it;
+ *   wav    [B, 1, T * hop], contiguous.
+ * B >= 1, T >= 1 and B * T * hop <= 2^25 samples, checked before any device access.  Each utterance of a batch gives the
+ * same bits as that utterance alone (its convolutions are zero padded at its own edges), and repeated calls give the same
+ * bits.  The workspace grows to the largest call: 928 bytes per output sample (fp32 x and skip sum, two fp16 copies of
+ * x, the fp16 upsampled conditioning), plus 640 bytes per sample of the last upsampling stage's input (B * T * hop /
+ * upsample_scales[num_scales - 1]), plus 320 bytes per padded frame with use_pitch_embed. */
+int dsx_pwg_forward(dsx_pwg* h, const float* z, const float* c, dsx_strides cs, const int64_t* pitch, int B, int T,
+                    float* wav, void* stream);
+
 /* ---- Pitch extractor: mel -> f0 -------------------------------------------------------------------------------------
  * Replaces: PitchExtractor (modules/fastspeech/pe.py:119-149) with its Prenet (:7-41), ConvStacks (:81-116, GroupNorm),
  * PitchPredictor (modules/fastspeech/tts_modules.py:192-235, sinusoidal position embedding of
