@@ -10,12 +10,12 @@
 // backward, not stored.
 //
 // Backward, with GU the fp16 gradient at conv_i's output (before the ReLU), scaled by S:
-//   k_dpt_amax, k_scale    S from amax |d_xs * !mask| (S amax in [2^5, 2^6))
+//   k_dpt_amax, k_scale    S from amax |d_xs * !mask| (S amax in [2^5, 2^6)), NaN when the tape is of another (B, T)
 //   k_pack_conv x L        conv_i^T (taps reversed), the data-gradient packs of this backward's weights
 //   k_dpt_head             per token: the head's backward (d linear partials), then layer L - 1's dropout, LayerNorm and
 //                          ReLU backward -> GU
 //   per layer i = L - 1 .. 0:
-//     k_wgrad + k_dpt_wreduce   d conv_i (taps as shifted B tiles, four per launch) and its bias (the A column sums)
+//     k_wgrad + k_wgrad_sum     d conv_i (taps as shifted B tiles, four per launch) and its bias (the A column sums)
 //     k_dpt_dgrad               conv_i's stride-1 transposed conv of GU on conv_k_loop (a whole row of chans <= 256
 //                               columns in one CTA), with layer i - 1's * !mask, dropout, LayerNorm and ReLU backward in
 //                               the epilogue -> the next GU; at layer 0, d_x = the transposed conv / S
@@ -44,26 +44,6 @@ constexpr int kHeadBlocks = 256;    // CTAs of k_dpt_head: fixed, so its partial
 constexpr float kLnEps = 1e-12f;    // LayerNorm of tts_modules.py (not the 1e-5 of the FFT blocks)
 
 using TapeHdr = Fs2TapeHdr;
-
-__device__ __forceinline__ Fs2Drop hdr_drop(const TapeHdr* h, int site) {
-  Fs2Drop d;
-  d.seed = h->seed;
-  d.p = h->p;
-  d.inv_keep = 1.f / (1.f - d.p);
-  d.site = site;
-  return d;
-}
-
-// 1 / S, or NaN when the backward's (B, T) is not the tape's: every gradient is written through it
-__device__ __forceinline__ float inv_scale(const TapeHdr* h, int B, int T, const float* scal) {
-  return (h->B != B || h->T != T) ? __int_as_float(0x7fc00000) : scal[1];
-}
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 // a scaled gradient operand as fp16: a value beyond fp16's range saturates at +-65504 instead of becoming inf (NaN stays
 // NaN).  S keeps d_xs's largest value 2^10 below that (oracle/precision_study_durtrain.py measures 2^10 to 2^12 of
@@ -225,7 +205,7 @@ __global__ void __launch_bounds__(256) k_dpt_head(const DpHeadArgs p) {
 struct DgradArgs {
   ConvGemm g;                  // conv_i^T: g.cin = P (GU's channels), g.n = conv_i's input channels
   const __half* x;             // GU of layer i [F][P]
-  int T, B;
+  int T;
   float* dx;                   // layer 0: d_x [F][g.n] = the transposed conv / S
   const float* r;              // else layer i - 1's LayerNorm input [F][g.n] (tape)
   const float* gamma;          // layer i - 1's LayerNorm weight
@@ -258,7 +238,7 @@ __global__ void __launch_bounds__(128 * DgShape<NT>::WG) k_dpt_dgrad(const Dgrad
   const size_t rbase = static_cast<size_t>(b) * T;
   const int mrow[2] = {m0 + r0, m0 + r0 + 8};
   if (p.dx) {
-    const float is = inv_scale(p.hdr, p.B, T, p.scal);
+    const float is = p.scal[1];
 #pragma unroll
     for (int e = 0; e < NH / 2; e += 2) {
       const int col = c0 + acc_col(wtid, e), m = mrow[(e >> 1) & 1];
@@ -369,37 +349,6 @@ __global__ void __launch_bounds__(128 * DgShape<NT>::WG) k_dpt_dgrad(const Dgrad
 }
 
 // ---- reductions ---------------------------------------------------------------------------------------------------------
-// d conv_i taps j0 .. j0 + ntl - 1 ([P][cin][k]) and, with db, its bias: the k_wgrad partials in split order, / S
-struct WredArgs {
-  const float* part;
-  const float* bpart;
-  int splits, Mpad, Ntot, P, cin, k, j0, ntl;
-  float* dw;
-  float* db;
-  const TapeHdr* hdr;
-  int B, T;
-  const float* scal;
-};
-
-__global__ void k_dpt_wreduce(const WredArgs p) {
-  const float is = inv_scale(p.hdr, p.B, p.T, p.scal);
-  const size_t per_m = static_cast<size_t>(p.ntl) * p.cin, total = static_cast<size_t>(p.P) * per_m;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int m = static_cast<int>(i / per_m), rem = static_cast<int>(i % per_m), jj = rem / p.cin, c = rem % p.cin;
-    float s = 0.f;
-    for (int z = 0; z < p.splits; ++z) s += p.part[(static_cast<size_t>(z) * p.Mpad + m) * p.Ntot + jj * 256 + c];
-    p.dw[(static_cast<size_t>(m) * p.cin + c) * p.k + p.j0 + jj] = s * is;
-  }
-  if (p.db) {
-    for (int m = blockIdx.x * blockDim.x + threadIdx.x; m < p.P; m += gridDim.x * blockDim.x) {
-      float s = 0.f;
-      for (int z = 0; z < p.splits; ++z) s += p.bpart[static_cast<size_t>(z) * p.Mpad + m];
-      p.db[m] = s * is;
-    }
-  }
-}
-
 // every LayerNorm affine gradient and the head's: layer l's partials part[l] (blocks[l] rows of stride[l] floats, d gamma
 // then d beta), the head's (d linear.weight [od][P], then d linear.bias [od]) from column 2 P of the last layer's rows,
 // summed in row order, / S
@@ -411,8 +360,6 @@ struct LnRedArgs {
   float* dwl;
   float* dbl;
   int L, P, od;
-  const TapeHdr* hdr;
-  int B, T;
   const float* scal;
 };
 
@@ -422,7 +369,7 @@ __global__ void k_dpt_lnreduce(const LnRedArgs p) {
   const int l = t < 2 * p.L * P ? t / (2 * P) : p.L - 1, c = t < 2 * p.L * P ? t % (2 * P) : t - 2 * p.L * P + 2 * P;
   float s = 0.f;
   for (int k = 0; k < p.blocks[l]; ++k) s += p.part[l][static_cast<size_t>(k) * p.stride[l] + c];
-  s *= inv_scale(p.hdr, p.B, p.T, p.scal);
+  s *= p.scal[1];
   if (t >= 2 * p.L * P) {
     if (c < (2 + p.od) * P) p.dwl[c - 2 * P] = s;
     else p.dbl[c - (2 + p.od) * P] = s;
@@ -431,12 +378,6 @@ __global__ void k_dpt_lnreduce(const LnRedArgs p) {
   } else {
     p.dbeta[l][c - P] = s;
   }
-}
-
-__global__ void k_dpt_masks(Fs2Drop d, size_t F, int n, uint8_t* out) {
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < F * n;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x)
-    out[i] = dropout_scale(d, i / n, static_cast<int>(i % n)) != 0.f;
 }
 
 // ---- tape and workspace -------------------------------------------------------------------------------------------------
@@ -481,18 +422,6 @@ namespace {
 
 int tap0_of(const dsx_durpred_config& c) { return c.padding ? -(c.kernel - 1) : -(c.kernel - 1) / 2; }
 
-// floats of the largest k_wgrad partial slab (weights, then bias) of a launch of ntl <= 4 taps
-size_t wgrad_part_floats(const dsx_durpred_config& c, int F, int device) {
-  const int mt = (c.chans + 63) / 64;
-  size_t worst = 0;
-  for (int ntl = 1; ntl <= std::min(c.kernel, 4); ++ntl) {
-    const int fchunk = wgrad_fchunk(F, mt * ntl, device);
-    const size_t sp = (F + fchunk - 1) / fchunk;
-    worst = std::max(worst, sp * mt * 64 * ntl * 256 + sp * mt * 64);
-  }
-  return worst;
-}
-
 struct Ws {
   unsigned* amax;   // the scale's words, then the gradient operands and partial sums of dpt_backward
   float* scal;
@@ -522,7 +451,9 @@ size_t ws_carve(const dsx_durpred_train* h, int B, int T, int od, uint8_t* base,
   ws.hpart = reinterpret_cast<float*>(take(4 * static_cast<size_t>(kHeadBlocks) * head_part_floats(c.chans, od)));
   ws.lnp_stride = align256(4 * B * mt * 2 * P) / 4;
   ws.lnp = reinterpret_cast<float*>(take(4 * ws.lnp_stride * (c.layers - 1)));
-  ws.wpart = reinterpret_cast<float*>(take(4 * wgrad_part_floats(c, static_cast<int>(F), h->device)));
+  std::vector<std::pair<int, int>> shapes;   // (m tiles, n tiles) of the weight gradients: ntl <= 4 taps a launch
+  for (int ntl = 1; ntl <= std::min(c.kernel, 4); ++ntl) shapes.push_back({(c.chans + 63) / 64, ntl});
+  ws.wpart = reinterpret_cast<float*>(take(4 * wgrad_part_floats(static_cast<int>(F), shapes, h->device)));
   return n;
 }
 
@@ -550,7 +481,6 @@ template <int NT>
 int run_dgrad(DgradArgs a, const ConvGemm& g, int B, int T, cudaStream_t s) {
   a.g = g;
   a.T = T;
-  a.B = B;
   k_dpt_dgrad<NT><<<dim3((T + kConvRows - 1) / kConvRows, B), 128 * DgShape<NT>::WG, conv_smem<NT>(), s>>>(a);
   return launch_check("k_dpt_dgrad");
 }
@@ -576,7 +506,7 @@ int dpt_backward(dsx_durpred_train* h, const dsx_durpred_params* w, const DurTap
 
   k_dpt_amax<<<1, 1024, 0, s>>>(d_out, tp.pad, static_cast<size_t>(F), od, ws.amax);
   DSX_TRY(launch_check("k_dpt_amax"));
-  k_scale<<<1, 1, 0, s>>>(ws.amax, ws.scal);
+  k_scale<<<1, 1, 0, s>>>(ws.amax, ws.scal, tp.hdr, B, T);
   DSX_TRY(launch_check("k_scale"));
   for (int i = (d_x ? 0 : 1); i < L; ++i) {
     const ConvGemm& g = h->dgrad[i];
@@ -612,40 +542,23 @@ int dpt_backward(dsx_durpred_train* h, const dsx_durpred_params* w, const DurTap
     for (int j0 = 0; j0 < k; j0 += 4) {
       WgradArgs t{};
       const int ntl = std::min(4, k - j0);
+      WgradDst o{};
       for (int jj = 0; jj < ntl; ++jj) {
         t.b[jj] = tp.tr.a[i];
         t.ldb[jj] = cin;
         t.bn[jj] = cin;
         t.shift[jj] = tap0_of(c) + j0 + jj;
+        o.dst[jj] = gp(grads->conv_w[i]) + j0 + jj;
+        o.ms[jj] = cin * k;
+        o.cs[jj] = k;
       }
+      o.db = j0 == 0 ? gp(grads->conv_b[i]) : nullptr;
       t.a = ws.gu[cur];
       t.lda = P;
       t.am = P;
       t.F = F;
       t.T = T;
-      const int mt = (P + 63) / 64, fch = wgrad_fchunk(F, mt * ntl, h->device), sp = (F + fch - 1) / fch;
-      float* bp = ws.wpart + static_cast<size_t>(sp) * mt * 64 * ntl * 256;
-      DSX_TRY(run_wgrad(t, ntl, h->device, ws.wpart, j0 == 0 ? bp : nullptr, s));
-      WredArgs r{};
-      r.part = ws.wpart;
-      r.bpart = bp;
-      r.splits = sp;
-      r.Mpad = mt * 64;
-      r.Ntot = ntl * 256;
-      r.P = P;
-      r.cin = cin;
-      r.k = k;
-      r.j0 = j0;
-      r.ntl = ntl;
-      r.dw = gp(grads->conv_w[i]);
-      r.db = j0 == 0 ? gp(grads->conv_b[i]) : nullptr;
-      r.hdr = tp.hdr;
-      r.B = B;
-      r.T = T;
-      r.scal = ws.scal;
-      const size_t total = static_cast<size_t>(P) * ntl * cin;
-      k_dpt_wreduce<<<static_cast<unsigned>(std::min<size_t>((total + 255) / 256, 4096)), 256, 0, s>>>(r);
-      DSX_TRY(launch_check("k_dpt_wreduce"));
+      DSX_TRY(run_wgrad(t, ntl, o, ws.wpart, ws.scal, h->device, s));
     }
     if (i == 0 && !d_x) break;
     DgradArgs a{};
@@ -681,9 +594,6 @@ int dpt_backward(dsx_durpred_train* h, const dsx_durpred_params* w, const DurTap
   lr.L = L;
   lr.P = P;
   lr.od = od;
-  lr.hdr = tp.hdr;
-  lr.B = B;
-  lr.T = T;
   lr.scal = ws.scal;
   const int nout = 2 * L * P + od * (P + 1);
   k_dpt_lnreduce<<<(nout + 255) / 256, 256, 0, s>>>(lr);
@@ -800,15 +710,12 @@ int dsx_durpred_train_masks(dsx_durpred_train* h, uint64_t seed, float p_drop, i
   DSX_CHECK(p_drop >= 0.f && p_drop < 1.f, DSX_E_INVALID, "dropout p = %g is outside [0, 1)", static_cast<double>(p_drop));
   DSX_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  DurTrain tr;
-  tr.seed = seed;
-  tr.p = p_drop;
   const size_t F = static_cast<size_t>(B) * T, n = h->cfg.chans;
   for (int site = 0; site < h->cfg.layers; ++site) {
     DSX_CHECK(out[site], DSX_E_INVALID, "mask %d is NULL", site);
-    k_dpt_masks<<<static_cast<unsigned>(std::min<size_t>((F * n + 255) / 256, 4096)), 256, 0, s>>>(
-        tr.drop(site), F, static_cast<int>(n), out[site]);
-    DSX_TRY(launch_check("k_dpt_masks"));
+    k_drop_masks<<<static_cast<unsigned>(std::min<size_t>((F * n + 255) / 256, 4096)), 256, 0, s>>>(
+        make_drop(seed, p_drop, site), F, static_cast<int>(n), out[site]);
+    DSX_TRY(launch_check("k_drop_masks"));
   }
   return DSX_OK;
 }

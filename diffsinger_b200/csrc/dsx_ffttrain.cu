@@ -18,10 +18,10 @@
 // Backward, with S1 a power of two from amax |d_eps| and S2 one from amax |d| (d = d decoder_inp):
 //   k_fftt_eps16        S1 d_eps -> fp16 [F][M]
 //   k_fftt_gemm         d_out = d_eps . W_mel (fp32 [F][H], the stack's d_out)
-//   k_wgrad             dW_mel = d_eps^T out16 and db_mel
+//   run_wgrad           dW_mel = d_eps^T out16 and db_mel
 //   dsx_fs2dec_train_backward   every stack gradient and d = d decoder_inp (fp32 [F][H])
 //   k_fftt_half         S2 d -> fp16 [F][H]
-//   k_wgrad             [G_spec | G_cond] = d^T [x_t | cond] (hi planes) with db_d = sum_f d; G_cond is dWd[:, dim:dim+H]
+//   run_wgrad           [G_spec | G_cond] = d^T [x_t | cond] (hi planes) with db_d = sum_f d; G_cond is dWd[:, dim:dim+H]
 //   k_fftt_colsum/usum  u_b = sum_t d[b, t] (fixed order)
 //   k_fftt_dwd          dWd[:, :dim] = G_spec W_in^T + db_d b_in^T, dWd[:, dim+H:] = sum_b u_b temb_b^T
 //   k_fftt_dwin         dW_in = Wd[:, :dim]^T G_spec, db_in = Wd[:, :dim]^T db_d (the fold's transpose)
@@ -42,11 +42,6 @@ namespace {
 
 constexpr int kMel = 80;
 constexpr int kSumRows = 128;   // frames per partial of k_fftt_colsum
-
-// a backward over another (B, T) than its tape's: S = NaN makes every gradient NaN (the stack does the same for its own)
-__global__ void k_fftt_check(const Fs2TapeHdr* h, int B, int T, float* scal) {
-  if (h->B != B || h->T != T) scal[0] = scal[1] = __int_as_float(0x7fc00000);
-}
 
 // o[i] = fp16(x[i] * S), S = scal[0] (scal null: 1)
 __global__ void k_fftt_half(const float* __restrict__ x, size_t n, const float* scal, __half* __restrict__ o) {
@@ -89,43 +84,6 @@ __global__ void __launch_bounds__(128 * (NT > 128 ? 2 : 1)) k_fftt_gemm(const Co
     const int col = c0 + acc_col(wtid, e), m = m0 + r0 + 8 * ((e >> 1) & 1);
     if (col >= n || m >= T) continue;
     *reinterpret_cast<float2*>(out + (static_cast<size_t>(b) * T + m) * n + col) = make_float2(acc[e] * is, acc[e + 1] * is);
-  }
-}
-
-// The fixed-order reduction of k_wgrad's partials over one or two B tiles: column c of tile j of output row m goes to
-// dst_j[m * ld_j + c], times 1 / S unless raw_j; the bias sums to db (raw or not) and, unscaled, to db2 (or null).
-struct RedArgs {
-  const float* part;
-  const float* bpart;
-  int splits, Mpad, Ntot, am;
-  int bn0, bn1;                // valid columns of tile 0 and tile 1 (0: one tile)
-  float *dst0, *dst1;
-  int ld0, ld1, raw0, raw1;
-  float *db, *db2;
-  int db_raw;
-  const float* scal;
-};
-
-__global__ void k_fftt_reduce(const RedArgs p) {
-  const float is = p.scal[1];
-  const int ncol = p.bn0 + p.bn1;
-  const size_t total = static_cast<size_t>(p.am) * ncol;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int m = static_cast<int>(i / ncol), j = static_cast<int>(i % ncol), tile = j >= p.bn0;
-    const int c = tile ? j - p.bn0 : j;
-    float s = 0.f;
-    for (int z = 0; z < p.splits; ++z) s += p.part[(static_cast<size_t>(z) * p.Mpad + m) * p.Ntot + tile * 256 + c];
-    if (tile) p.dst1[static_cast<size_t>(m) * p.ld1 + c] = p.raw1 ? s : s * is;
-    else p.dst0[static_cast<size_t>(m) * p.ld0 + c] = p.raw0 ? s : s * is;
-  }
-  if (p.db) {
-    for (int m = blockIdx.x * blockDim.x + threadIdx.x; m < p.am; m += gridDim.x * blockDim.x) {
-      float s = 0.f;
-      for (int z = 0; z < p.splits; ++z) s += p.bpart[static_cast<size_t>(z) * p.Mpad + m];
-      p.db[m] = p.db_raw ? s : s * is;
-      if (p.db2) p.db2[m] = s * is;
-    }
   }
 }
 
@@ -255,16 +213,10 @@ int check_geom(const dsx_fft_train* h, int B, int T, Sizes* z) {
   z->tape = z->dec_tape + align256(4 * B * dim) + align256(36 * B * dim) + align256(6 * F * M) + align256(6 * F * H) +
             align256(2 * F * H);
   z->fwd_ws = 3 * align256(4 * F * H) + align256(F) + align256(4 * B * H) + z->dec_ws;
-  size_t part = 0;   // the larger of the two weight-gradient launches: dW_mel (M rows, 1 tile), [G_spec | G_cond]
-  const int shapes[2][2] = {{(kMel + 63) / 64, 1}, {static_cast<int>(H) / 64, 2}};
-  for (auto& sh : shapes) {
-    const int fch = wgrad_fchunk(static_cast<int>(F), sh[0] * sh[1], h->device);
-    const size_t sp = (F + fch - 1) / fch;
-    part = std::max(part, sp * sh[0] * 64 * sh[1] * 256 + sp * sh[0] * 64);
-  }
-  z->part = part;
+  // the two weight-gradient launches: dW_mel (M rows, 1 tile), [G_spec | G_cond]
+  z->part = wgrad_part_floats(static_cast<int>(F), {{(kMel + 63) / 64, 1}, {static_cast<int>(H) / 64, 2}}, h->device);
   const size_t chunks = (T + kSumRows - 1) / kSumRows;
-  z->bwd_ws = 256 + align256(2 * F * M) + 2 * align256(4 * F * H) + align256(2 * F * H) + align256(4 * part) +
+  z->bwd_ws = 256 + align256(2 * F * M) + 2 * align256(4 * F * H) + align256(2 * F * H) + align256(4 * z->part) +
               align256(4 * H * M) + align256(4 * H) + align256(4 * B * chunks * H) + align256(4 * B * H) +
               align256(4 * B * dim) + align256(16 * B * dim) + z->dec_ws;
   return DSX_OK;
@@ -485,38 +437,19 @@ int dsx_fft_train_backward(dsx_fft_train* h, const dsx_fft_params* w, const void
   void* DECWS = bp.take<uint8_t>(z.dec_ws);
   auto gp = [](const float* p) { return const_cast<float*>(p); };
 
-  // S from amax |g| of n values, NaN when the tape is of another (B, T)
-  auto scale = [&](const float* g, size_t n, unsigned* am, float* sc) -> int {
-    DSX_CUDA(cudaMemsetAsync(am, 0, sizeof(unsigned), s));
-    k_amax<<<static_cast<unsigned>(std::min<size_t>((n + 255) / 256, 1024)), 256, 0, s>>>(g, n, am);
-    DSX_TRY(launch_check("k_amax"));
-    k_scale<<<1, 1, 0, s>>>(am, sc);
-    DSX_TRY(launch_check("k_scale"));
-    k_fftt_check<<<1, 1, 0, s>>>(tp.hdr, B, T, sc);
-    return launch_check("k_fftt_check");
-  };
-  // sum_f A[f][m] B_j[f][c] over the frames for ntiles B tiles, then the reduction r
-  auto wgrad = [&](const __half* A, int lda, int am, WgradArgs t, int ntiles, RedArgs r) -> int {
+  // sum_f A[f][m] B_j[f][c] over the frames for ntiles B tiles into o, scaled by sc
+  auto wgrad = [&](const __half* A, int lda, int am, WgradArgs t, int ntiles, const WgradDst& o,
+                   const float* sc) -> int {
     t.a = A;
     t.lda = lda;
     t.am = am;
     t.F = F;
     t.T = T;
-    const int mt = (am + 63) / 64, fch = wgrad_fchunk(F, mt * ntiles, h->device), sp = (F + fch - 1) / fch;
-    float* bpart = PART + static_cast<size_t>(sp) * mt * 64 * ntiles * 256;
-    DSX_TRY(run_wgrad(t, ntiles, h->device, PART, bpart, s));
-    r.part = PART;
-    r.bpart = bpart;
-    r.splits = sp;
-    r.Mpad = mt * 64;
-    r.Ntot = ntiles * 256;
-    r.am = am;
-    k_fftt_reduce<<<blocks_for(static_cast<size_t>(am) * (r.bn0 + r.bn1)), 256, 0, s>>>(r);
-    return launch_check("k_fftt_reduce");
+    return run_wgrad(t, ntiles, o, PART, sc, h->device, s);
   };
 
-  // get_mel_out: d_out = d_eps . W_mel for the stack, dW_mel, db_mel
-  DSX_TRY(scale(d_eps, static_cast<size_t>(F) * M, amax, sc1));
+  // get_mel_out: d_out = d_eps . W_mel for the stack, dW_mel, db_mel; S1 is NaN when the tape is of another (B, T)
+  DSX_TRY(run_scale(d_eps, static_cast<size_t>(F) * M, amax, sc1, tp.hdr, B, T, s));
   k_fftt_eps16<<<dim3((T + 31) / 32, (M + 31) / 32, B), dim3(32, 8), 0, s>>>(d_eps, sc1, T, M, E16);
   DSX_TRY(launch_check("k_fftt_eps16"));
   DSX_TRY(gemm_run(h->melt, E16, B, T, sc1, DOUT, s));
@@ -525,20 +458,19 @@ int dsx_fft_train_backward(dsx_fft_train* h, const dsx_fft_params* w, const void
     t.b[0] = tp.out16;
     t.ldb[0] = H;
     t.bn[0] = H;
-    RedArgs r{};
-    r.bn0 = H;
-    r.dst0 = gp(grads->mel_out_w);
-    r.ld0 = H;
-    r.db = gp(grads->mel_out_b);
-    r.scal = sc1;
-    DSX_TRY(wgrad(E16, M, M, t, 1, r));
+    WgradDst o{};
+    o.dst[0] = gp(grads->mel_out_w);
+    o.ms[0] = H;
+    o.cs[0] = 1;
+    o.db = gp(grads->mel_out_b);
+    DSX_TRY(wgrad(E16, M, M, t, 1, o, sc1));
   }
 
   // the stack: every FFTBlocks gradient and d = d decoder_inp
   DSX_TRY(dsx_fs2dec_train_backward(h->dec, &w->dec, tp.dec, DOUT, &grads->dec, DX, B, T, DECWS, z.dec_ws, stream));
 
   // get_decode_inp and input_projection: [G_spec | G_cond] = d^T [x_t | cond] with db_d
-  DSX_TRY(scale(DX, static_cast<size_t>(F) * H, amax + 1, sc2));
+  DSX_TRY(run_scale(DX, static_cast<size_t>(F) * H, amax + 1, sc2, tp.hdr, B, T, s));
   k_fftt_half<<<blocks_for(static_cast<size_t>(F) * H), 256, 0, s>>>(DX, static_cast<size_t>(F) * H, sc2, D16);
   DSX_TRY(launch_check("k_fftt_half"));
   {
@@ -549,19 +481,18 @@ int dsx_fft_train_backward(dsx_fft_train* h, const dsx_fft_params* w, const void
     t.b[1] = tp.xc;
     t.ldb[1] = kSplit * H;
     t.bn[1] = H;
-    RedArgs r{};
-    r.bn0 = M;
-    r.dst0 = GS;
-    r.ld0 = M;
-    r.raw0 = 1;
-    r.bn1 = H;
-    r.dst1 = gp(grads->decode_inp_w) + dim;
-    r.ld1 = ldw;
-    r.db = DBD;
-    r.db_raw = 1;
-    r.db2 = gp(grads->decode_inp_b);
-    r.scal = sc2;
-    DSX_TRY(wgrad(D16, H, H, t, 2, r));
+    WgradDst o{};   // G_spec and db_d unscaled (k_fftt_dwd and k_fftt_dwin scale them), G_cond and db scaled
+    o.dst[0] = GS;
+    o.ms[0] = M;
+    o.cs[0] = 1;
+    o.raw[0] = 1;
+    o.dst[1] = gp(grads->decode_inp_w) + dim;
+    o.ms[1] = ldw;
+    o.cs[1] = 1;
+    o.db = DBD;
+    o.db_raw = 1;
+    o.db2 = gp(grads->decode_inp_b);
+    DSX_TRY(wgrad(D16, H, H, t, 2, o, sc2));
   }
   // the step part: u_b = sum_t d[b, t]
   k_fftt_colsum<<<dim3(chunks, B), H, 0, s>>>(DX, T, H, UPART);

@@ -21,7 +21,8 @@
 //   k_f2b_ln           G += LN1 backward(gA), * !pad; the operand of the layer below (dropout 3 + 3 (i - 1)), or at
 //                      layer 0 the entry: d_x = G * dropout(0) and d alpha = sum d_x . table[pos]
 // The attention backward runs on wgmma (P and dS go through shared memory as fp16 tiles); nothing of size T^2 reaches
-// global memory.  Weight gradients use k_wgrad (dsx_wgrad.cuh): frames split over CTAs, partials summed in a fixed order.
+// global memory.  Weight gradients use run_wgrad (dsx_wgrad.cuh): k_wgrad splits the frames over CTAs, k_wgrad_sum sums
+// the partials in a fixed order.
 // LayerNorm affine gradients and d alpha are per-CTA partials of k_f2b_ln (a fixed grid) summed in order.  No atomics
 // touch a result, so two backwards of one tape are bitwise equal.
 //
@@ -48,27 +49,6 @@ constexpr float kLnEps = 1e-5f;
 enum { B_GC, B_F32, B_F16 };
 
 using TapeHdr = Fs2TapeHdr;
-
-__global__ void k_tape_hdr(TapeHdr* h, uint64_t seed, float p, int B, int T) {
-  h->seed = seed;
-  h->p = p;
-  h->B = B;
-  h->T = T;
-}
-
-// a backward over another (B, T) than its tape's would read the wrong regions: S = NaN then makes every gradient NaN
-__global__ void k_tape_check(const TapeHdr* h, int B, int T, float* scal) {
-  if (h->B != B || h->T != T) scal[0] = scal[1] = __int_as_float(0x7fc00000);
-}
-
-__device__ __forceinline__ Fs2Drop hdr_drop(const TapeHdr* h, int site) {
-  Fs2Drop d;
-  d.seed = h->seed;
-  d.p = h->p;
-  d.inv_keep = 1.f / (1.f - d.p);
-  d.site = site;
-  return d;
-}
 
 struct BwdGemmArgs {
   ConvGemm g;
@@ -138,12 +118,6 @@ struct LnArgs {
   const float* scal;           // S, 1 / S
   int F, H;
 };
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 __global__ void __launch_bounds__(256) k_f2b_ln(const LnArgs p) {
   __shared__ float red[8][2 * 256 + 1];
@@ -233,37 +207,6 @@ __global__ void k_f2b_ln_reduce(const float* part, int blocks, int H, const floa
   if (t < H) dgamma[t] = s;
   else if (t < 2 * H) dbeta[t - H] = s;
   else if (dalpha) dalpha[0] = s;
-}
-
-// ---- weight-gradient reduction: dst[m * ms + c * cs + (j0 + jj) * js] = (sum of the partials in split order) / S for
-// output row m < am, B tile jj < ntl, its column c < bn; bias db[m] likewise from the column-sum partials -----------------
-struct RedArgs {
-  const float* part;
-  const float* bpart;
-  int splits, Mpad, Ntot, am, ntl, bn;
-  float* dst;
-  int ms, cs, js, j0;
-  float* db;
-  const float* scal;
-};
-
-__global__ void k_f2b_wreduce(const RedArgs p) {
-  const float is = p.scal[1];
-  const size_t per_m = static_cast<size_t>(p.ntl) * p.bn, total = static_cast<size_t>(p.am) * per_m;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int m = static_cast<int>(i / per_m), rem = static_cast<int>(i % per_m), jj = rem / p.bn, c = rem % p.bn;
-    float s = 0.f;
-    for (int z = 0; z < p.splits; ++z) s += p.part[(static_cast<size_t>(z) * p.Mpad + m) * p.Ntot + jj * 256 + c];
-    p.dst[static_cast<size_t>(m) * p.ms + static_cast<size_t>(c) * p.cs + static_cast<size_t>(p.j0 + jj) * p.js] = s * is;
-  }
-  if (p.db) {
-    for (int m = blockIdx.x * blockDim.x + threadIdx.x; m < p.am; m += gridDim.x * blockDim.x) {
-      float s = 0.f;
-      for (int z = 0; z < p.splits; ++z) s += p.bpart[static_cast<size_t>(z) * p.Mpad + m];
-      p.db[m] = s * is;
-    }
-  }
 }
 
 // ---- attention backward -----------------------------------------------------------------------------------------------
@@ -530,13 +473,6 @@ __global__ void __launch_bounds__(128) k_attn_bwd_q(const AttnBwdArgs p) {
   }
 }
 
-// ---- masks for tests ----------------------------------------------------------------------------------------------------
-__global__ void k_f2_masks(Fs2Drop d, size_t F, int n, uint8_t* out) {
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < F * n;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x)
-    out[i] = dropout_scale(d, i / n, static_cast<int>(i % n)) != 0.f;
-}
-
 // ---- tape -------------------------------------------------------------------------------------------------------------
 using Tape = Fs2TrainTape;
 
@@ -615,28 +551,21 @@ int run_bwd_gemm(BwdGemmArgs a, const ConvGemm& g, int B, int T, cudaStream_t s)
 
 int tap0_of(const dsx_fs2dec_config& c) { return c.padding ? -(c.kernel - 1) : -(c.kernel / 2); }
 
-// (m tiles, n tiles) of the backward's weight-gradient GEMMs: ffn_2, ffn_1 (4 taps a launch), out_proj, in_proj
-size_t wgrad_part_floats(const dsx_fs2dec_config& c, int F, int device) {
-  const int H = c.hidden;
-  const int shapes[][2] = {{H / 64, 4 * H / 256}, {4 * H / 64, std::min(c.kernel, 4)}, {H / 64, 1}, {3 * H / 64, 1}};
-  size_t worst = 0;
-  for (auto& sh : shapes) {
-    const int fchunk = wgrad_fchunk(F, sh[0] * sh[1], device);
-    const size_t sp = (F + fchunk - 1) / fchunk;
-    worst = std::max(worst, sp * sh[0] * 64 * sh[1] * 256 + sp * sh[0] * 64);
-  }
-  return worst;
-}
-
 // the backward's workspace: scalars, G, gA (fp32 [F][H]), gY (fp16 [F][H]), gC (fp16 [F][4H]), dO (fp16 [F][H]),
 // d in_proj output (fp16 [F][3H]), D of the attention, LayerNorm partials, weight-gradient partials
 constexpr int kBwdRegions = 10;
 void bwd_sizes(const dsx_fs2dec_config& c, int B, int T, int device, size_t (&sz)[kBwdRegions]) {
   const size_t F = static_cast<size_t>(B) * T, H = c.hidden;
+  // (m tiles, n tiles) of the weight-gradient GEMMs: ffn_2, ffn_1 (4 taps a launch), out_proj, in_proj
+  const int h = c.hidden;
+  const size_t part = wgrad_part_floats(static_cast<int>(F),
+                                        {{h / 64, 4 * h / 256}, {4 * h / 64, std::min(c.kernel, 4)}, {h / 64, 1},
+                                         {3 * h / 64, 1}},
+                                        device);
   const size_t v[kBwdRegions] = {256,       F * H * 4, F * H * 4,
                                  F * H * 2, F * 4 * H * 2, F * H * 2,
                                  F * 3 * H * 2, F * c.heads * 4, static_cast<size_t>(kLnBlocks) * (2 * H + 1) * 4,
-                                 wgrad_part_floats(c, static_cast<int>(F), device) * 4};
+                                 part * 4};
   for (int i = 0; i < kBwdRegions; ++i) sz[i] = v[i];
 }
 
@@ -732,14 +661,7 @@ int fs2t_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* t
   float* PART = bump.take<float>(sizes[9]);
   auto gp = [](const float* p) { return const_cast<float*>(p); };
 
-  DSX_CUDA(cudaMemsetAsync(amax, 0, sizeof(unsigned), s));
-  const size_t ne = static_cast<size_t>(F) * H;
-  k_amax<<<static_cast<unsigned>(std::min<size_t>((ne + 255) / 256, 1024)), 256, 0, s>>>(d_out, ne, amax);
-  DSX_TRY(launch_check("k_amax"));
-  k_scale<<<1, 1, 0, s>>>(amax, scal);
-  DSX_TRY(launch_check("k_scale"));
-  k_tape_check<<<1, 1, 0, s>>>(tp.hdr, B, T, scal);
-  DSX_TRY(launch_check("k_tape_check"));
+  DSX_TRY(run_scale(d_out, static_cast<size_t>(F) * H, amax, scal, tp.hdr, B, T, s));
 
   // LayerNorm backward into G, then its affine gradients
   auto ln = [&](const float* gin, int from_dout, const float* x, const float* gamma, int accumulate, __half* o16,
@@ -768,36 +690,25 @@ int fs2t_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* t
     k_f2b_ln_reduce<<<(2 * H + 1 + 255) / 256, 256, 0, s>>>(LNP, kLnBlocks, H, scal, dgamma, dbeta, dalpha);
     return launch_check("k_f2b_ln_reduce");
   };
-  // weight gradient sum_f A[f][m] B_jj[f + shift_jj][c] of ntiles B tiles, then its reduction (see RedArgs)
-  auto wgrad = [&](const __half* A, int lda, int am, WgradArgs t, int ntiles, RedArgs r) -> int {
+  // weight gradient sum_f A[f][m] B_jj[f + shift_jj][c] of ntiles B tiles into o
+  auto wgrad = [&](const __half* A, int lda, int am, WgradArgs t, int ntiles, const WgradDst& o) -> int {
     t.a = A;
     t.lda = lda;
     t.am = am;
     t.F = F;
     t.T = T;
-    const int mt = (am + 63) / 64, fch = wgrad_fchunk(F, mt * ntiles, h->device), sp = (F + fch - 1) / fch;
-    float* bp = PART + static_cast<size_t>(sp) * mt * 64 * ntiles * 256;   // the bias partials follow the weights'
-    DSX_TRY(run_wgrad(t, ntiles, h->device, PART, r.db ? bp : nullptr, s));
-    r.part = PART;
-    r.bpart = bp;
-    r.splits = sp;
-    r.Mpad = mt * 64;
-    r.Ntot = ntiles * 256;
-    r.am = am;
-    r.ntl = ntiles;
-    r.scal = scal;
-    const size_t total = static_cast<size_t>(am) * ntiles * r.bn;
-    k_f2b_wreduce<<<static_cast<unsigned>(std::min<size_t>((total + 255) / 256, 4096)), 256, 0, s>>>(r);
-    return launch_check("k_f2b_wreduce");
+    return run_wgrad(t, ntiles, o, PART, scal, h->device, s);
   };
-  auto rows = [](float* dst, int ms, int bn, float* db) {   // dst[m][c], row length ms
-    RedArgs r{};
-    r.dst = dst;
-    r.ms = ms;
-    r.cs = 1;
-    r.bn = bn;
-    r.db = db;
-    return r;
+  // tile jj to dst[m * ms + c * cs + jj * js]
+  auto rows = [](float* dst, int ms, int cs, int js, float* db) {
+    WgradDst o{};
+    for (int jj = 0; jj < 4; ++jj) {
+      o.dst[jj] = dst + jj * js;
+      o.ms[jj] = ms;
+      o.cs[jj] = cs;
+    }
+    o.db = db;
+    return o;
   };
   auto single = [](const __half* b, int ldb, int bn) {
     WgradArgs t{};
@@ -831,9 +742,7 @@ int fs2t_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* t
         t.ldb[j] = 4 * H;
         t.bn[j] = 256;
       }
-      RedArgs r = rows(gp(grads->ffn2_w[i]), 4 * H, 256, gp(grads->ffn2_b[i]));
-      r.js = 256;
-      DSX_TRY(wgrad(GY, H, H, t, nt, r));
+      DSX_TRY(wgrad(GY, H, H, t, nt, rows(gp(grads->ffn2_w[i]), 4 * H, 1, 256, gp(grads->ffn2_b[i]))));
     }
     a = BwdGemmArgs{};
     a.mode = B_F32;
@@ -849,11 +758,8 @@ int fs2t_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* t
         t.bn[jj] = H;
         t.shift[jj] = tap0_of(c) + j0 + jj;
       }
-      RedArgs r = rows(gp(grads->ffn1_w[i]), H * k, H, j0 == 0 ? gp(grads->ffn1_b[i]) : nullptr);
-      r.cs = k;
-      r.js = 1;
-      r.j0 = j0;
-      DSX_TRY(wgrad(GC, 4 * H, 4 * H, t, nt, r));
+      DSX_TRY(wgrad(GC, 4 * H, 4 * H, t, nt,
+                    rows(gp(grads->ffn1_w[i]) + j0, H * k, k, 1, j0 == 0 ? gp(grads->ffn1_b[i]) : nullptr)));
     }
     DSX_TRY(ln(GA, 0, tr.xin[2 * i + 1], w->ln2_w[i], 1, GY, 1 + 3 * i, 0, gp(grads->ln2_w[i]), gp(grads->ln2_b[i]),
                nullptr));
@@ -863,7 +769,7 @@ int fs2t_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* t
     a.x = GY;
     a.o16 = GO;
     DSX_TRY(run_bwd_gemm(a, pk.out_t, B, T, s));
-    DSX_TRY(wgrad(GY, H, H, single(tr.o[i], H, H), 1, rows(gp(grads->out_proj_w[i]), H, H, nullptr)));
+    DSX_TRY(wgrad(GY, H, H, single(tr.o[i], H, H), 1, rows(gp(grads->out_proj_w[i]), H, 1, 0, nullptr)));
     k_attn_delta<<<(F * heads + 255) / 256, 256, 0, s>>>(GO, tr.o[i], F, T, heads, D, DELTA);
     DSX_TRY(launch_check("k_attn_delta"));
     AttnBwdArgs ab{};
@@ -894,7 +800,7 @@ int fs2t_backward(dsx_fs2dec_train* h, const dsx_fs2dec_params* w, const void* t
     a.x = GQKV;
     a.o32 = GA;
     DSX_TRY(run_bwd_gemm(a, pk.in_t, B, T, s));
-    DSX_TRY(wgrad(GQKV, 3 * H, 3 * H, single(tr.a1[i], H, H), 1, rows(gp(grads->in_proj_w[i]), H, H, nullptr)));
+    DSX_TRY(wgrad(GQKV, 3 * H, 3 * H, single(tr.a1[i], H, H), 1, rows(gp(grads->in_proj_w[i]), H, 1, 0, nullptr)));
     // LN1, then the operand of the layer below, or the entry: x + alpha * table[pos] -> dropout -> * !pad
     DSX_TRY(ln(GA, 0, tr.xin[2 * i], w->ln1_w[i], 1, i > 0 ? GY : nullptr, i > 0 ? 3 * i : 0, i == 0,
                gp(grads->ln1_w[i]), gp(grads->ln1_b[i]), i == 0 ? d_alpha : nullptr));
@@ -1012,16 +918,13 @@ int dsx_fs2dec_train_masks(dsx_fs2dec_train* h, uint64_t seed, float p_drop, int
   DSX_CHECK(p_drop >= 0.f && p_drop < 1.f, DSX_E_INVALID, "dropout p = %g is outside [0, 1)", static_cast<double>(p_drop));
   DSX_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  Fs2Train tr;
-  tr.seed = seed;
-  tr.p = p_drop;
   const size_t F = static_cast<size_t>(B) * T;
   for (int site = 0; site < 1 + 3 * h->cfg.layers; ++site) {
     DSX_CHECK(out[site], DSX_E_INVALID, "mask %d is NULL", site);
     const int n = (site > 0 && site % 3 == 2) ? 4 * h->cfg.hidden : h->cfg.hidden;
-    k_f2_masks<<<static_cast<unsigned>(std::min<size_t>((F * n + 255) / 256, 4096)), 256, 0, s>>>(tr.drop(site), F, n,
-                                                                                                    out[site]);
-    DSX_TRY(launch_check("k_f2_masks"));
+    k_drop_masks<<<static_cast<unsigned>(std::min<size_t>((F * n + 255) / 256, 4096)), 256, 0, s>>>(
+        make_drop(seed, p_drop, site), F, n, out[site]);
+    DSX_TRY(launch_check("k_drop_masks"));
   }
   return DSX_OK;
 }

@@ -370,14 +370,7 @@ struct Fs2Train {
                                                     // [B][heads][T][D]; attention output [F][H]; ffn_1 output * k^-0.5
                                                     // before the activation and the ffn_2 input after dropout [F][4H]
   std::vector<float*> lse;                          // per layer: softmax log-sum-exp [B][heads][T] (+inf: no key)
-  Fs2Drop drop(int site) const {
-    Fs2Drop d;
-    d.seed = seed;
-    d.p = p;
-    d.inv_keep = 1.f / (1.f - p);
-    d.site = site;
-    return d;
-  }
+  Fs2Drop drop(int site) const { return make_drop(seed, p, site); }
 };
 // the first region of a dsx_fs2dec_train tape: the forward's dropout, so that the backward draws the same masks from the
 // tape alone, and its (B, T), which the backward checks on the device
@@ -450,14 +443,7 @@ struct DurTrain {
   std::vector<__half*> a;
   std::vector<float*> r;
   float* hin = nullptr;
-  Fs2Drop drop(int site) const {
-    Fs2Drop d;
-    d.seed = seed;
-    d.p = p;
-    d.inv_keep = 1.f / (1.f - p);
-    d.site = site;
-    return d;
-  }
+  Fs2Drop drop(int site) const { return make_drop(seed, p, site); }
 };
 // The training step's forward packs live in a dsx_durpred handle: durpred_train_alloc sizes them once (the handle then
 // counts as loaded), durpred_train_pack refills them from the caller's fp32 weights on the stream (no allocation, no

@@ -6,7 +6,7 @@
 // duration predictor's (a dsx_durpred for eval, a dsx_durpred_train for training) and add only those:
 //   forward   k_pos_scan and k_pos_add (dsx_posemb.cuh): x + alpha table[pos] -> layer 0's fp16 operand; dp_stack_run
 //             without a mask: each layer's k_pe_conv, the last one writing its output (after dropout) in fp32; k_ppt_head:
-//             Linear(P, odim), one warp per frame.  Training adds k_ppt_hdr (the tape's header) and the duration
+//             Linear(P, odim), one warp per frame.  Training adds k_tape_hdr (the tape's header) and the duration
 //             predictor's conv weight pack (without its head), and saves the positions, the layers' inputs and the head's input to the tape.
 //   backward  dpt_backward with no mask and odim outputs (the head's backward, then per layer wgrad and the transposed
 //             conv with the layer below's backward in its epilogue), always down to d_in, the gradient at layer 0's
@@ -21,19 +21,13 @@
 #include "dsx_conv.cuh"
 #include "dsx_internal.h"
 #include "dsx_posemb.cuh"
+#include "dsx_wgrad.cuh"
 
 namespace dsx {
 namespace {
 
 constexpr int kPpMaxOdim = 16;
 constexpr int kAlphaBlocks = 256;   // CTAs of k_ppt_alpha_part: fixed, so the partial sums have a fixed order
-
-__global__ void k_ppt_hdr(Fs2TapeHdr* h, uint64_t seed, float p, int B, int T) {
-  h->seed = seed;
-  h->p = p;
-  h->B = B;
-  h->T = T;
-}
 
 // out[f][o] = b[o] + sum_c hin[f][c] W[o][c] (tts_modules.py:234), one warp per frame, P <= 256
 __global__ void __launch_bounds__(256) k_ppt_head(const float* hin, const float* W, const float* b, int F, int P, int od,
@@ -316,8 +310,8 @@ int dsx_pitchpred_train_forward(dsx_pitchpred_train* h, const dsx_pitchpred_para
   pp_tape_carve(c, B, T, static_cast<uint8_t*>(tape), &tp);
   tp.d.tr.seed = seed;
   tp.d.tr.p = p_drop;
-  k_ppt_hdr<<<1, 1, 0, s>>>(tp.d.hdr, seed, p_drop, B, T);
-  DSX_TRY(launch_check("k_ppt_hdr"));
+  k_tape_hdr<<<1, 1, 0, s>>>(tp.d.hdr, seed, p_drop, B, T);
+  DSX_TRY(launch_check("k_tape_hdr"));
   dsx_durpred* fwd = dpt_forward_handle(h->dp);
   const dsx_durpred_params dpp = dp_params(*w);
   DSX_TRY(durpred_train_pack(fwd, &dpp, s, false));

@@ -68,6 +68,14 @@ struct Fs2Drop {
   float p = 0.f, inv_keep = 1.f;
   int site = -1;                 // < 0: no dropout (scale 1)
 };
+__host__ __device__ __forceinline__ Fs2Drop make_drop(uint64_t seed, float p, int site) {
+  Fs2Drop d;
+  d.seed = seed;
+  d.p = p;
+  d.inv_keep = 1.f / (1.f - p);
+  d.site = site;
+  return d;
+}
 __device__ __forceinline__ uint4 dropout_block(const Fs2Drop& d, size_t frame, int channel) {
   const uint4 ctr = make_uint4(static_cast<uint32_t>(channel >> 2), static_cast<uint32_t>(frame),
                                static_cast<uint32_t>(d.site), static_cast<uint32_t>(frame >> 32));

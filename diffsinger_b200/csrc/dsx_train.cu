@@ -16,7 +16,7 @@
 //           dx_l = dx_{l+1} / sqrt(2) + dy_l and the per-tile column sums of dy_l (the gradient of d_l(t))
 //   B_COND  d_cond = sum_l W_cond,l^T dpre_l as one GEMM with K = L * 2C: tap l reads layer l's dpre
 // Weight gradients reduce over the frame axis, so both operands are frames-major and enter wgmma MN-major
-// (k_wgrad): the frames split over CTAs, each writes an fp32 partial, and k_wgrad_reduce sums the partials in a fixed
+// (k_wgrad): the frames split over CTAs, each writes an fp32 partial, and k_wgrad_sum sums the partials in a fixed
 // order (no atomics: gradients are bitwise reproducible).  Bias gradients are the column sums of the same A tiles.  The
 // dilated conv and the conditioner projection share one wgrad launch whose B operand is [y(-d) | y | y(+d) | cond].  The
 // step-embedding MLP and diffusion_projection (B rows) are on CUDA cores.
@@ -245,47 +245,6 @@ __global__ void __launch_bounds__(256) k_train_gemm(const GemmArgs p) {
   }
 }
 
-// dst = (sum of the partials in split order) / S.  mode 0: dst[m * ldd + n] for n < nvalid; mode 1: the dilated conv
-// and the conditioner projection, columns [tap 0 | tap 1 | tap 2 | cond] -> dil_w [m][c][tap], cond_w [m][h]
-struct ReduceArgs {
-  const float* part;
-  const float* bpart;
-  int splits, Mpad, Ntot, am, nvalid, ldd, mode;
-  float* dst;
-  float* dst2;                 // mode 1: cond_w
-  float* db;                   // bias gradient [am], or null
-  float* db2;                  // a second copy of it (mode 1: cond_b), or null
-  const float* inv_s;
-};
-
-__global__ void k_wgrad_reduce(const ReduceArgs p) {
-  const float is = *p.inv_s;
-  const size_t total = static_cast<size_t>(p.am) * p.nvalid;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int m = static_cast<int>(i / p.nvalid), n = static_cast<int>(i % p.nvalid);
-    float s = 0.f;
-    for (int z = 0; z < p.splits; ++z) s += p.part[(static_cast<size_t>(z) * p.Mpad + m) * p.Ntot + n];
-    s *= is;
-    if (p.mode == 0) {
-      p.dst[static_cast<size_t>(m) * p.ldd + n] = s;
-    } else if (n < 3 * kC) {
-      p.dst[(static_cast<size_t>(m) * kC + n % kC) * 3 + n / kC] = s;
-    } else {
-      p.dst2[static_cast<size_t>(m) * kH + n - 3 * kC] = s;
-    }
-  }
-  if (p.db) {
-    for (int m = blockIdx.x * blockDim.x + threadIdx.x; m < p.am; m += gridDim.x * blockDim.x) {
-      float s = 0.f;
-      for (int z = 0; z < p.splits; ++z) s += p.bpart[static_cast<size_t>(z) * p.Mpad + m];
-      s *= is;
-      p.db[m] = s;
-      if (p.db2) p.db2[m] = s;
-    }
-  }
-}
-
 // ---- packing --------------------------------------------------------------------------------------------------------
 // the dilated conv (k = 3) or the conditioner projection (k = 1) with gate / filter columns interleaved by 8 (see
 // F_GATE); bias (b1 + b2, either may be null) -> g.b
@@ -468,26 +427,9 @@ int run_gemm(const GemmArgs& a, int B, int T, cudaStream_t s) {
   return launch_check("k_train_gemm");
 }
 
-int run_reduce(ReduceArgs r, cudaStream_t s) {
-  const size_t total = static_cast<size_t>(r.am) * r.nvalid;
-  k_wgrad_reduce<<<static_cast<unsigned>(std::min<size_t>((total + 255) / 256, 4096)), 256, 0, s>>>(r);
-  return launch_check("k_wgrad_reduce");
-}
-
-// the largest partial buffer (floats) a wgrad of this call needs
-size_t wgrad_part_floats(int F, int device) {
-  size_t worst = 0;
-  const int shapes[][2] = {{8, 4}, {8, 1}, {4, 1}, {2, 1}};   // (m tiles, n tiles) of the backward's wgrads
-  for (auto& sh : shapes) {
-    const int fchunk = wgrad_fchunk(F, sh[0] * sh[1], device);
-    const int sp = (F + fchunk - 1) / fchunk;
-    worst = std::max(worst, static_cast<size_t>(sp) * sh[0] * 64 * sh[1] * 256 + static_cast<size_t>(sp) * sh[0] * 64);
-  }
-  return worst;
-}
-
 // the backward's workspace regions: scalars, d eps (fp16), dh1, [d res | d skip] (fp16), dx (fp32), d of
-// input_projection, dpre of every layer, tile column sums, dE per layer, dh of the MLP, wgrad partials, dE summed
+// input_projection, dpre of every layer, tile column sums, dE per layer, dh of the MLP, wgrad partials (for the
+// (m tiles, n tiles) of the backward's wgrads), dE summed
 constexpr int kBwdRegions = 12;
 void bwd_sizes(int L, int B, int T, int device, size_t (&sz)[kBwdRegions]) {
   const size_t F = static_cast<size_t>(B) * T;
@@ -502,7 +444,7 @@ void bwd_sizes(int L, int B, int T, int device, size_t (&sz)[kBwdRegions]) {
                                  static_cast<size_t>(L) * B * mtiles * kC * 4,
                                  static_cast<size_t>(L) * B * kC * 4,
                                  static_cast<size_t>(B) * 4 * kC * 4,
-                                 wgrad_part_floats(static_cast<int>(F), device) * 4,
+                                 wgrad_part_floats(static_cast<int>(F), {{8, 4}, {8, 1}, {4, 1}, {2, 1}}, device) * 4,
                                  static_cast<size_t>(B) * kC * 4};
   for (int i = 0; i < kBwdRegions; ++i) sz[i] = v[i];
 }
@@ -777,45 +719,29 @@ int dsx_train_backward(dsx_train* h, const dsx_diffnet_params* w, const void* ta
   float* PART = bump.take<float>(sizes[10]);
   float* DESUM = bump.take<float>(sizes[11]);
 
-  DSX_CUDA(cudaMemsetAsync(amax, 0, sizeof(unsigned), s));
   DSX_CUDA(cudaMemsetAsync(GO, 0, F * kN1 * 2, s));   // d res of the last layer is 0
   const size_t ne = F * kM;
-  k_amax<<<static_cast<unsigned>(std::min<size_t>((ne + 255) / 256, 1024)), 256, 0, s>>>(d_eps, ne, amax);
-  DSX_TRY(launch_check("k_amax"));
-  k_scale<<<1, 1, 0, s>>>(amax, scal);
-  DSX_TRY(launch_check("k_scale"));
+  DSX_TRY(run_scale(d_eps, ne, amax, scal, nullptr, B, T, s));
   k_grad_in<<<static_cast<unsigned>(std::min<size_t>((ne + 255) / 256, 4096)), 256, 0, s>>>(d_eps, scal, B, T, G0);
   DSX_TRY(launch_check("k_grad_in"));
   const float* inv_s = scal + 1;
 
-  // wgrad of one GEMM, then its reduction into grads
-  auto wgrad = [&](const __half* A, int lda, int am, int ntiles, const WgradArgs& tmpl, ReduceArgs r) -> int {
-    WgradArgs wa = tmpl;
-    wa.a = A;
-    wa.lda = lda;
-    wa.am = am;
-    wa.F = static_cast<int>(F);
-    wa.T = T;
-    const int mt = (am + 63) / 64;
-    const int sp = (wa.F + wgrad_fchunk(wa.F, mt * ntiles, h->device) - 1) / wgrad_fchunk(wa.F, mt * ntiles, h->device);
-    float* bp = PART + static_cast<size_t>(sp) * mt * 64 * ntiles * 256;   // the bias partials follow the weights'
-    DSX_TRY(run_wgrad(wa, ntiles, h->device, PART, r.db ? bp : nullptr, s));
-    r.part = PART;
-    r.bpart = bp;
-    r.splits = sp;
-    r.Mpad = mt * 64;
-    r.Ntot = ntiles * 256;
-    r.am = am;
-    r.inv_s = inv_s;
-    return run_reduce(r, s);
+  // wgrad of one GEMM into grads
+  auto wgrad = [&](const __half* A, int lda, int am, int ntiles, WgradArgs t, const WgradDst& o) -> int {
+    t.a = A;
+    t.lda = lda;
+    t.am = am;
+    t.F = static_cast<int>(F);
+    t.T = T;
+    return run_wgrad(t, ntiles, o, PART, scal, h->device, s);
   };
-  auto plain = [](int nvalid, int ldd, float* dst, float* db) {
-    ReduceArgs r{};
-    r.nvalid = nvalid;
-    r.ldd = ldd;
-    r.dst = dst;
-    r.db = db;
-    return r;
+  auto plain = [](int ldd, float* dst, float* db) {   // dst[m * ldd + c]
+    WgradDst o{};
+    o.dst[0] = dst;
+    o.ms[0] = ldd;
+    o.cs[0] = 1;
+    o.db = db;
+    return o;
   };
   auto single = [](const __half* b, int ldb, int bn) {
     WgradArgs t{};
@@ -838,15 +764,15 @@ int dsx_train_backward(dsx_train* h, const dsx_diffnet_params* w, const void* ta
   a.aux = tp.h1;
   a.o16 = DH;
   DSX_TRY(run_gemm(a, B, T, s));
-  DSX_TRY(wgrad(G0, kM, kM, 1, single(tp.h1, kC, kC), plain(kC, kC, const_cast<float*>(grads->fin_w),
-                                                               const_cast<float*>(grads->fin_b))));
+  DSX_TRY(wgrad(G0, kM, kM, 1, single(tp.h1, kC, kC),
+                plain(kC, const_cast<float*>(grads->fin_w), const_cast<float*>(grads->fin_b))));
   a.mode = B_SKIP;
   a.g = h->skip_t;
   a.x = DH;
   a.o16 = GO;
   DSX_TRY(run_gemm(a, B, T, s));
-  DSX_TRY(wgrad(DH, kC, kC, 1, single(tp.s16, kC, kC), plain(kC, kC, const_cast<float*>(grads->skip_w),
-                                                              const_cast<float*>(grads->skip_b))));
+  DSX_TRY(wgrad(DH, kC, kC, 1, single(tp.s16, kC, kC),
+                plain(kC, const_cast<float*>(grads->skip_w), const_cast<float*>(grads->skip_b))));
   for (int l = L - 1; l >= 0; --l) {
     const int d = 1 << (l % h->cycle);
     __half* dpre = DPRE + static_cast<size_t>(l) * F * kN1;
@@ -858,7 +784,7 @@ int dsx_train_backward(dsx_train* h, const dsx_diffnet_params* w, const void* ta
     a.o16 = dpre;
     DSX_TRY(run_gemm(a, B, T, s));
     DSX_TRY(wgrad(GO, kN1, kN1, 1, single(tp.z[l], kC, kC),
-                  plain(kC, kC, const_cast<float*>(grads->out_w[l]), const_cast<float*>(grads->out_b[l]))));
+                  plain(kC, const_cast<float*>(grads->out_w[l]), const_cast<float*>(grads->out_b[l]))));
     a.mode = B_DIL;
     a.g = h->dil_t[l];
     a.x = dpre;
@@ -868,21 +794,21 @@ int dsx_train_backward(dsx_train* h, const dsx_diffnet_params* w, const void* ta
     a.o16b = DIN;
     a.o32 = DDP + static_cast<size_t>(l) * B * mtiles * kC;
     DSX_TRY(run_gemm(a, B, T, s));
+    // columns [tap 0 | tap 1 | tap 2 | cond] -> dil_w [m][c][tap], cond_w [m][h]
     WgradArgs t4{};
+    WgradDst o{};
     for (int j = 0; j < 4; ++j) {
       t4.b[j] = j < 3 ? tp.y[l] : tp.cond;
       t4.ldb[j] = kC;
       t4.bn[j] = kC;
       t4.shift[j] = j < 3 ? (j - 1) * d : 0;
+      o.dst[j] = j < 3 ? const_cast<float*>(grads->dil_w[l]) + j : const_cast<float*>(grads->cond_w[l]);
+      o.ms[j] = j < 3 ? 3 * kC : kH;
+      o.cs[j] = j < 3 ? 3 : 1;
     }
-    ReduceArgs r{};
-    r.mode = 1;
-    r.nvalid = 4 * kC;
-    r.dst = const_cast<float*>(grads->dil_w[l]);
-    r.dst2 = const_cast<float*>(grads->cond_w[l]);
-    r.db = const_cast<float*>(grads->dil_b[l]);
-    r.db2 = const_cast<float*>(grads->cond_b[l]);
-    DSX_TRY(wgrad(dpre, kN1, kN1, 4, t4, r));
+    o.db = const_cast<float*>(grads->dil_b[l]);
+    o.db2 = const_cast<float*>(grads->cond_b[l]);
+    DSX_TRY(wgrad(dpre, kN1, kN1, 4, t4, o));
     k_dif_grad<<<kC + B, kC, 0, s>>>(DDP + static_cast<size_t>(l) * B * mtiles * kC, mtiles, B, tp.emb, w->dif_w[l], scal,
                                      const_cast<float*>(grads->dif_w[l]), const_cast<float*>(grads->dif_b[l]),
                                      DE + static_cast<size_t>(l) * B * kC);
@@ -890,7 +816,7 @@ int dsx_train_backward(dsx_train* h, const dsx_diffnet_params* w, const void* ta
   }
   // input_projection (its ReLU mask is in DIN), the MLP, and d_cond
   DSX_TRY(wgrad(DIN, kC, kC, 1, single(tp.spec, kM, kM),
-                plain(kM, kM, const_cast<float*>(grads->in_w), const_cast<float*>(grads->in_b))));
+                plain(kM, const_cast<float*>(grads->in_w), const_cast<float*>(grads->in_b))));
   k_de_sum<<<(B * kC + 255) / 256, 256, 0, s>>>(DE, L, B, DESUM);
   DSX_TRY(launch_check("k_de_sum"));
   DSX_TRY(run_mlp_grad(DESUM, B, kC, tp.save, w->mlp2_w, scal, const_cast<float*>(grads->mlp2_w),

@@ -1,8 +1,11 @@
-// Training helpers shared by the DiffNet (dsx_train.cu), FastSpeech2 decoder (dsx_fs2train.cu) and FFT denoiser
-// (dsx_ffttrain.cu) training steps: the weight-gradient GEMM over the frame axis with its fixed-order split (k_wgrad), the
-// device-chosen power-of-two gradient scale (k_amax, k_scale) and the step-embedding MLP's backward (run_mlp_grad).
+// Training helpers shared by the DiffNet (dsx_train.cu), FastSpeech2 decoder (dsx_fs2train.cu), FFT denoiser
+// (dsx_ffttrain.cu), duration predictor (dsx_durtrain.cu) and pitch predictor (dsx_pitchtrain.cu) training steps: the
+// weight-gradient GEMM over the frame axis with its fixed-order split and reduction (run_wgrad: k_wgrad, k_wgrad_sum),
+// the device-chosen power-of-two gradient scale with the tape's (B, T) check (run_scale: k_amax, k_scale), the tape
+// header and dropout helpers (k_tape_hdr, hdr_drop, k_drop_masks) and the step-embedding MLP's backward (run_mlp_grad).
 #pragma once
 #include <algorithm>
+#include <vector>
 
 #include "dsx_internal.h"
 #include "dsx_ptx.cuh"
@@ -109,6 +112,48 @@ __global__ void __launch_bounds__(kWgThreads) k_wgrad(const WgradArgs p) {
   }
 }
 
+// Where the reduction of a wgrad's partials writes: column c < bn of B tile j of output row m goes to
+// dst[j][m * ms[j] + c * cs[j]], times 1 / S unless raw[j]; the bias (the column sums of A) to db, times 1 / S unless
+// db_raw, and times 1 / S to db2 (or null).  db null: no bias partials are computed.
+struct WgradDst {
+  float* dst[4];
+  int ms[4], cs[4], raw[4];
+  float *db, *db2;
+  int db_raw;
+};
+
+struct WgradSumArgs {
+  const float* part;           // k_wgrad's [splits][Mpad][Ntot]
+  const float* bpart;          // and its [splits][Mpad] bias partials
+  int splits, Mpad, Ntot, am;
+  int ncol, bn[4];             // valid columns of all B tiles, of each
+  WgradDst o;
+  const float* scal;           // S, 1 / S
+};
+
+// each output is 0 plus the partials in split order, then times 1 / S once: no atomics, bitwise reproducible.  Thread i
+// takes row m, then the tiles' columns in order, so concurrent CTAs read whole rows of the partials.
+__global__ void k_wgrad_sum(const WgradSumArgs p) {
+  const int total = p.am * p.ncol;
+  const float is = p.scal[1];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const int m = i / p.ncol;
+    int j = 0, c = i - m * p.ncol;
+    while (c >= p.bn[j]) c -= p.bn[j++];
+    float s = 0.f;
+    for (int z = 0; z < p.splits; ++z) s += p.part[(static_cast<size_t>(z) * p.Mpad + m) * p.Ntot + j * 256 + c];
+    p.o.dst[j][static_cast<size_t>(m) * p.o.ms[j] + static_cast<size_t>(c) * p.o.cs[j]] = p.o.raw[j] ? s : s * is;
+  }
+  if (p.o.db) {
+    for (int m = blockIdx.x * blockDim.x + threadIdx.x; m < p.am; m += gridDim.x * blockDim.x) {
+      float s = 0.f;
+      for (int z = 0; z < p.splits; ++z) s += p.bpart[static_cast<size_t>(z) * p.Mpad + m];
+      p.o.db[m] = p.o.db_raw ? s : s * is;
+      if (p.o.db2) p.o.db2[m] = s * is;
+    }
+  }
+}
+
 // ---- gradient scale: S from amax |g| ---------------------------------------------------------------------------------
 __global__ void k_amax(const float* g, size_t n, unsigned* amax_bits) {
   float m = 0.f;
@@ -120,8 +165,13 @@ __global__ void k_amax(const float* g, size_t n, unsigned* amax_bits) {
   if ((threadIdx.x & 31) == 0) atomicMax(amax_bits, __float_as_uint(m));   // max of non-negative floats: order-free
 }
 
-// scal[0] = S, scal[1] = 1 / S: S * amax in [2^5, 2^6); S = 1 when amax is 0 or not finite
-__global__ void k_scale(const unsigned* amax_bits, float* scal) {
+// scal[0] = S, scal[1] = 1 / S: S * amax in [2^5, 2^6); S = 1 when amax is 0 or not finite.  A backward over another
+// (B, T) than its tape's (hdr non-null) would read the wrong regions: S = 1 / S = NaN then makes every gradient NaN.
+__global__ void k_scale(const unsigned* amax_bits, float* scal, const Fs2TapeHdr* hdr, int B, int T) {
+  if (hdr && (hdr->B != B || hdr->T != T)) {
+    scal[0] = scal[1] = __int_as_float(0x7fc00000);
+    return;
+  }
   const float a = __uint_as_float(*amax_bits);
   int e = 0;
   if (a > 0.f && isfinite(a)) {
@@ -130,6 +180,40 @@ __global__ void k_scale(const unsigned* amax_bits, float* scal) {
   }
   scal[0] = ldexpf(1.f, e);
   scal[1] = ldexpf(1.f, -e);
+}
+
+// S from amax |g| over n values into scal (amax: a scratch word), checked against the tape's header hdr (or null)
+int run_scale(const float* g, size_t n, unsigned* amax, float* scal, const Fs2TapeHdr* hdr, int B, int T,
+              cudaStream_t s) {
+  DSX_CUDA(cudaMemsetAsync(amax, 0, sizeof(unsigned), s));
+  k_amax<<<static_cast<unsigned>(std::min<size_t>((n + 255) / 256, 1024)), 256, 0, s>>>(g, n, amax);
+  DSX_TRY(launch_check("k_amax"));
+  k_scale<<<1, 1, 0, s>>>(amax, scal, hdr, B, T);
+  return launch_check("k_scale");
+}
+
+// ---- the tape's header and dropout ------------------------------------------------------------------------------------
+__global__ void k_tape_hdr(Fs2TapeHdr* h, uint64_t seed, float p, int B, int T) {
+  h->seed = seed;
+  h->p = p;
+  h->B = B;
+  h->T = T;
+}
+
+// the dropout of site `site` as the tape's forward drew it
+__device__ __forceinline__ Fs2Drop hdr_drop(const Fs2TapeHdr* h, int site) { return make_drop(h->seed, h->p, site); }
+
+// out[f][c] = 1 where dropout d keeps element (f, c) of [F][n], else 0
+__global__ void k_drop_masks(Fs2Drop d, size_t F, int n, uint8_t* out) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < F * n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    out[i] = dropout_scale(d, i / n, static_cast<int>(i % n)) != 0.f;
+}
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
 }
 
 // ---- step-embedding MLP backward (mlp.0 -> Mish -> mlp.2 of C = residual_channels), from the saves of k_embed_table
@@ -200,17 +284,42 @@ int wgrad_fchunk(int F, int tiles, int device) {
   return ((fch + sp - 1) / sp) * 64;
 }
 
-// partials of D[am x ntiles*256] = A^T B over F frames, one [Mpad][Ntot] slab per split
-int run_wgrad(WgradArgs a, int ntiles, int device, float* part, float* bpart, cudaStream_t s) {
+// floats of the largest partial buffer (weights, then bias) among wgrads over F frames of these (m tiles, n tiles)
+size_t wgrad_part_floats(int F, const std::vector<std::pair<int, int>>& shapes, int device) {
+  size_t worst = 0;
+  for (const auto& [mt, nt] : shapes) {
+    const int fchunk = wgrad_fchunk(F, mt * nt, device);
+    const size_t sp = (F + fchunk - 1) / fchunk;
+    worst = std::max(worst, sp * mt * 64 * nt * 256 + sp * mt * 64);
+  }
+  return worst;
+}
+
+// D[am x ntiles*256] = A^T B over a.F frames (a's operands and tiles set) into o, scaled by scal[1] as o says: k_wgrad's
+// split partials in part (wgrad_part_floats), then k_wgrad_sum
+int run_wgrad(WgradArgs a, int ntiles, const WgradDst& o, float* part, const float* scal, int device, cudaStream_t s) {
   const int mtiles = (a.am + 63) / 64;
   a.fchunk = wgrad_fchunk(a.F, mtiles * ntiles, device);
   const int sp = (a.F + a.fchunk - 1) / a.fchunk;
   a.part = part;
-  a.bpart = bpart;
   a.Mpad = mtiles * 64;
   a.Ntot = ntiles * 256;
+  a.bpart = o.db ? part + static_cast<size_t>(sp) * a.Mpad * a.Ntot : nullptr;   // the bias partials follow the weights'
   k_wgrad<<<dim3(mtiles, ntiles, sp), kWgThreads, kWgSmem, s>>>(a);
-  return launch_check("k_wgrad");
+  DSX_TRY(launch_check("k_wgrad"));
+  WgradSumArgs r{};
+  r.part = part;
+  r.bpart = a.bpart;
+  r.splits = sp;
+  r.Mpad = a.Mpad;
+  r.Ntot = a.Ntot;
+  r.am = a.am;
+  for (int j = 0; j < ntiles; ++j) r.ncol += (r.bn[j] = a.bn[j]);
+  r.o = o;
+  r.scal = scal;
+  const size_t total = static_cast<size_t>(a.am) * r.ncol;
+  k_wgrad_sum<<<static_cast<unsigned>(std::min<size_t>((total + 255) / 256, 4096)), 256, 0, s>>>(r);
+  return launch_check("k_wgrad_sum");
 }
 
 }  // namespace
