@@ -45,6 +45,7 @@ SYMBOLS = (
     "dsx_pitchpred_train_workspace_bytes", "dsx_pitchpred_train_forward", "dsx_pitchpred_train_backward",
     "dsx_pitchpred_train_masks",
     "dsx_pwg_create", "dsx_pwg_destroy", "dsx_pwg_load", "dsx_pwg_forward",
+    "dsx_ssim_forward", "dsx_ssim_backward",
 )
 _VOID = ("dsx_last_error", "dsx_destroy", "dsx_hifigan_destroy", "dsx_pe_destroy", "dsx_fs2dec_destroy",
          "dsx_fs2enc_destroy", "dsx_durpred_destroy", "dsx_train_destroy", "dsx_fs2dec_train_destroy",
@@ -291,6 +292,8 @@ lib.dsx_pwg_destroy.argtypes = [_vp]
 lib.dsx_pwg_destroy.restype = None
 lib.dsx_pwg_load.argtypes = [_vp, ctypes.POINTER(PwgParams), _vp]
 lib.dsx_pwg_forward.argtypes = [_vp, _vp, _vp, Strides, _vp, _i, _i, _vp, _vp]
+lib.dsx_ssim_forward.argtypes = [_vp, _vp, _i, _i, _i, _vp, _vp]
+lib.dsx_ssim_backward.argtypes = [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]
 for _n in SYMBOLS:
     if _n not in _VOID:
         getattr(lib, _n).restype = _i

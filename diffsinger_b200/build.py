@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = [os.path.join(HERE, "csrc", f) for f in ("dsx_api.cu", "dsx_simt.cu", "dsx_hopper.cu", "dsx_hifigan.cu", "dsx_pe.cu",
                                                 "dsx_fs2dec.cu", "dsx_fftdiff.cu", "dsx_fs2enc.cu", "dsx_train.cu",
                                                 "dsx_fs2train.cu", "dsx_ffttrain.cu", "dsx_fs2enctrain.cu", "dsx_durtrain.cu",
-                                                "dsx_pitchtrain.cu", "dsx_pwg.cu")]
+                                                "dsx_pitchtrain.cu", "dsx_pwg.cu", "dsx_ssim.cu")]
 HDR = [os.path.join(HERE, "csrc", f) for f in ("dsx_internal.h", "dsx_ptx.cuh", "dsx_rng.cuh", "dsx_conv.cuh",
                                                "dsx_posemb.cuh", "dsx_wgrad.cuh", "dsx_fftentry.cuh", "dsx_wnorm.cuh")] + \
       [os.path.join(os.path.dirname(HERE), "include", "dsx.h")]

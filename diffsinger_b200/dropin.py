@@ -65,6 +65,14 @@ PitchPredictor)`` included, whose ``Linear`` stays eager -- and its energy predi
 their sm_90a training steps.  ``modules.fastspeech.tts_modules`` and ``modules.fastspeech.pe`` keep the reference's
 classes, so the reference's ``PitchExtractor`` keeps its own predictor.  ``uninstall_fs2_predictors()`` restores
 whatever was swapped.
+
+    dropin.install_ssim()
+
+rebinds ``ssim`` in ``modules.commons.ssim`` -- and the name bound from it in ``tasks.*`` / ``usr.*`` modules already
+imported (tasks/tts/fs2.py binds it at import) -- to ``diffsinger_b200.ssim``, so ``FastSpeech2Task.ssim_loss`` and
+``cwt_loss`` run the SSIM loss, forward and backward, on dsx unchanged.  The ``l1`` half of ``mel_loss``, the
+nonzero-speech weights and the reference's ``SSIM`` module class stay eager.  ``uninstall_ssim()`` restores the
+reference's function.
 """
 import importlib
 import sys
@@ -376,3 +384,29 @@ def uninstall_fs2_predictors():
         if mod is not None:
             setattr(mod, attr, ref)
         del _fs2pred[(name, attr)]
+
+
+_ssim = {}
+
+
+def install_ssim():
+    from .ssim import ssim
+    mod = importlib.import_module("modules.commons.ssim")
+    if mod.ssim is not ssim:
+        _ssim["ref"] = mod.ssim
+    _swap_ssim(_ssim["ref"], ssim)
+    return ssim
+
+
+def uninstall_ssim():
+    if _ssim:
+        from .ssim import ssim
+        _swap_ssim(ssim, _ssim["ref"])
+
+
+def _swap_ssim(old, new):
+    for name, mod in list(sys.modules.items()):
+        if mod is None or not (name == "modules.commons.ssim" or name.startswith(("tasks.", "usr."))):
+            continue
+        if getattr(mod, "ssim", None) is old:
+            mod.ssim = new

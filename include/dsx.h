@@ -1010,6 +1010,24 @@ int dsx_fft_train_backward(dsx_fft_train* h, const dsx_fft_params* w, const void
                            const dsx_fft_params* grads, float* d_cond, int B, int T, void* workspace,
                            size_t workspace_bytes, void* stream);
 
+/* ---- SSIM mel loss ---------------------------------------------------------------------------------------------------
+ * Replaces: ssim(img1, img2, window_size=11) (modules/commons/ssim.py:319-391) -- _ssim's five 11 x 11 conv2d and the
+ * elementwise formula (:331-346) -- and its autograd backward, for one channel, as FastSpeech2Task.ssim_loss and
+ * cwt_loss (tasks/tts/fs2.py:166-175, 271-277) call it.  Stateless, on the current device, like dsx_length_*.
+ *
+ * x, y, map, d_map, d_x, d_y: contiguous fp32 [B, H, W] (the [B, 1, H, W] images without the channel).  The window is
+ * the outer product of the reference's float32 gaussian(11, 1.5), applied as two 11-tap passes with zero padding 5 in H
+ * and W; C1 = 0.01^2, C2 = 0.03^2.  fp32 on CUDA cores throughout (no TF32).  B >= 1, H >= 1 and 1 <= W <= 256, else
+ * DSX_E_INVALID.  One launch each; no workspace, atomics or handle.  Each image gives the same bits alone as in a
+ * batch, and repeated calls give the same bits.
+ *
+ * dsx_ssim_forward: map = the SSIM map (_ssim's ssim_map; size_average=False returns it as ssim_map.mean(1)).
+ * dsx_ssim_backward: d_x and d_y = the gradients of sum(d_map * map) with respect to x and y; either may be NULL (not
+ * computed; both NULL launches nothing).  It recomputes the forward's moments instead of reading saved ones. */
+int dsx_ssim_forward(const float* x, const float* y, int B, int H, int W, float* map, void* stream);
+int dsx_ssim_backward(const float* x, const float* y, const float* d_map, int B, int H, int W, float* d_x, float* d_y,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif
